@@ -1,4 +1,4 @@
-"""allegro_b200: a B200 (sm_100a)-native implementation of Allegro's per-edge equivariant
+"""allegro_b200: an H100 (sm_90a)-native implementation of Allegro's per-edge equivariant
 hot path behind the NequIP/Allegro model and operator API.  See DESIGN.md."""
 from . import data, o3, systems  # noqa: F401
 

@@ -222,7 +222,7 @@ def linear(
     a_aux: Optional[Sequence[Optional[torch.Tensor]]] = None,
 ):
     """Out (+)= epi(act(cat(a_segs, -1)) @ W); a_segs / o_segs are 2-D row-strided views.
-    ``W_packed`` (from ``linear_pack``) enables the tcgen05 tensor-core path."""
+    ``W_packed`` (from ``linear_pack``) enables the wgmma tensor-core path."""
     M = a_segs[0].shape[0]
     K, N = W.shape
     dt = W.dtype

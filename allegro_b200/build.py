@@ -1,8 +1,8 @@
-"""Build liballegro_b200.so in-tree with nvcc for sm_100a (no torch types, plain C ABI).
+"""Build liballegro_b200.so in-tree with nvcc for sm_90a (no torch types, plain C ABI).
 
     python -m allegro_b200.build [--force] [--verbose]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so and its object files are build products (git-ignored); build() rebuilds whenever a source or flag changes.
 """
 from __future__ import annotations
 
@@ -20,7 +20,7 @@ LIB = os.path.join(LIBDIR, "liballegro_b200.so")
 STAMP = os.path.join(LIBDIR, "build.stamp")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -84,7 +84,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     # export only the extern "C" ab2_* symbols
     # link into a temporary name and move it into place: a failed link must not take the previous library with it
     tmp = LIB + ".tmp"
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", tmp] + objs
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", tmp] + objs
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout)

@@ -1,4 +1,4 @@
-// Shared helpers for the allegro_b200 kernels (sm_100a only).
+// Shared helpers for the allegro_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -121,6 +121,9 @@ __device__ __forceinline__ T dsilu_f(T x) {
 
 // irrep (l) of SH component j: floor(sqrt(j)) for j < 25
 __host__ __device__ __forceinline__ int sh_l_of(int j) { return (j >= 16) ? 4 : (j >= 9) ? 3 : (j >= 4) ? 2 : (j >= 1) ? 1 : 0; }
+
+// a * b + c per component (two FFMA on sm_90: Hopper has no paired FP32 FMA)
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
 template <typename T>
 __device__ __forceinline__ T warp_sum(T v) {

@@ -192,7 +192,7 @@ extern "C" int ab2_env_bwd(int dtype, int lmax, int64_t N, int64_t E, int U, con
         return 0;
     }
     if (g_ab2_opt_tp_fast && row_ptr && lmax <= 3) {
-        // auto (0): split only when a centre needs several channel chunks (U = 64: 500 -> 345 us; U = 32: no gain)
+        // auto (0): split only when a centre needs several channel chunks (U > 32)
         const int opt = g_ab2_opt_env_split ? g_ab2_opt_env_split : (U > 32 && dtype != AB2_F64 ? 4 : 1);
         const int split = opt >= 4 ? 4 : opt >= 2 ? 2 : 1;
         const int64_t warps = N * ((U + 31) / 32) * split;

@@ -53,7 +53,7 @@ extern "C" int ab2_device_ok(void) {
     if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return 0; }
     cudaDeviceProp p;
     if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) { cudaGetLastError(); return 0; }
-    return p.major == 10 ? 1 : 0;
+    return (p.major == 9 && p.minor == 0) ? 1 : 0;
 }
 
 // ---------------------------------------------------------------------------------------

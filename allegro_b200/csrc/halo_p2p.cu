@@ -3,8 +3,8 @@
 // Spatial decomposition (SURVEY section 8e): per force evaluation a rank sends the positions of its boundary atoms to
 // the two neighbouring slabs (forward halo), receives the gradients accumulated on its ghosts' owners' behalf back
 // (reverse halo), and all ranks sum one scalar energy.  Messages are tens of KB, so the cost is latency: through
-// torch.distributed / NCCL point-to-point the three exchanges cost ~170 us of a ~3 ms step inside the CUDA graph
-// (pack / unpack torch kernels + NCCL kernels).  Here every rank owns a small MAILBOX allocation that its peers map
+// torch.distributed / NCCL point-to-point the three exchanges add pack / unpack torch kernels and NCCL kernels to every
+// step inside the CUDA graph.  Here every rank owns a small MAILBOX allocation that its peers map
 // through CUDA IPC; the sender's kernel gathers the rows and STORES them straight into the receiver's mailbox over
 // NVLink, then publishes the step number with a system-scope release store; the receiver's kernel spins on that flag
 // (acquire) and unpacks.  Everything is ordinary kernels, so the whole step -- halo included -- stays one CUDA graph.

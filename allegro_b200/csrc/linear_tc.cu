@@ -1,23 +1,24 @@
-// tcgen05 (5th-gen tensor core) path of the fused linear layer -- same contract as linear.cu:
+// wgmma (Hopper warpgroup tensor core) path of the fused linear layer -- same contract as linear.cu:
 //
 //   Out[M][N] (+)= epi( act([A_0 | A_1 | ...])[M][K] @ W[K][N] )
 //
-// M = number of edges (10^5..10^8), K,N <= 256: a tall-skinny GEMM that is HBM-bound once the
-// MACs run on tensor cores (12-25 KFLOP per ~0.5-1 KB row).  Structure (one persistent CTA per
-// SM, 13 warps, warp-specialised, all hand-written PTX):
+// M = number of edges (10^5..10^8), K <= 512, N <= 128 per launch (wider outputs run as column
+// slices): a tall-skinny GEMM that is HBM-bound once the MACs run on tensor cores (12-25 KFLOP per
+// ~0.5-1 KB row).  Structure (one persistent CTA per SM, 16 warps, warp-specialised, hand-written PTX):
 //
 //   warps 0-7  producers : coalesced global loads of the concatenated A row segments
 //                          (8 rows x 128 B per warp instruction), optional SiLU, split of the fp32
 //                          value into bf16 hi + bf16 lo, 16-byte st.shared into a ring of
-//                          128-row x 32-k stages in the UMMA canonical K-major (no-swizzle,
+//                          128-row x 32-k stages in the GMMA canonical K-major (no-swizzle,
 //                          8x16B core matrix) layout; fence.proxy.async + mbarrier arrive.
-//   warp  8    MMA       : one elected lane issues tcgen05.mma.cta_group::1.kind::f16
-//                          (M=128, N<=256, K=16) from shared-memory descriptors into one of two
-//                          TMEM accumulators; fp32 storage uses the 3-term split
-//                          A_hi W_hi + A_lo W_hi + A_hi W_lo (~2^-16 relative, fp32 accumulate);
-//                          tcgen05.commit releases ring slots / publishes the accumulator.
-//   warps 9-12 epilogue  : tcgen05.ld 32x32b (lane = row), silu' / accumulate epilogue, split
-//                          into the output column segments, vectorised global stores.
+//   warps 8-15 consumers : two warpgroups, one per 64-row half of the tile.  Each issues
+//                          wgmma.mma_async m64nNk16 (N = Npad <= 128) from shared-memory descriptors
+//                          into register accumulators; fp32 storage uses the 3-term split
+//                          A_hi W_hi + A_lo W_hi + A_hi W_lo (~2^-16 relative, fp32 accumulate).
+//                          A ring slot is released once the wgmma group that read it has retired.
+//                          The epilogue runs from the accumulator registers: staged per warp through
+//                          shared memory, silu' / accumulate, split into the output column segments,
+//                          vectorised global stores.
 //
 // W (all of it: <= 128 KB as bf16 hi+lo) is staged once per CTA from a pre-packed image
 // (ab2_linear_pack) and stays resident in shared memory.
@@ -31,23 +32,23 @@ extern int g_ab2_opt_tc_debug;  // bit0: no epilogue global stores, bit1: no pro
 
 namespace {
 
-constexpr int BM = 128;       // rows per tile = UMMA M
+constexpr int BM = 128;       // rows per tile = 2 consumer warpgroups x wgmma M (64)
 constexpr int KC = 32;        // k per ring stage
 constexpr int NSTAGE = 4;        // max ring stages (run-time count p.nstage <= NSTAGE)
-constexpr int RAW_DEPTH = 4;     // max cp.async stages in flight per producer thread
 constexpr int RAW_STAGE = 256 * 4 * 16;  // bytes: 256 producer threads x 4 x 16-byte chunks (x2 with aux)
-constexpr int EPI_LD = 36;       // floats per staged row (32 + 4 pad): conflict-free 16-byte accesses
-constexpr int EPI_BYTES = 4 * 32 * EPI_LD * 4;  // 4 epilogue warps x 32 rows
-constexpr int PF_BYTES = 2 * EPI_BYTES;         // 2 prefetch buffers per epilogue warp (aux / old tiles)
+constexpr int EPI_LD = 40;       // floats per staged row (32 + 8 pad): conflict-free float2 writes / float4 reads
+constexpr int NCONS = 8;         // consumer warps (2 warpgroups)
+constexpr int EPI_BYTES = NCONS * 16 * EPI_LD * 4;  // 16 rows x 32 columns per consumer warp
 constexpr int STAGE_HALF = BM * KC * 2;  // bytes of one bf16 [128][32] operand image (8 KB)
 constexpr int NPROD = 8;                       // producer warps
-constexpr int NTHREADS = (NPROD + 1 + 4) * 32;  // producers + MMA issuer + epilogue
+constexpr int NTHREADS = (NPROD + NCONS) * 32;  // producers + consumers
 constexpr int MAX_W_BYTES = 128 * 1024;
 constexpr int MAX_K = 512;                     // k-chunk table size (MAX_K / 8 entries)
-constexpr int MAX_CHUNK = 8;                   // 32-column output chunks (Npad <= 256)
-// tail of the shared-memory plan: barriers | TMEM base word | output chunk table | A / aux k-chunk tables
-constexpr int TAIL_BARS = 96, TAIL_SLOT = 16, TAIL_CHUNK = MAX_CHUNK * 32, TAIL_KMAP = (MAX_K / 8) * 16;
-constexpr int TAIL_BYTES = TAIL_BARS + TAIL_SLOT + TAIL_CHUNK + 2 * TAIL_KMAP;
+constexpr int MAX_N = 128;                     // columns per launch: wgmma N <= 128 keeps the accumulator at 64 registers
+constexpr int MAX_CHUNK = MAX_N / 32;          // 32-column output chunks
+// tail of the shared-memory plan: barriers | output chunk table | A / aux k-chunk tables
+constexpr int TAIL_BARS = 2 * NSTAGE * 8, TAIL_CHUNK = MAX_CHUNK * 32, TAIL_KMAP = (MAX_K / 8) * 16;
+constexpr int TAIL_BYTES = TAIL_BARS + TAIL_CHUNK + 2 * TAIL_KMAP;
 
 struct TcSeg {
     const void* ptr;
@@ -74,15 +75,13 @@ struct TcParams {
     int64_t num_tiles;
     int nstage;
     int debug;
-    int pf_mode;    // epilogue prefetch: 0 none, 1 aux (silu' epilogue), 2 old values (accumulate)
     int raw_depth;  // cp.async stages in flight per producer thread (2 or 4)
     int has_aux;    // act == AB2_ACT_MUL_DSILU: the raw slots carry A and aux chunks
 };
 
 // Address tables built once per CTA so that the per-item / per-chunk code of the producer and
 // epilogue warps is a shared-memory lookup plus 32-bit offsets.  (Walking the segment list and doing
-// 64-bit index arithmetic per access made both warp groups instruction-latency bound: ~1 us per
-// 32x32 output chunk on a single warp, a third of the HBM write rate.)
+// 64-bit index arithmetic per access makes both warp groups instruction-latency bound.)
 struct KEnt {        // source of concat columns [8e, 8e+8): pointer to (row 0, that column), row stride
     const void* ptr; // null: beyond K (or, in the aux table, a segment without silu' multiplier)
     int64_t ld;      // elements
@@ -105,11 +104,6 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// arrive without release ordering of this thread's earlier global stores (the consumer only needs
-// the tcgen05 / shared-memory effects, which are ordered by the explicit fences)
-__device__ __forceinline__ void mbar_arrive_relaxed(uint32_t bar) {
-    asm volatile("mbarrier.arrive.relaxed.cta.shared::cta.b64 _, [%0];" ::"r"(bar));
-}
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     asm volatile(
         "{\n\t"
@@ -125,47 +119,43 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// ---- wgmma (sm_90a) ----
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64][32*NCH] (+)= A[smem desc] * B[smem desc]^T, bf16 inputs, both K-major, fp32 accumulate in registers.
+// Accumulator fragment of thread (warp w of the warpgroup, lane l): d[4j + {0,1}] = row 16w + l/4,
+// columns 8j + 2(l%4) + {0,1}; d[4j + {2,3}] = the same columns of row 16w + l/4 + 8.
+template <int NCH>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[16 * NCH], uint64_t da, uint64_t db, uint32_t scale_d) {
+    if constexpr (NCH == 1) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(da), "l"(db), "r"(scale_d));
+    } else if constexpr (NCH == 2) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(da), "l"(db), "r"(scale_d));
+    } else if constexpr (NCH == 3) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+            : "l"(da), "l"(db), "r"(scale_d));
+    } else if constexpr (NCH == 4) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(da), "l"(db), "r"(scale_d));
+    }
+
 }
 
 __device__ __forceinline__ void cp_async16(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
@@ -216,7 +206,7 @@ __device__ __forceinline__ const TSrc* seg_aux_ptr(const TcParams& p, int64_t m,
     return nullptr;
 }
 
-// shared-memory matrix descriptor: K-major, SWIZZLE_NONE, 8x16B core matrices.
+// wgmma shared-memory matrix descriptor: K-major, no swizzle (interleave), 8x16B core matrices.
 // canonical layout (16-byte units) ((8,n),2):((1,SBO),LBO): LBO = byte distance between core
 // matrices adjacent in K, SBO = between 8-row groups.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
@@ -224,8 +214,7 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-    return d;                // base_offset = 0, lbo_mode = 0, layout_type = 0 (SWIZZLE_NONE)
+    return d;  // base_offset = 0, layout_type = 0 (no swizzle)
 }
 
 // branch-free SiLU and SiLU' (MUFU ex2 / rcp, ~2 ulp): IEEE division has a slow-path branch that
@@ -305,120 +294,74 @@ struct TcCtx {
     uint8_t* sW;
     uint8_t* sA;
     float* sEpi;
-    float* sPf;
     ChunkInfo* sChunk;
-    uint32_t bar0;       // full[NSTAGE], empty[NSTAGE], tmem_full[2], tmem_empty[2]
-    uint32_t tmem_base;
+    uint32_t bar0;       // full[NSTAGE], empty[NSTAGE]
     int nkb, stage_bytes, w_half;
-    uint32_t idesc;
     __device__ __forceinline__ uint32_t full_bar(int s) const { return bar0 + 8u * s; }
     __device__ __forceinline__ uint32_t empty_bar(int s) const { return bar0 + 8u * (NSTAGE + s); }
-    __device__ __forceinline__ uint32_t tfull_bar(int a) const { return bar0 + 8u * (2 * NSTAGE + a); }
-    __device__ __forceinline__ uint32_t tempty_bar(int a) const { return bar0 + 8u * (2 * NSTAGE + 2 + a); }
 };
 
-// =============================== MMA issuer (one warp, one elected lane) ===============================
-template <bool SPLIT>
-__device__ __forceinline__ void tc_mma_role(const TcParams& p, const TcCtx& c, int lane) {
+// =============================== consumers (2 warpgroups: wgmma + epilogue) ===============================
+// cw: consumer warp 0..7; warpgroup cw / 4 owns rows [64 (cw / 4), 64 (cw / 4) + 64) of each tile, warp cw % 4 of it
+// holds the accumulator rows [16 (cw % 4), 16 (cw % 4) + 16) of that half.
+template <typename TSrc, bool SPLIT, int NCH>
+__device__ __forceinline__ void tc_consumer_role(const TcParams& p, const TcCtx& c, int cw, int lane) {
+    const int wg = cw >> 2, w4 = cw & 3;
     const int nkb = c.nkb, stage_bytes = c.stage_bytes, w_half = c.w_half;
-    const uint32_t tmem_base = c.tmem_base, idesc = c.idesc;
-    uint8_t* sW = c.sW;
-    uint8_t* sA = c.sA;
-    auto full_bar = [&](int s) { return c.full_bar(s); };
-    auto empty_bar = [&](int s) { return c.empty_bar(s); };
-    auto tfull_bar = [&](int a) { return c.tfull_bar(a); };
-    auto tempty_bar = [&](int a) { return c.tempty_bar(a); };
+    const uint32_t sW_u = smem_u32(c.sW);
+    const uint32_t w_sbo = (uint32_t)(p.K / 8) * 128;  // bytes between 8-column (n) groups of W
+    constexpr uint32_t A_SBO = (KC / 8) * 128;         // bytes between 8-row groups of a stage
+    float* stg = c.sEpi + cw * 16 * EPI_LD;
     int stage = 0;
     uint32_t phase = 0;
-    int64_t it = 0;
-    const uint32_t sW_u = smem_u32(sW);
-    const uint32_t w_sbo = (uint32_t)(p.K / 8) * 128;  // bytes between 8-column (n) groups of W
-    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-        const int a = (int)(it & 1);
-        const uint32_t aphase = (uint32_t)((it >> 1) & 1);
-        mbar_wait(tempty_bar(a), aphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(a * 256);
+    float acc[16 * NCH];
+    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        int prev = -1;
         for (int kb = 0; kb < nkb; ++kb) {
-            mbar_wait(full_bar(stage), phase);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t a_hi = smem_u32(sA + stage * stage_bytes);
-                const int ksteps = min(2, (p.K - kb * KC) / 16);
-                for (int ks = 0; ks < ((p.debug & 4) ? 0 : ksteps); ++ks) {
-                    const uint64_t da_hi = make_desc(a_hi + ks * 256, 128, (KC / 8) * 128);
-                    const uint32_t wk = sW_u + (uint32_t)(kb * (KC / 8) + ks * 2) * 128;
-                    const uint64_t db_hi = make_desc(wk, 128, w_sbo);
-                    umma_bf16(d_tmem, da_hi, db_hi, idesc, (kb | ks) ? 1u : 0u);
-                    if constexpr (SPLIT) {
-                        const uint64_t da_lo = make_desc(a_hi + STAGE_HALF + ks * 256, 128, (KC / 8) * 128);
-                        const uint64_t db_lo = make_desc(wk + w_half, 128, w_sbo);
-                        umma_bf16(d_tmem, da_lo, db_hi, idesc, 1u);
-                        umma_bf16(d_tmem, da_hi, db_lo, idesc, 1u);
-                    }
+            mbar_wait(c.full_bar(stage), phase);
+            wgmma_fence();
+            const uint32_t a_hi = smem_u32(c.sA + stage * stage_bytes) + (uint32_t)wg * 8 * A_SBO;
+            const int ksteps = min(2, (p.K - kb * KC) / 16);
+            for (int ks = 0; ks < ((p.debug & 4) ? 0 : ksteps); ++ks) {
+                const uint64_t da_hi = make_desc(a_hi + ks * 256, 128, A_SBO);
+                const uint32_t wk = sW_u + (uint32_t)(kb * (KC / 8) + ks * 2) * 128;
+                const uint64_t db_hi = make_desc(wk, 128, w_sbo);
+                wgmma_bf16<NCH>(acc, da_hi, db_hi, (kb | ks) ? 1u : 0u);
+                if constexpr (SPLIT) {
+                    const uint64_t da_lo = make_desc(a_hi + STAGE_HALF + ks * 256, 128, A_SBO);
+                    const uint64_t db_lo = make_desc(wk + w_half, 128, w_sbo);
+                    wgmma_bf16<NCH>(acc, da_lo, db_hi, 1u);
+                    wgmma_bf16<NCH>(acc, da_hi, db_lo, 1u);
                 }
-                umma_commit(empty_bar(stage));                  // ring slot free once these MMAs retire
-                if (kb == nkb - 1) umma_commit(tfull_bar(a));   // accumulator complete
             }
-            __syncwarp();
+            wgmma_commit();
+            // the group of the previous k block has retired: its ring slot is free (this one stays in flight)
+            if (prev >= 0) {
+                wgmma_wait<1>();
+                if (lane == 0) mbar_arrive(c.empty_bar(prev));
+            }
+            prev = stage;
             if (++stage == p.nstage) { stage = 0; phase ^= 1; }
         }
-    }
-}
+        wgmma_wait<0>();
+        if (lane == 0 && prev >= 0) mbar_arrive(c.empty_bar(prev));
+        if (p.debug & 4) {
+#pragma unroll
+            for (int j = 0; j < 16 * NCH; ++j) acc[j] = 0.f;
+        }
 
-// =============================== epilogue (4 warps, one TMEM lane quadrant each) ===============================
-template <typename TSrc, int PF>
-__device__ __forceinline__ void tc_epilogue_role(const TcParams& p, const TcCtx& c, int warp, int lane) {
-    const uint32_t tmem_base = c.tmem_base;
-    float* sEpi = c.sEpi;
-    float* sPf = c.sPf;
-    ChunkInfo* sChunk = c.sChunk;
-    auto tfull_bar = [&](int a) { return c.tfull_bar(a); };
-    auto tempty_bar = [&](int a) { return c.tempty_bar(a); };
-    const int q = warp & 3;  // TMEM lane quadrant this warp may access
-    int64_t it = 0;
-    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-        const int a = (int)(it & 1);
-        const uint32_t aphase = (uint32_t)((it >> 1) & 1);
-        // ---- epilogue-side global reads (silu' aux or old values to accumulate) are prefetched with
-        //      cp.async into per-warp buffers, two 32-column chunks ahead, starting BEFORE the
-        //      accumulator is ready ----
-        const int64_t m_base = tile * BM + q * 32;
-        const int64_t left64 = p.M - m_base;  // <= 0: this warp's 32 rows lie beyond M
-        const int rows_left = left64 >= 32 ? 32 : (left64 > 0 ? (int)left64 : 0);
-        const bool full = rows_left == 32;
+        // ---- epilogue: this warp's 16 rows, one 32-column chunk at a time ----
+        const int64_t m_base = tile * BM + wg * 64 + w4 * 16;
+        const int64_t left64 = p.M - m_base;  // <= 0: this warp's rows lie beyond M
+        const int rows_left = left64 >= 16 ? 16 : (left64 > 0 ? (int)left64 : 0);
         const int rsub = lane >> 3, c4 = lane & 7;
         // row handled in slot itr: itr*4 + rsub; loads of a partial tile read a clamped (valid) row
-        auto row_of = [&](int itr) { const int r = itr * 4 + rsub; return full ? r : (r < rows_left ? r : rows_left - 1); };
-        float* pfw = sPf + q * 2 * 32 * EPI_LD;
-        auto prefetch = [&](int c0) {
-            if constexpr (PF == 0) return;
-            if (c0 < p.Npad && rows_left > 0) {
-                const ChunkInfo ci = sChunk[c0 >> 5];
-                if (ci.ok && (PF == 1 || ci.accum)) {
-                    const int64_t gld = (PF == 1) ? p.aux_ld : ci.ld;
-                    const float* tb = ((PF == 1) ? ci.aptr : (const float*)ci.optr) + m_base * gld + c4 * 4;
-                    const uint32_t gl = (uint32_t)gld;
-                    float* dstb = pfw + ((c0 >> 5) & 1) * 32 * EPI_LD + c4 * 4;
-#pragma unroll
-                    for (int itr = 0; itr < 8; ++itr)
-                        cp_async16(smem_u32(dstb + (itr * 4 + rsub) * EPI_LD), tb + (uint32_t)row_of(itr) * gl, 16u);
-                }
-            }
-            cp_async_commit();
-        };
-        prefetch(0);
-        prefetch(32);
-        mbar_wait(tfull_bar(a), aphase);
-        tc_fence_after();
-        const int64_t m = tile * BM + q * 32 + lane;
-        const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * 256);
-        // two 16-column TMEM loads in flight, then the epilogue of both
-        auto process = [&](int c0, const uint32_t (&r)[16]) {
-            if (m >= p.M) return;
+        auto row_of = [&](int itr) { const int r = itr * 4 + rsub; return r < rows_left ? r : rows_left - 1; };
+        // generic path: 16 consecutive columns [c0, c0 + 16) of row m
+        auto process = [&](int64_t m, int c0, const float (&vin)[16]) {
             float v[16];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
+            for (int j = 0; j < 16; ++j) v[j] = vin[j];
             if (p.epi == AB2_EPI_MUL_DSILU) {
                 const TSrc* ax = (const TSrc*)p.aux + m * p.aux_ld + c0;
                 if (sizeof(TSrc) == 4 && c0 + 16 <= p.N && ((reinterpret_cast<uintptr_t>(ax) & 15) == 0)) {
@@ -471,90 +414,77 @@ __device__ __forceinline__ void tc_epilogue_role(const TcParams& p, const TcCtx&
                 }
             }
         };
-        float* stg = sEpi + q * 32 * EPI_LD;
-        for (int c0 = 0; c0 < p.Npad; c0 += 32) {
-            uint32_t r0[16], r1[16];
-            const bool two = c0 + 16 < p.Npad;
-            tmem_ld16_nowait(t_row + c0, r0);
-            if (two) tmem_ld16_nowait(t_row + c0 + 16, r1);
-            tmem_ld_wait();
-            const ChunkInfo ci = sChunk[c0 >> 5];
-            if constexpr (PF != 0) cp_async_wait<1>();  // this chunk's prefetch group (if any) has landed
+#pragma unroll
+        for (int ch = 0; ch < NCH; ++ch) {
+            const int c0 = ch * 32;
+            // accumulator fragment -> staging rows (row = lane / 4 and lane / 4 + 8)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int col = 8 * j + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(stg + (lane >> 2) * EPI_LD + col) = make_float2(acc[16 * ch + 4 * j], acc[16 * ch + 4 * j + 1]);
+                *reinterpret_cast<float2*>(stg + ((lane >> 2) + 8) * EPI_LD + col) = make_float2(acc[16 * ch + 4 * j + 2], acc[16 * ch + 4 * j + 3]);
+            }
+            __syncwarp();
+            const ChunkInfo ci = c.sChunk[ch];
             if ((p.debug & 1) || rows_left == 0) {
             } else if (ci.ok) {
-                // coalesced path (ok implies two): stage my row (lane): 32 floats -> shared, then every
-                // global access covers 4 rows x 128 B
-                float4* srow = reinterpret_cast<float4*>(stg + lane * EPI_LD);
+                // coalesced path: every global access covers 4 rows x 128 B.
+                // 1) shared-memory reads, 2) (uniform) epilogue variants with all global loads issued before use,
+                // 3) stores: tile base pointer + 32-bit row offsets.
+                float4 x[4];
 #pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                    srow[t] = make_float4(__uint_as_float(r0[4 * t]), __uint_as_float(r0[4 * t + 1]), __uint_as_float(r0[4 * t + 2]), __uint_as_float(r0[4 * t + 3]));
-                    srow[4 + t] = make_float4(__uint_as_float(r1[4 * t]), __uint_as_float(r1[4 * t + 1]), __uint_as_float(r1[4 * t + 2]), __uint_as_float(r1[4 * t + 3]));
-                }
-                __syncwarp();
-                // 1) all shared-memory reads, 2) (uniform) epilogue variants with all global loads
-                //    issued before use, 3) stores: tile base pointer + 32-bit row offsets.
-                float4 x[8];
-#pragma unroll
-                for (int itr = 0; itr < 8; ++itr) x[itr] = *reinterpret_cast<const float4*>(stg + (itr * 4 + rsub) * EPI_LD + c4 * 4);
+                for (int itr = 0; itr < 4; ++itr) x[itr] = *reinterpret_cast<const float4*>(stg + (itr * 4 + rsub) * EPI_LD + c4 * 4);
                 float* tb = ci.optr + m_base * ci.ld + c4 * 4;
                 const uint32_t ol = (uint32_t)ci.ld;
-                uint32_t off[8];
+                uint32_t off[4];
 #pragma unroll
-                for (int itr = 0; itr < 8; ++itr) off[itr] = (uint32_t)row_of(itr) * ol;
-                const float* pfb = pfw + ((c0 >> 5) & 1) * 32 * EPI_LD;
+                for (int itr = 0; itr < 4; ++itr) off[itr] = (uint32_t)row_of(itr) * ol;
                 if (p.epi == AB2_EPI_MUL_DSILU) {
-                    float4 ax[8];
+                    float4 ax[4];
                     const float* ab = ci.aptr + m_base * p.aux_ld + c4 * 4;
                     const uint32_t al = (uint32_t)p.aux_ld;
 #pragma unroll
-                    for (int itr = 0; itr < 8; ++itr)
-                        ax[itr] = (PF == 1) ? *reinterpret_cast<const float4*>(pfb + (itr * 4 + rsub) * EPI_LD + c4 * 4)
-                                                   : ldg128_nc(ab + (uint32_t)row_of(itr) * al);
+                    for (int itr = 0; itr < 4; ++itr) ax[itr] = ldg128_nc(ab + (uint32_t)row_of(itr) * al);
 #pragma unroll
-                    for (int itr = 0; itr < 8; ++itr) {
+                    for (int itr = 0; itr < 4; ++itr) {
                         x[itr].x *= dsilu_fast(ax[itr].x); x[itr].y *= dsilu_fast(ax[itr].y);
                         x[itr].z *= dsilu_fast(ax[itr].z); x[itr].w *= dsilu_fast(ax[itr].w);
                     }
                 }
                 if (ci.accum) {
-                    float4 old[8];
+                    float4 old[4];
 #pragma unroll
-                    for (int itr = 0; itr < 8; ++itr)
-                        old[itr] = (PF == 2) ? *reinterpret_cast<const float4*>(pfb + (itr * 4 + rsub) * EPI_LD + c4 * 4)
-                                                    : ldg128(tb + off[itr]);
+                    for (int itr = 0; itr < 4; ++itr) old[itr] = ldg128(tb + off[itr]);
 #pragma unroll
-                    for (int itr = 0; itr < 8; ++itr) {
+                    for (int itr = 0; itr < 4; ++itr) {
                         x[itr].x += old[itr].x; x[itr].y += old[itr].y; x[itr].z += old[itr].z; x[itr].w += old[itr].w;
                     }
                 }
-                if (full) {
 #pragma unroll
-                    for (int itr = 0; itr < 8; ++itr) stg128(tb + off[itr], x[itr]);
-                } else {
-#pragma unroll
-                    for (int itr = 0; itr < 8; ++itr)
-                        if (itr * 4 + rsub < rows_left) stg128(tb + off[itr], x[itr]);
-                }
-                __syncwarp();
+                for (int itr = 0; itr < 4; ++itr)
+                    if (itr * 4 + rsub < rows_left) stg128(tb + off[itr], x[itr]);
             } else {
-                process(c0, r0);
-                if (two) process(c0 + 16, r1);
+                // generic path: lane -> (row lane % 16, columns c0 + 16 (lane / 16) .. + 16)
+                const int r = lane & 15, h = lane >> 4;
+                if (r < rows_left && c0 + 16 * h < p.N) {
+                    float v[16];
+#pragma unroll
+                    for (int t = 0; t < 4; ++t) {
+                        const float4 q = *reinterpret_cast<const float4*>(stg + r * EPI_LD + 16 * h + 4 * t);
+                        v[4 * t] = q.x; v[4 * t + 1] = q.y; v[4 * t + 2] = q.z; v[4 * t + 3] = q.w;
+                    }
+                    process(m_base + r, c0 + 16 * h, v);
+                }
             }
-            if constexpr (PF != 0) {
-                __syncwarp();
-                prefetch(c0 + 64);  // refill the buffer just consumed (always commits a group)
-            }
+            __syncwarp();  // staging buffer is rewritten by the next chunk
         }
-        tc_fence_before();
-        if (p.debug & 8) mbar_arrive(tempty_bar(a));
-        else mbar_arrive_relaxed(tempty_bar(a));
     }
 }
 
-template <typename TSrc, bool SPLIT, int PF>
+template <typename TSrc, bool SPLIT, int NCH>
 __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const TcParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;  // warp-uniform role index
     const int w_half = p.Npad * p.K * 2;                     // bytes of one W image
     const int w_bytes = SPLIT ? 2 * w_half : w_half;
     uint8_t* sW = smem;
@@ -563,33 +493,22 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const TcParams p
     uint8_t* sRaw = sA + p.nstage * stage_bytes;
     const int raw_stage = RAW_STAGE * (p.has_aux ? 2 : 1);
     float* sEpi = reinterpret_cast<float*>(sRaw + p.raw_depth * raw_stage);
-    float* sPf = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sEpi) + EPI_BYTES);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sEpi) + EPI_BYTES + (PF ? PF_BYTES : 0));
-    // bars: full[NSTAGE], empty[NSTAGE], tmem_full[2], tmem_empty[2]; then the TMEM base word
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * NSTAGE + 4);
-    static_assert((2 * NSTAGE + 4) * 8 == TAIL_BARS, "barrier block size");
-    ChunkInfo* sChunk = reinterpret_cast<ChunkInfo*>(reinterpret_cast<uint8_t*>(bars) + TAIL_BARS + TAIL_SLOT);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sEpi) + EPI_BYTES);  // full[NSTAGE], empty[NSTAGE]
+    ChunkInfo* sChunk = reinterpret_cast<ChunkInfo*>(reinterpret_cast<uint8_t*>(bars) + TAIL_BARS);
     KEnt* sKmap = reinterpret_cast<KEnt*>(reinterpret_cast<uint8_t*>(sChunk) + TAIL_CHUNK);
     KEnt* sKaux = sKmap + MAX_K / 8;
     const uint32_t bar0 = smem_u32(bars);
     auto full_bar = [&](int s) { return bar0 + 8u * s; };
     auto empty_bar = [&](int s) { return bar0 + 8u * (NSTAGE + s); };
-    auto tfull_bar = [&](int a) { return bar0 + 8u * (2 * NSTAGE + a); };
-    auto tempty_bar = [&](int a) { return bar0 + 8u * (2 * NSTAGE + 2 + a); };
 
     // ---- one-time setup ----
     if (threadIdx.x == 0) {
         for (int s = 0; s < NSTAGE; ++s) {
             mbar_init(full_bar(s), NPROD * 32);
-            mbar_init(empty_bar(s), 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tfull_bar(a), 1);
-            mbar_init(tempty_bar(a), 128);
+            mbar_init(empty_bar(s), NCONS);  // one arrive per consumer warp once its wgmma reads of the slot retired
         }
         fence_barrier_init();
     }
-    if (warp == NPROD) tmem_alloc(smem_u32(tmem_slot), 512);
     if (threadIdx.x < MAX_K / 8) {
         // k-chunk tables: which A segment (and aux segment) holds concat columns [8e, 8e+8)
         const int e = threadIdx.x;
@@ -627,17 +546,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const TcParams p
             for (int e = threadIdx.x; e < w_half / 16; e += NTHREADS) dstl[e] = __ldg(srcl + e);
         }
     }
-    fence_proxy_async();  // W was written through the generic proxy, tcgen05.mma reads via the async proxy
-    tc_fence_before();
+    fence_proxy_async();  // W was written through the generic proxy, wgmma reads via the async proxy
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     const int nkb = (p.K + KC - 1) / KC;
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.Npad >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
     TcCtx ctx;
-    ctx.sW = sW; ctx.sA = sA; ctx.sEpi = sEpi; ctx.sPf = sPf; ctx.sChunk = sChunk; ctx.bar0 = bar0; ctx.tmem_base = tmem_base;
-    ctx.nkb = nkb; ctx.stage_bytes = stage_bytes; ctx.w_half = w_half; ctx.idesc = idesc;
+    ctx.sW = sW; ctx.sA = sA; ctx.sEpi = sEpi; ctx.sChunk = sChunk; ctx.bar0 = bar0;
+    ctx.nkb = nkb; ctx.stage_bytes = stage_bytes; ctx.w_half = w_half;
 
     if (warp < NPROD) {
         // =============================== producers ===============================
@@ -773,32 +688,26 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const TcParams p
             emit(v);
         }
         cp_async_wait<0>();
-    } else if (warp == NPROD) {
-        tc_mma_role<SPLIT>(p, ctx, lane);
     } else {
-        tc_epilogue_role<TSrc, PF>(p, ctx, warp, lane);
+        tc_consumer_role<TSrc, SPLIT, NCH>(p, ctx, warp - NPROD, lane);
     }
-    // ---- teardown ----
-    tc_fence_before();
-    __syncthreads();
-    if (warp == NPROD) tmem_dealloc(tmem_base, 512);
 }
 
 // =========================================================================================
 // TMA-producer variant (fp32 storage, every A segment a multiple of 32 columns wide).
 //
-//   warp 13      : one elected lane issues cp.async.bulk.tensor.2d loads (SASS UTMALDG) of 128-row x 32-column fp32
-//                  boxes (16 KB, SWIZZLE_128B) into a ring of NR raw slots, one box per k-chunk (+ one for the silu'
-//                  multiplier of that chunk), completing on an mbarrier; rows beyond M are zero-filled by the TMA unit.
-//   warps 0-7    : four converter GROUPS of two warps.  Group g owns the stages q = g (mod 4): it waits for the raw
-//                  slot, reads it conflict-free (the 128-byte swizzle puts the 8 rows of a core matrix in 8 different
-//                  bank groups), applies SiLU / silu'(aux), splits into bf16 hi + lo and writes the canonical K-major
-//                  stage.  Four stages are in conversion at once, so the fixed latency of one stage (mbarrier wait, LDS,
-//                  convert, STS, fence.proxy.async, arrive) no longer bounds the load rate: round 1's eight producer
-//                  warps all worked on the SAME stage and topped out at 2.3-3.2 TB/s on the load side.
-//   warp 8 / 9-12: MMA issuer and epilogue, unchanged (tc_mma_role / tc_epilogue_role).
+//   warps 0-7    : four converter GROUPS of two warps.  Group g owns the stages q = g (mod 4) and the raw slots that feed
+//                  them.  One elected lane of the group issues cp.async.bulk.tensor.2d loads (SASS UTMALDG) of 128-row x
+//                  32-column fp32 boxes (16 KB, SWIZZLE_128B) into its raw slots, one box per k-chunk (+ one for the
+//                  silu' multiplier of that chunk), completing on an mbarrier; rows beyond M are zero-filled by the TMA
+//                  unit.  The group waits for the raw slot, reads it conflict-free (the 128-byte swizzle puts the 8 rows
+//                  of a core matrix in 8 different bank groups), refills it NR sequence numbers ahead once all its warps
+//                  have drained it, applies SiLU / silu'(aux), splits into bf16 hi + lo and writes the canonical
+//                  K-major stage.  Four stages are in conversion at once, so the fixed latency of one stage (mbarrier
+//                  wait, LDS, convert, STS, fence.proxy.async, arrive) does not bound the load rate.  No separate TMA
+//                  warp: a 17th warp would cost the consumers their 128-register budget.
+//   warps 8-15   : consumers, unchanged (tc_consumer_role).
 // =========================================================================================
-constexpr int TMA_THREADS = NTHREADS + 32;
 constexpr int TMA_BOX_BYTES = BM * KC * 4;  // 16 KB
 
 struct alignas(64) TmaMaps {
@@ -819,14 +728,14 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 // (NR % G == 0 and nstage % G == 0, checked on the host): a group then never waits more than one mbarrier phase ahead
 // of its own slot.  (With slots shared between groups a group's first wait can be for the SECOND fill of a slot whose
 // first fill has not completed yet -- the parity wait returns immediately and the pipeline falls apart.)
-template <int PF, int G>
-__global__ void __launch_bounds__(TMA_THREADS, 1) linear_tma_kernel(const TcParams p, const __grid_constant__ TmaMaps maps, int NR) {
+template <int G, int NCH>
+__global__ void __launch_bounds__(NTHREADS, 1) linear_tma_kernel(const TcParams p, const __grid_constant__ TmaMaps maps, int NR) {
     constexpr int WPG = NPROD / G;      // warps per converter group
     constexpr int RGW = 16 / WPG;       // 8-row groups of a stage handled by one warp
     using TSrc = float;
     constexpr bool SPLIT = true;
     extern __shared__ __align__(1024) uint8_t smem[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;  // warp-uniform role index
     const int w_half = p.Npad * p.K * 2;
     const int w_bytes = 2 * w_half;
     const int stage_bytes = 2 * STAGE_HALF;
@@ -836,35 +745,24 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) linear_tma_kernel(const TcPara
     uint8_t* sW = sRaw + (size_t)NR * raw_slot;
     uint8_t* sA = sW + ((w_bytes + 127) & ~127);
     float* sEpi = reinterpret_cast<float*>(sA + p.nstage * stage_bytes);
-    float* sPf = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sEpi) + EPI_BYTES);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sEpi) + EPI_BYTES + (PF ? PF_BYTES : 0));
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * NSTAGE + 4);
-    ChunkInfo* sChunk = reinterpret_cast<ChunkInfo*>(reinterpret_cast<uint8_t*>(bars) + TAIL_BARS + TAIL_SLOT);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sEpi) + EPI_BYTES);
+    ChunkInfo* sChunk = reinterpret_cast<ChunkInfo*>(reinterpret_cast<uint8_t*>(bars) + TAIL_BARS);
     // k-chunk table (one entry per 32 columns): segment index, column offset inside the segment, has-aux flag
     int4* sKseg = reinterpret_cast<int4*>(reinterpret_cast<uint8_t*>(sChunk) + TAIL_CHUNK);
-    uint64_t* rbars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sKseg) + (MAX_K / 32) * 16);  // raw_full[8], raw_empty[8]
+    uint64_t* rbars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sKseg) + (MAX_K / 32) * 16);  // raw_full[8]
     const uint32_t bar0 = smem_u32(bars), rbar0 = smem_u32(rbars);
     auto rfull_bar = [&](int s) { return rbar0 + 8u * s; };
-    auto rempty_bar = [&](int s) { return rbar0 + 8u * (8 + s); };
     const int nkb = p.K / KC;
 
     // ---- one-time setup ----
     if (threadIdx.x == 0) {
         for (int s = 0; s < NSTAGE; ++s) {
             mbar_init(bar0 + 8u * s, WPG * 32);          // canonical stage full: the warps of one converter group
-            mbar_init(bar0 + 8u * (NSTAGE + s), 1);      // empty: tcgen05.commit
+            mbar_init(bar0 + 8u * (NSTAGE + s), NCONS);  // empty: one arrive per consumer warp
         }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(bar0 + 8u * (2 * NSTAGE + a), 1);
-            mbar_init(bar0 + 8u * (2 * NSTAGE + 2 + a), 128);
-        }
-        for (int s = 0; s < 8; ++s) {
-            mbar_init(rfull_bar(s), 1);                  // expect_tx arrive of the TMA lane
-            mbar_init(rempty_bar(s), WPG * 32);
-        }
+        for (int s = 0; s < 8; ++s) mbar_init(rfull_bar(s), 1);  // expect_tx arrive of the issuing lane
         fence_barrier_init();
     }
-    if (warp == NPROD) tmem_alloc(smem_u32(tmem_slot), 512);
     if (threadIdx.x < MAX_K / 32) {
         int kk = threadIdx.x * KC;
         int4 ent = make_int4(-1, 0, 0, 0);
@@ -882,55 +780,51 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) linear_tma_kernel(const TcPara
     {
         const uint4* src = reinterpret_cast<const uint4*>(p.Wpacked);
         uint4* dst = reinterpret_cast<uint4*>(sW);
-        for (int e = threadIdx.x; e < w_half / 16; e += TMA_THREADS) dst[e] = __ldg(src + e);
+        for (int e = threadIdx.x; e < w_half / 16; e += NTHREADS) dst[e] = __ldg(src + e);
         const uint4* srcl = reinterpret_cast<const uint4*>(p.Wlo);
         uint4* dstl = reinterpret_cast<uint4*>(sW + w_half);
-        for (int e = threadIdx.x; e < w_half / 16; e += TMA_THREADS) dstl[e] = __ldg(srcl + e);
+        for (int e = threadIdx.x; e < w_half / 16; e += NTHREADS) dstl[e] = __ldg(srcl + e);
     }
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
     TcCtx ctx;
-    ctx.sW = sW; ctx.sA = sA; ctx.sEpi = sEpi; ctx.sPf = sPf; ctx.sChunk = sChunk; ctx.bar0 = bar0; ctx.tmem_base = *tmem_slot;
+    ctx.sW = sW; ctx.sA = sA; ctx.sEpi = sEpi; ctx.sChunk = sChunk; ctx.bar0 = bar0;
     ctx.nkb = nkb; ctx.stage_bytes = stage_bytes; ctx.w_half = w_half;
-    ctx.idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.Npad >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
     const int64_t my_tiles = (p.num_tiles > blockIdx.x) ? (p.num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
     const int64_t total = my_tiles * nkb;
 
-    if (warp == NPROD + 5) {
-        // =============================== TMA producer ===============================
-        if (lane == 0) {
-            for (int sgi = 0; sgi < p.n_a; ++sgi) {
-                asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&maps.a[sgi])) : "memory");
-                if (p.a[sgi].aux) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&maps.x[sgi])) : "memory");
-            }
-            int rs = 0, kb = 0;
-            uint32_t rph = 0;
-            int64_t tile = blockIdx.x;
-            for (int64_t qs = 0; qs < total; ++qs) {
-                mbar_wait(rempty_bar(rs), rph ^ 1);
-                const int4 ent = sKseg[kb];
-                const uint32_t dst = smem_u32(sRaw + (size_t)rs * raw_slot);
-                const bool ax = p.has_aux && ent.z;
-                mbar_expect_tx(rfull_bar(rs), TMA_BOX_BYTES * (ax ? 2u : 1u));
-                if (!(p.debug & 2)) {
-                    tma_load_2d(dst, &maps.a[ent.x], ent.y, (int)(tile * BM), rfull_bar(rs));
-                    if (ax) tma_load_2d(dst + TMA_BOX_BYTES, &maps.x[ent.x], ent.y, (int)(tile * BM), rfull_bar(rs));
-                } else {
-                    asm volatile("mbarrier.complete_tx.shared::cta.b64 [%0], %1;" ::"r"(rfull_bar(rs)), "r"(TMA_BOX_BYTES * (ax ? 2u : 1u)) : "memory");
-                }
-                if (++rs == NR) { rs = 0; rph ^= 1; }
-                if (++kb == nkb) { kb = 0; tile += gridDim.x; }
-            }
+    // loads of sequence number qs (k block qs % nkb of this CTA's tile qs / nkb) into raw slot rs
+    auto tma_issue = [&](int64_t qs, int rs) {
+        const int64_t tile = blockIdx.x + (qs / nkb) * gridDim.x;
+        const int4 ent = sKseg[(int)(qs % nkb)];
+        const uint32_t dst = smem_u32(sRaw + (size_t)rs * raw_slot);
+        const bool ax = p.has_aux && ent.z;
+        mbar_expect_tx(rfull_bar(rs), TMA_BOX_BYTES * (ax ? 2u : 1u));
+        if (!(p.debug & 2)) {
+            tma_load_2d(dst, &maps.a[ent.x], ent.y, (int)(tile * BM), rfull_bar(rs));
+            if (ax) tma_load_2d(dst + TMA_BOX_BYTES, &maps.x[ent.x], ent.y, (int)(tile * BM), rfull_bar(rs));
+        } else {
+            asm volatile("mbarrier.complete_tx.shared::cta.b64 [%0], %1;" ::"r"(rfull_bar(rs)), "r"(TMA_BOX_BYTES * (ax ? 2u : 1u)) : "memory");
         }
-    } else if (warp < NPROD) {
+    };
+
+    if (warp >= NPROD) {
+        tc_consumer_role<TSrc, SPLIT, NCH>(p, ctx, warp - NPROD, lane);
+    } else {
         // =============================== converters ===============================
         const int grp = warp / WPG, sub = warp % WPG;
         const int r8 = lane & 7, kc = lane >> 3;
         // raw slot / canonical stage of sequence number qs: plain counters (advance by G per iteration)
         int rs = grp % NR, cs = grp % p.nstage, kb = grp % nkb;
         uint32_t rph = (uint32_t)((grp / NR) & 1), cph = (uint32_t)((grp / p.nstage) & 1);
+        const bool leader = sub == 0 && lane == 0;
+        if (leader) {
+            for (int sgi = 0; sgi < p.n_a; ++sgi) {
+                asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&maps.a[sgi])) : "memory");
+                if (p.a[sgi].aux) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&maps.x[sgi])) : "memory");
+            }
+            for (int q = grp; q < NR && q < total; q += G) tma_issue(q, q);  // first fill of this group's raw slots
+        }
         for (int64_t qs = grp; qs < total; qs += G) {
             mbar_wait(rfull_bar(rs), rph);
             const uint8_t* raw = sRaw + (size_t)rs * raw_slot;
@@ -955,8 +849,9 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) linear_tma_kernel(const TcPara
                     v[i][4] *= dsilu_fast(y.x); v[i][5] *= dsilu_fast(y.y); v[i][6] *= dsilu_fast(y.z); v[i][7] *= dsilu_fast(y.w);
                 }
             }
-            __syncwarp();
-            mbar_arrive(rempty_bar(rs));  // raw slot drained (values are in registers)
+            // raw slot drained by every warp of the group (values are in registers): refill it
+            asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "r"(WPG * 32) : "memory");
+            if (leader && qs + NR < total) tma_issue(qs + NR, rs);
             mbar_wait(ctx.empty_bar(cs), cph ^ 1);
             uint8_t* st_hi = sA + cs * stage_bytes;
 #pragma unroll
@@ -989,15 +884,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) linear_tma_kernel(const TcPara
             cs += G; if (cs >= p.nstage) { cs -= p.nstage; cph ^= 1; }
             kb += G; while (kb >= nkb) kb -= nkb;
         }
-    } else if (warp == NPROD) {
-        tc_mma_role<SPLIT>(p, ctx, lane);
-    } else {
-        tc_epilogue_role<TSrc, PF>(p, ctx, warp, lane);
     }
-    // ---- teardown ----
-    tc_fence_before();
-    __syncthreads();
-    if (warp == NPROD) tmem_dealloc(ctx.tmem_base, 512);
 }
 
 // W[K][N] (row-major TSrc) -> canonical K-major no-swizzle bf16 images (hi, lo), Npad rows:
@@ -1017,7 +904,8 @@ __global__ void pack_w_kernel(int K, int N, int Npad, const TSrc* __restrict__ W
 
 }  // namespace
 
-static int tc_npad(int N) { return (N + 15) / 16 * 16; }
+// W images are padded to whole 32-column chunks (the wgmma N granularity used here)
+static int tc_npad(int N) { return (N + 31) / 32 * 32; }
 
 extern "C" int64_t ab2_linear_packed_bytes(int dtype, int K, int N) {
     if (dtype == AB2_F64 || K % 16 != 0 || K <= 0 || K > MAX_K || N <= 0) return 0;
@@ -1025,11 +913,11 @@ extern "C" int64_t ab2_linear_packed_bytes(int dtype, int K, int N) {
     return (int64_t)Npad * K * 2 * 2;  // hi + lo images (any N: wide outputs run as column slices, see ab2_linear_tc_try)
 }
 
-// widest column slice (multiple of 32, <= 256) whose resident W image fits MAX_W_BYTES
+// widest column slice (multiple of 32, <= MAX_N) whose resident W image fits MAX_W_BYTES
 static int tc_slice_cap(int dtype, int K) {
     const int per_col = K * 2 * (dtype == AB2_F32 ? 2 : 1);
     int cap = (MAX_W_BYTES / per_col) / 32 * 32;
-    if (cap > 256) cap = 256;
+    if (cap > MAX_N) cap = MAX_N;
     return cap;
 }
 
@@ -1078,7 +966,7 @@ static bool tc_make_map(CUtensorMap* map, const void* ptr, int64_t ld, int width
               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-static int tc_launch_tma(TcParams& p, int pf_mode, int w_bytes, int stage_bytes, int max_smem, unsigned grid, cudaStream_t st, bool dry) {
+static int tc_launch_tma(TcParams& p, int w_bytes, int stage_bytes, int max_smem, unsigned grid, cudaStream_t st, bool dry) {
     TmaMaps maps;
     memset(&maps, 0, sizeof(maps));
     if (!tc_encode_fn()) return -1;
@@ -1093,7 +981,7 @@ static int tc_launch_tma(TcParams& p, int pf_mode, int w_bytes, int stage_bytes,
     int G = 0, NR = 0, nstage = 0;
     size_t smem = 0;
     for (int q = 0; q < 6 && !G; ++q) {
-        const size_t need = 1024 + ((w_bytes + 127) & ~127) + (size_t)plans[q][2] * stage_bytes + EPI_BYTES + (pf_mode ? PF_BYTES : 0) + TAIL_BYTES +
+        const size_t need = 1024 + ((w_bytes + 127) & ~127) + (size_t)plans[q][2] * stage_bytes + EPI_BYTES + TAIL_BYTES +
                             (size_t)plans[q][1] * raw_slot;
         if (need <= (size_t)max_smem) { G = plans[q][0]; NR = plans[q][1]; nstage = plans[q][2]; smem = need; }
     }
@@ -1105,17 +993,20 @@ static int tc_launch_tma(TcParams& p, int pf_mode, int w_bytes, int stage_bytes,
             cudaGetLastError();
             return -1;
         }
-        kern<<<grid, TMA_THREADS, smem, st>>>(p, maps, NR);
+        kern<<<grid, NTHREADS, smem, st>>>(p, maps, NR);
         return 0;
     };
-    if (G == 4) {
-        if (pf_mode == 1) return go(linear_tma_kernel<1, 4>);
-        if (pf_mode == 2) return go(linear_tma_kernel<2, 4>);
-        return go(linear_tma_kernel<0, 4>);
+    switch ((G == 4 ? 4 : 0) + p.Npad / 32) {
+        case 1: return go(linear_tma_kernel<2, 1>);
+        case 2: return go(linear_tma_kernel<2, 2>);
+        case 3: return go(linear_tma_kernel<2, 3>);
+        case 4: return go(linear_tma_kernel<2, 4>);
+        case 5: return go(linear_tma_kernel<4, 1>);
+        case 6: return go(linear_tma_kernel<4, 2>);
+        case 7: return go(linear_tma_kernel<4, 3>);
+        case 8: return go(linear_tma_kernel<4, 4>);
     }
-    if (pf_mode == 1) return go(linear_tma_kernel<1, 2>);
-    if (pf_mode == 2) return go(linear_tma_kernel<2, 2>);
-    return go(linear_tma_kernel<0, 2>);
+    return -1;
 }
 
 // One column slice [n0, n0 + N) of the GEMM with its W images resident in shared memory.
@@ -1124,11 +1015,7 @@ static int tc_launch_slice(int dtype, int64_t M, int K, int N, int n_a, const vo
                            int n_o, void* const* o_ptr, const int64_t* o_ld, const int32_t* o_width, const int32_t* o_accum, int epi,
                            const void* aux, int64_t aux_ld, cudaStream_t st, bool dry = false) {
     const int has_aux = (act == AB2_ACT_MUL_DSILU && a_aux) ? 1 : 0;
-    int pf_mode = 0;
-    if (dtype == AB2_F32) {
-        if (epi == AB2_EPI_MUL_DSILU) pf_mode = 1;
-        else if (o_accum) for (int s = 0; s < n_o; ++s) if (o_accum[s]) pf_mode = 2;
-    }
+    if (tc_npad(N) > MAX_N) return -1;
     static int num_sms = 0;
     static int max_smem = 0;
     if (num_sms == 0) {
@@ -1157,21 +1044,20 @@ static int tc_launch_slice(int dtype, int64_t M, int K, int N, int n_a, const vo
     const int plans[4][2] = {{4, NSTAGE}, {4, 2}, {2, NSTAGE}, {2, 2}};
     for (int q = 0; q < 4 && !nstage; ++q) {
         const size_t need = ((w_bytes + 127) & ~127) + (size_t)plans[q][1] * stage_bytes + (size_t)plans[q][0] * raw_stage + EPI_BYTES +
-                            (pf_mode ? PF_BYTES : 0) + TAIL_BYTES;
+                            TAIL_BYTES;
         if ((int)need <= max_smem) { raw_depth = plans[q][0]; nstage = plans[q][1]; smem = need; }
     }
     if (!nstage) return -1;
     if (dry) return 0;
     p.nstage = nstage;
     p.raw_depth = raw_depth;
-    p.pf_mode = pf_mode;
     p.debug = g_ab2_opt_tc_debug;
     const unsigned grid = (unsigned)((p.num_tiles < num_sms) ? p.num_tiles : num_sms);
     // ---- TMA-producer kernel: fp32 storage, every A segment (and K) a multiple of 32 columns ----
     bool tma_ok = g_ab2_opt_linear_tma && split && K % KC == 0 && M < ((int64_t)1 << 31);
     for (int s = 0; s < n_a && tma_ok; ++s) tma_ok = a_width[s] % KC == 0;
     if (tma_ok) {
-        const int rc = tc_launch_tma(p, pf_mode, w_bytes, stage_bytes, max_smem, grid, st, dry);
+        const int rc = tc_launch_tma(p, w_bytes, stage_bytes, max_smem, grid, st, dry);
         if (rc == 0) return 0;
     }
     auto go = [&](auto kern) -> int {
@@ -1182,16 +1068,21 @@ static int tc_launch_slice(int dtype, int64_t M, int K, int N, int n_a, const vo
         kern<<<grid, NTHREADS, smem, st>>>(p);
         return 0;
     };
-    if (split) {
-        if (pf_mode == 1) return go(linear_tc_kernel<float, true, 1>);
-        if (pf_mode == 2) return go(linear_tc_kernel<float, true, 2>);
-        return go(linear_tc_kernel<float, true, 0>);
+    switch ((split ? 4 : 0) + p.Npad / 32) {
+        case 1: return go(linear_tc_kernel<bf16, false, 1>);
+        case 2: return go(linear_tc_kernel<bf16, false, 2>);
+        case 3: return go(linear_tc_kernel<bf16, false, 3>);
+        case 4: return go(linear_tc_kernel<bf16, false, 4>);
+        case 5: return go(linear_tc_kernel<float, true, 1>);
+        case 6: return go(linear_tc_kernel<float, true, 2>);
+        case 7: return go(linear_tc_kernel<float, true, 3>);
+        case 8: return go(linear_tc_kernel<float, true, 4>);
     }
-    return go(linear_tc_kernel<bf16, false, 0>);
+    return -1;
 }
 
 // returns 0 if launched, -1 if this call is not eligible (caller falls back to linear.cu).
-// Outputs wider than 256 columns, or whose W image exceeds the shared-memory budget, run as column slices (one launch
+// Outputs wider than MAX_N columns, or whose W image exceeds the shared-memory budget, run as column slices (one launch
 // per slice, each with its W slice resident; the A rows are re-read per slice).
 int ab2_linear_tc_try(int dtype, int64_t M, int K, int N, int n_a, const void* const* a_ptr, const int64_t* a_ld,
                       const int32_t* a_width, const void* const* a_aux, const int64_t* a_aux_ld, int act, const void* Wpacked, int n_o, void* const* o_ptr, const int64_t* o_ld,

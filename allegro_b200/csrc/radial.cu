@@ -352,9 +352,8 @@ __global__ void __launch_bounds__(128) radial_pq_bwd_kernel(int64_t E, int S, TA
 }
 
 // (A warp-cooperative variant -- 32-column chunks moved with row-contiguous 128-byte segments through a padded shared-memory
-// tile, then the same row walk -- was tried in round 2 and lost: 174 us instead of 115 us at the c2 shapes.  The tile's
-// load -> silu' -> store -> sync -> load chain with 16 resident warps hides less latency than 32 independent 16-byte loads per
-// thread with 32+ resident warps, uncoalesced as they are; profiles/README.md, r2q.)
+// tile, then the same row walk -- is slower: the tile's load -> silu' -> store -> sync -> load chain with 16 resident warps
+// hides less latency than 32 independent 16-byte loads per thread with 32+ resident warps, uncoalesced as they are.)
 
 #define AB2_RADIAL_PQ_DISPATCH(KERNEL, ...)                                                                       \
     do {                                                                                                          \

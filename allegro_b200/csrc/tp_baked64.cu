@@ -6,8 +6,8 @@
 // with V0 = Y (x) w0 formed on the fly (tensorembed.py:95).
 //
 // Why.  The shape-generic kernels (tp.cu) walk the run-time table per (edge, channel) with dynamically indexed per-thread
-// arrays -> local memory, three index loads and two global loads per entry: 36-65 ms per launch at the c5 size, two thirds
-// of that config's step.  The table's (i, j, k) structure is fixed by the selection rules (tools/gen_tp_tables.py emits it
+// arrays -> local memory, three index loads and two global loads per entry, which makes them the larger part of the c5
+// step.  The table's (i, j, k) structure is fixed by the selection rules (tools/gen_tp_tables.py emits it
 // as constexpr), only cgw[nnz][u] is data.  With the structure baked the 611-entry contraction is straight-line DFMAs on
 // REGISTERS (<= 63 live doubles: the backward runs its two products as two launches -- in one kernel the compiler parks
 // ~5 KB per thread in local memory between the passes), the 32-channel slice of

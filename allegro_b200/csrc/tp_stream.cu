@@ -10,7 +10,7 @@
 // (cp.async.bulk.shared.global, SASS UBLKCP) per stage of TE edges, issued by ONE elected producer
 // thread and completed on an mbarrier -- the memory-level parallelism (NS stages x several CTAs per
 // SM, 100+ KB in flight per SM) no longer depends on registers or on the number of resident warps,
-// which is what held the register-/shared-memory-M kernels of round 1 at 0.2-0.37 of the HBM rate.
+// which is what limits kernels that keep M in registers or shared memory and load with plain per-thread loads.
 //
 // Work split.  Persistent-style grid: CTA b owns a contiguous range of centres holding ~E/grid edges
 // (binary search over row_ptr), i.e. one contiguous edge stream.  Per CTA:
@@ -23,7 +23,7 @@
 //                              (<= 45 + 45 values) at ~130 registers -> 4-5 CTAs per SM.
 // The backward is ONE launch: gVin / gw0 / gY per edge and gM accumulated over the centre's row, then
 // ggamma[c][j] = sum_nnz cgw * gM[i][k] once per centre -- written exactly once, no atomics, fixed order
-// (deterministic), gVout / w0 / Y read exactly once (round 1 read them twice in two launches).
+// (deterministic), gVout / w0 / Y read exactly once.
 #include <type_traits>
 
 #include "common.cuh"
@@ -31,11 +31,15 @@
 #include "tp_tables_generated.cuh"
 #include "stream_common.cuh"
 
+#if !defined(AB2_TP_STREAM_GROUP) || AB2_TP_STREAM_GROUP == 0  // defined once, in group 0 (see the end of this file)
 int g_ab2_opt_tp_stream = 1;    // 1: use these kernels where instantiated, 0: round-1 kernels
 int g_ab2_opt_tp_stream_te = 0;  // edges per stage (0 = default 8), 8 or 16
 int g_ab2_opt_tp_stream_cps = 0; // cap on CTAs per SM (0 = occupancy limit)
 int g_ab2_opt_tp_stream_last = 1;    // 9 -> 1 (last layer) backward through the streaming kernel instead of tp_smem + split
 int g_ab2_opt_tp_stream_gytile = 1;  // layer-0 backward: gY reduced through a shared-memory tile instead of per-edge shuffles
+#else
+extern int g_ab2_opt_tp_stream, g_ab2_opt_tp_stream_te, g_ab2_opt_tp_stream_cps, g_ab2_opt_tp_stream_last, g_ab2_opt_tp_stream_gytile;
+#endif
 
 namespace {
 
@@ -307,8 +311,8 @@ __device__ __forceinline__ void tp_stream_body(const StreamParams& p) {
         constexpr int NI = MODE == 1 ? (ROLE ? D_IN - IS : IS) : D_IN;
         constexpr int K0 = MODE == 0 ? (ROLE ? KS : 0) : 0;
         constexpr int NK = MODE == 0 ? (ROLE ? D_OUT - KS : KS) : D_OUT;
-        // Blackwell issues one 3-register FFMA per 2 cycles per SM sub-partition; the full fp32 rate needs the packed
-        // FFMA2 (fma.rn.f32x2).  M and gM are therefore held as column PAIRS (k, k+1) (+ one single column when NK is odd).
+        // M and gM are held as column PAIRS (k, k+1) (+ one single column when NK is odd); fma2 (common.cuh) updates a
+        // pair with two FFMAs.
         constexpr int KP = NK / 2, KR = NK % 2;
         [[maybe_unused]] constexpr int YP = (D_IN + 3) / 4 * 4;  // padded Y row in shared memory
         float2 M2[NI][KP > 0 ? KP : 1];
@@ -524,7 +528,7 @@ __device__ __forceinline__ void tp_stream_body(const StreamParams& p) {
                     for (int i = 0; i < D_IN; ++i) {
                         const float2 vv = make_float2(v[i], v[i]);
 #pragma unroll
-                        for (int kp = 0; kp < KP; ++kp) o2[kp] = __ffma2_rn(vv, M2[i][kp], o2[kp]);
+                        for (int kp = 0; kp < KP; ++kp) o2[kp] = fma2(vv, M2[i][kp], o2[kp]);
                         if (KR) o_r = fmaf(v[i], Mr[i], o_r);
                     }
                     if (live) {
@@ -575,8 +579,8 @@ __device__ __forceinline__ void tp_stream_body(const StreamParams& p) {
                         const float2 vv = make_float2(v[i], v[i]);
 #pragma unroll
                         for (int kp = 0; kp < KP; ++kp) {
-                            a2 = __ffma2_rn(M2[i][kp], go2[kp], a2);
-                            gM2[i][kp] = __ffma2_rn(vv, go2[kp], gM2[i][kp]);
+                            a2 = fma2(M2[i][kp], go2[kp], a2);
+                            gM2[i][kp] = fma2(vv, go2[kp], gM2[i][kp]);
                         }
                         float s = a2.x + a2.y;
                         if (KR) {
@@ -601,8 +605,8 @@ __device__ __forceinline__ void tp_stream_body(const StreamParams& p) {
                         for (int i = 0; i < NI; ++i) part[i] = wl[sh_l_of(I0 + i)] * gin[i];
                         if constexpr (GYT) {
                             // one xor-16 step (independent shuffles, no chain), lanes 0-15 park the half sums in the tile;
-                            // the stage's rows are summed once per stage below.  The multi-level shuffle reduction per edge
-                            // was ~45 % of an edge's latency (profiles/r2j_bwd_l0_analysis.md).
+                            // the stage's rows are summed once per stage below, instead of a multi-level shuffle chain
+                            // per edge on the edge's critical path.
 #pragma unroll
                             for (int i = 0; i < NI; ++i) {
                                 const float pr = part[i] + __shfl_xor_sync(0xffffffffu, part[i], 16);
@@ -707,9 +711,12 @@ int launch_cfg(const StreamParams& p, cudaStream_t st) {
         cudaGetLastError();
         return -1;
     }
-    // the 9 -> 1 backward is purely memory-bound: 3 CTAs/SM stream 5.9 TB/s, the 5 the occupancy allows 5.3 TB/s (r2s)
+    // the 9 -> 1 backward is purely memory-bound: 3 CTAs/SM keep enough bytes in flight.  On an H100 (700 W limit, c2
+    // shapes) the cap and the occupancy limit give the same time (0.42 ms per launch), so the cap
+    // stays as it is.
     if (D_OUT == 1 && MODE == 1 && cps > 3 && g_ab2_opt_tp_stream_cps == 0) cps = 3;
-    // explicit 9 x 9 -> 9 forward (middle layers of deeper models): 187 us at 3 CTAs/SM, 213 us at the occupancy limit (r2t)
+    // explicit 9 x 9 -> 9 forward (middle layers of models with 3+ layers): capped at 3 CTAs/SM like the 9 -> 1 backward;
+    // not measured on an H100 (the benchmark config has no middle layer).  tp_stream_cps overrides both caps.
     if (D_IN == 9 && D_OUT == 9 && MODE == 0 && !IMPLICIT && NCH == 1 && cps > 3 && g_ab2_opt_tp_stream_cps == 0) cps = 3;
     if (g_ab2_opt_tp_stream_cps > 0 && cps > g_ab2_opt_tp_stream_cps) cps = g_ab2_opt_tp_stream_cps;
     int64_t grid = (int64_t)num_sms * cps;
@@ -740,7 +747,71 @@ int launch_shape(const StreamParams& p, cudaStream_t st) {
     return -1;
 }
 
+// The instantiations are compiled in eight translation units so that a parallel build compiles them side by side
+// (about 70 kernels: one translation unit takes about 12 minutes of ptxas time for sm_90a, the slowest of the
+// eight under 3 minutes):
+// this file (group 0, plus the entry point ab2_tp_stream) and tp_stream_g1.cu .. tp_stream_g7.cu, which define
+// AB2_TP_STREAM_GROUP and include this file.  Per storage type TA, the groups are
+//   d_in 9 forward | d_in 9 backward with implicit V0 | d_in 9 backward with explicit input (+ 9 -> 1 last layer) | d_in 4.
+// Each group is one function: part 0 forward, 1 backward with implicit V0, 2 backward with explicit input.
+#ifndef AB2_TP_STREAM_GROUP
+#define AB2_TP_STREAM_GROUP 0
+#endif
+template <typename TA>
+int tp_stream_fwd9(const StreamParams& p, bool implicit_v0, cudaStream_t st) {
+    return implicit_v0 ? launch_shape<TA, float, 9, 9, true, 0>(p, st) : launch_shape<TA, float, 9, 9, false, 0>(p, st);
+}
+template <typename TA>
+int tp_stream_bwd9_explicit(const StreamParams& p, bool last9, cudaStream_t st) {
+    return last9 ? launch_shape<TA, float, 9, 1, false, 1>(p, st) : launch_shape<TA, float, 9, 9, false, 1>(p, st);
+}
+template <typename TA>
+int tp_stream_all4(const StreamParams& p, int part, bool implicit_v0, cudaStream_t st) {
+    if (part == 0) return implicit_v0 ? launch_shape<TA, float, 4, 4, true, 0>(p, st) : launch_shape<TA, float, 4, 4, false, 0>(p, st);
+    return implicit_v0 ? launch_shape<TA, float, 4, 4, true, 1>(p, st) : launch_shape<TA, float, 4, 4, false, 1>(p, st);
+}
 }  // namespace
+
+int ab2_tp_stream_group(int group, const void* params, int part, bool implicit_v0, bool last9, cudaStream_t st);
+#if AB2_TP_STREAM_GROUP != 0
+// group g of storage type TA = (g < 4 ? float : bf16), kind g % 4
+static int ab2_tp_stream_group_impl(const void* params, int part, bool implicit_v0, bool last9, cudaStream_t st) {
+    using TA = std::conditional<(AB2_TP_STREAM_GROUP < 4), float, bf16>::type;
+    const StreamParams& p = *static_cast<const StreamParams*>(params);
+    constexpr int kind = AB2_TP_STREAM_GROUP % 4;
+    if constexpr (kind == 0) return tp_stream_fwd9<TA>(p, implicit_v0, st);
+    else if constexpr (kind == 1) return launch_shape<TA, float, 9, 9, true, 1>(p, st);
+    else if constexpr (kind == 2) return tp_stream_bwd9_explicit<TA>(p, last9, st);
+    else return tp_stream_all4<TA>(p, part, implicit_v0, st);
+}
+#define AB2_TP_STREAM_GROUP_SYM_(g) ab2_tp_stream_group##g
+#define AB2_TP_STREAM_GROUP_SYM(g) AB2_TP_STREAM_GROUP_SYM_(g)
+int AB2_TP_STREAM_GROUP_SYM(AB2_TP_STREAM_GROUP)(const void* params, int part, bool implicit_v0, bool last9, cudaStream_t st) {
+    return ab2_tp_stream_group_impl(params, part, implicit_v0, last9, st);
+}
+#else
+int ab2_tp_stream_group1(const void*, int, bool, bool, cudaStream_t);
+int ab2_tp_stream_group2(const void*, int, bool, bool, cudaStream_t);
+int ab2_tp_stream_group3(const void*, int, bool, bool, cudaStream_t);
+int ab2_tp_stream_group4(const void*, int, bool, bool, cudaStream_t);
+int ab2_tp_stream_group5(const void*, int, bool, bool, cudaStream_t);
+int ab2_tp_stream_group6(const void*, int, bool, bool, cudaStream_t);
+int ab2_tp_stream_group7(const void*, int, bool, bool, cudaStream_t);
+
+// launches of group `group` (see above); group 0 (fp32, d_in 9 forward) is instantiated here
+int ab2_tp_stream_group(int group, const void* params, int part, bool implicit_v0, bool last9, cudaStream_t st) {
+    switch (group) {
+        case 0: return tp_stream_fwd9<float>(*static_cast<const StreamParams*>(params), implicit_v0, st);
+        case 1: return ab2_tp_stream_group1(params, part, implicit_v0, last9, st);
+        case 2: return ab2_tp_stream_group2(params, part, implicit_v0, last9, st);
+        case 3: return ab2_tp_stream_group3(params, part, implicit_v0, last9, st);
+        case 4: return ab2_tp_stream_group4(params, part, implicit_v0, last9, st);
+        case 5: return ab2_tp_stream_group5(params, part, implicit_v0, last9, st);
+        case 6: return ab2_tp_stream_group6(params, part, implicit_v0, last9, st);
+        case 7: return ab2_tp_stream_group7(params, part, implicit_v0, last9, st);
+    }
+    return -1;
+}
 
 // returns 0 if launched, -1 if (dtype, shape, alignment) has no streaming instantiation
 int ab2_tp_stream(int mode, int dtype, int64_t N, int64_t E, int U, int D, int d_in, int d_out, int nnz, const int32_t* tab,
@@ -769,24 +840,14 @@ int ab2_tp_stream(int mode, int dtype, int64_t N, int64_t E, int U, int D, int d
     if (mode == 1 && implicit_v0 && dtype == AB2_F32 && d_in == 9 && D == 9 && U == 32 && nnz == Tab9x9x9::NNZ && E < ((int64_t)1 << 31) &&
         ab2_tp_stream3_bwd(N, E, tab, cgw, row_ptr, ctr, gamma, Y, w0, gVout, gw0, gY, ggamma, st) == 0)
         p.skip_if_baked = 1;
+    const int base = dtype == AB2_F32 ? 0 : 4;
     if (last9) {
         p.skip_if_baked = 0;
         p.gy_tile = 0;
-        if (dtype == AB2_F32) return launch_shape<float, float, 9, 1, false, 1>(p, st);
-        return launch_shape<bf16, float, 9, 1, false, 1>(p, st);
+        return ab2_tp_stream_group(base + 2, &p, 2, false, true, st);
     }
-#define AB2_STREAM_CASE(TA, DI)                                                                                        \
-    if (d_in == DI) {                                                                                                   \
-        if (mode == 0) return implicit_v0 ? launch_shape<TA, float, DI, DI, true, 0>(p, st) : launch_shape<TA, float, DI, DI, false, 0>(p, st); \
-        return implicit_v0 ? launch_shape<TA, float, DI, DI, true, 1>(p, st) : launch_shape<TA, float, DI, DI, false, 1>(p, st);               \
-    }
-    if (dtype == AB2_F32) {
-        AB2_STREAM_CASE(float, 9)
-        AB2_STREAM_CASE(float, 4)
-    } else {
-        AB2_STREAM_CASE(bf16, 9)
-        AB2_STREAM_CASE(bf16, 4)
-    }
-#undef AB2_STREAM_CASE
-    return -1;
+    if (d_in == 4) return ab2_tp_stream_group(base + 3, &p, mode, implicit_v0, false, st);
+    if (mode == 0) return ab2_tp_stream_group(base + 0, &p, 0, implicit_v0, false, st);
+    return ab2_tp_stream_group(base + (implicit_v0 ? 1 : 2), &p, 1, implicit_v0, false, st);
 }
+#endif

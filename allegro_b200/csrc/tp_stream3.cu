@@ -1,13 +1,13 @@
-// Layer-0 tensor-product backward, THREE consumer warps per 32-channel centre stream (round 2, second half).
+// Layer-0 tensor-product backward, THREE consumer warps per 32-channel centre stream.
 //
 // Same semantics, data layout and TMA-staged pipeline as tp_stream_kernel<9, 9, implicit, bwd> (tp_stream.cu; reference:
 // Contracter._contract, allegro/nn/_strided/_contract.py:213-251, its two backward products _flashallegro.py:347-360,
 // and the V0 = Y (x) w0 embedding of tensorembed.py:95 folded in), specialised to the l_max = 2 layer-0 shape
 // (d_in = d_env = d_out = 9, fp32, U = 32) with the baked 83-entry coupling-table structure.
 //
-// Why.  The two-warp kernel is latency-bound, not throughput-bound (ncu, profiles/r2f_ncu_full_summary.md: issue active
-// 44 %, FMA pipe 33 %, DRAM 37 %, stalls `wait` + short scoreboard): 168 registers -> 4 CTAs/SM -> only 8 consumer warps
-// per SM (2 per sub-partition) to cover the LDS -> FFMA2 chain -> shuffle-reduction latency of an edge.  Splitting the
+// Why.  The two-warp kernel is latency-bound, not throughput-bound (no pipe saturated, stalls on fixed-latency
+// dependencies and the shared-memory scoreboard): 168 registers -> 4 CTAs/SM -> only 8 consumer warps per SM
+// (2 per sub-partition) to cover the LDS -> FMA chain -> shuffle-reduction latency of an edge.  Splitting the
 // coupling matrix M_c and its gradient gM_c over THREE row groups {1,2,3} | {4,5,6} | {0,7,8} needs 27 + 27 resident values
 // per lane instead of 45 + 45 -> <= 128 registers -> 4 CTAs/SM x 3 = 12 consumer warps per SM at the same shared-memory
 // footprint.  The l = 2 block of gw0 straddles two warps (rows 4-6 | 7-8): warp C parks its partial in a per-stage slot
@@ -20,7 +20,7 @@
 #include "tp_tables_generated.cuh"
 #include "stream_common.cuh"
 
-int g_ab2_opt_tp_stream3 = 1;  // 1 (default): three-warp backward where eligible (265 us at the c2 shapes), 0: two-warp tp_stream kernel (285 us)
+int g_ab2_opt_tp_stream3 = 1;  // 1 (default): three-warp backward where eligible, 0: two-warp tp_stream kernel
 // stage knock-outs for tools/time_tp3.py (results are WRONG when non-zero): bit0 consumers skip the edge arithmetic,
 // bit1 no gY reduction / RED, bit2 no RED only, bit3 producer polls without back-off, bit4 no Y copies, bit5 no per-centre work,
 // bit6 compute only (no bulk copies); bit8 selects the unroll-2 build instead of the default unroll-1 (results stay right)
@@ -322,8 +322,8 @@ __global__ void __launch_bounds__(128, 4) tp_bwd3_kernel(const Params3 p) {
                 }
                 const int t_end = (row_end32 - za) < n ? (row_end32 - za) : n;
                 if (dbg & 1) t = t_end;
-                // (a hand-made software pipeline -- reads of edge t + 1 issued before the arithmetic of edge t -- was tried
-                // and lost: 355 us instead of 305 us, more registers and moves; profiles/README.md r2m)
+                // (a hand-made software pipeline -- reads of edge t + 1 issued before the arithmetic of edge t -- costs
+                // more registers and moves than it hides)
 #pragma unroll UNR
                 for (; t < t_end; ++t) {
                     EdgeIn cur;
@@ -336,8 +336,8 @@ __global__ void __launch_bounds__(128, 4) tp_bwd3_kernel(const Params3 p) {
                         float2 a2 = make_float2(0.f, 0.f);
 #pragma unroll
                         for (int kp = 0; kp < 4; ++kp) {
-                            a2 = __ffma2_rn(M2[r][kp], cur.go2[kp], a2);
-                            gM2[r][kp] = __ffma2_rn(vv, cur.go2[kp], gM2[r][kp]);
+                            a2 = fma2(M2[r][kp], cur.go2[kp], a2);
+                            gM2[r][kp] = fma2(vv, cur.go2[kp], gM2[r][kp]);
                         }
                         gin[r] = fmaf(Mr[r], cur.go_r, a2.x + a2.y);
                         gMr[r] = fmaf(v[r], cur.go_r, gMr[r]);
@@ -352,8 +352,8 @@ __global__ void __launch_bounds__(128, 4) tp_bwd3_kernel(const Params3 p) {
                         xw[t * U3] = fmaf(cur.Yv[2], gin[2], cur.Yv[1] * gin[1]);
                     }
                     // gY[z][i] += sum_u w0[l(i)][u] gin[i][u]: one xor-16 step in registers (three independent shuffles, no
-                    // chain), lanes 0-15 park the half sums; the stage's rows are summed once per stage below.  The
-                    // five-level shuffle reduction per edge was ~45 % of the edge's latency (profiles/r2j, r2l: 331 -> 306 us).
+                    // chain), lanes 0-15 park the half sums; the stage's rows are summed once per stage below, instead of
+                    // a five-level shuffle chain per edge on the edge's critical path.
                     if (!(dbg & 2)) {
 #pragma unroll
                         for (int r = 0; r < 3; ++r) {
@@ -433,7 +433,7 @@ int ab2_tp_stream3_bwd(int64_t N, int64_t E, const int32_t* tab, const void* cgw
     p.N = N; p.E = E; p.tab = tab; p.cgw = (const float*)cgw; p.row_ptr = row_ptr; p.ctr = ctr; p.gamma = (const float*)gamma;
     p.Y = (const float*)Y; p.w0 = (const float*)w0; p.gVout = (const float*)gVout; p.gw0 = (float*)gw0; p.gY = (float*)gY; p.ggamma = (float*)ggamma;
     p.debug = g_ab2_opt_tp_stream3_debug & 0xff;
-    const int unr1 = ((g_ab2_opt_tp_stream3_debug >> 8) & 1) ^ 1;  // default: the unroll-1 build (259 us vs 265 us); bit 8 selects unroll 2
+    const int unr1 = ((g_ab2_opt_tp_stream3_debug >> 8) & 1) ^ 1;  // default: the unroll-1 build; bit 8 selects unroll 2
     kerns[(p.debug ? 2 : 0) + unr1]<<<(unsigned)grid, 128, SMEM3, st>>>(p);
     return 0;
 }

@@ -1,6 +1,6 @@
 """CUDA-graph capture of one energy+forces evaluation.
 
-The step is a fixed sequence of ~50 kernel launches from Python/ctypes; at ~2 ms per step the
+The step is a fixed sequence of ~50 kernel launches from Python/ctypes; at a few ms per step the
 launch path matters, so (instead of a tracing compiler) the whole sequence is captured once into a
 CUDA graph and replayed: positions are copied into a static buffer, outputs live in static buffers.
 Valid as long as the neighbour list (edge_index / shifts / types / cell) is unchanged -- exactly

@@ -1,4 +1,4 @@
-"""Contracter: the reference's kernel plug-in point, backed by the sm_100a operator kernels.
+"""Contracter: the reference's kernel plug-in point, backed by the sm_90a operator kernels.
 
 Mirrors allegro/nn/_strided/_contract.py:11-313 -- same constructor kwargs, same
 ``state_dict`` (``weights`` of shape (mul,P)/(mul,)/(P,)/(), dense ``w3j`` buffer), same
@@ -288,7 +288,7 @@ class Contracter(torch.nn.Module):
     @classmethod
     def enable_B200Contracter(cls, model: torch.nn.Module) -> torch.nn.Module:
         """Replace every module whose class is named ``Contracter`` (reference or ours) by a
-        B200-backed one with identical constructor kwargs and state_dict."""
+        CUDA-backed one with identical constructor kwargs and state_dict."""
 
         def factory(old):
             dt = old.w3j.dtype

@@ -109,7 +109,7 @@ class PackedMLP:
         self.silu = mlp.nonlinearity == "silu"
         self.W = [w.to(device=device, dtype=dtype).contiguous() for w in ws]
         self.WT = [w.T.to(device=device, dtype=dtype).contiguous() for w in ws]
-        # tcgen05 path: packed bf16 hi/lo images (None where the shape is not eligible)
+        # wgmma path: packed bf16 hi/lo images (None where the shape is not eligible)
         self.Wp = [_lib.linear_pack(w) for w in self.W]
         self.WTp = [_lib.linear_pack(w) for w in self.WT]
         # a width-<16 output (the readout's single energy column) makes the backward GEMM's K < 16, which the

@@ -97,8 +97,8 @@ class AllegroCore:
         # along K, each consumer's g_h scaled by silu'(pre) in the GEMM prologue -- no accumulation.
         import os as _os
 
-        # measured on B200 (c2): 5.17 ms/step with this plan vs 4.79 ms with the epilogue/accumulate plan, so it is
-        # opt-in (ALLEGRO_B200_PLAIN_BWD=1); both are covered by the GPU tests.
+        # the epilogue/accumulate plan is the default, this one is opt-in (ALLEGRO_B200_PLAIN_BWD=1); both are covered
+        # by the GPU tests.
         self.plain_ok = (_os.environ.get("ALLEGRO_B200_PLAIN_BWD", "0") == "1" and self.readout.is_two_layer_silu
                          and all(ly["mlp"].is_two_layer_silu for ly in self.layers))
         if self.plain_ok:
@@ -285,7 +285,7 @@ class UpstreamPack:
         # fold_embed_of: x_emb only feeds two LINEAR maps (tensorembed.py:88-89 env_embed_linear, _allegro.py:251
         # first_layer_env_embed_projection), and the scalar-embed MLP ends in a linear layer, so their product is
         # one matrix: [w0 | x_0 | omega_0] = silu(h) @ (W_last @ W_embed).  One GEMM and the x_emb round trip less
-        # in each direction.  Default since round 2 (c2: 4.00 -> 3.88 ms/step); ALLEGRO_B200_FOLD_EMBED=0 switches it off.
+        # in each direction.  Default on; ALLEGRO_B200_FOLD_EMBED=0 switches it off.
         self.fold = fold_embed_of is not None
         self.mlp = PackedMLP(scalar_embed_mlp, dtype, device, post=fold_embed_of.embed.W64[0] if self.fold else None)
         self.dtype = dtype

@@ -1,4 +1,4 @@
-"""Host-side O(3) bookkeeping and constant tables for the B200 kernels.
+"""Host-side O(3) bookkeeping and constant tables for the CUDA kernels.
 
 Setup-time only (runs once per model build, on the CPU): irreps algebra, the real-basis
 Wigner-3j table generator and the per-layer sparse coupling tables the CUDA kernels consume.

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- atom-steps/s (energy + forces) of the Allegro hot path on B200.
+"""bench.py -- atom-steps/s (energy + forces) of the Allegro hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W            # this framework
     python bench.py --impl reference --gpus N --steps K ...  # CPU reference arm (oracle port)
+    python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR   # also write the last timed step's outputs as .npy
 
 One "step" = one energy+forces evaluation of the configured model on one synthetic frame
 (neighbour list given, built outside the timed region).  N=1 workload: BASELINE.json
@@ -74,6 +75,46 @@ class ClockSampler:
         sm.sort()
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": sorted(reasons),
                 "samples": len(sm)}
+
+
+def gpu_info(index: int):
+    """Name and power limit of the card a number is measured on (both are part of the number)."""
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=10).stdout.strip()
+        name, limit = [c.strip() for c in out.split(",")]
+        return {"name": name, "power_limit_w": float(limit)}
+    except Exception:  # noqa: BLE001 -- no nvidia-smi: fall back to what the runtime reports
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+
+
+DUMP_BYTES = 60 << 20  # whole dump (kept under 64 MB); at most 8 MB per array
+DUMP_BYTES_PER_ARRAY = 8 << 20
+
+
+def dump_outputs(out: dict, path: str):
+    """Write what the timed path returned in its last step as DIR/<key>.npy (float64 outputs as float64, everything
+    else as float32).  An array larger than its share of DUMP_BYTES is replaced by a fixed, seeded sample of its rows,
+    so that two builds run with the same arguments can be compared output for output."""
+    import numpy as np
+
+    os.makedirs(path, exist_ok=True)
+    arrays = {k: v for k, v in sorted(out.items()) if isinstance(v, torch.Tensor) and (v.is_floating_point() or v.dtype in (torch.int32, torch.int64))}
+    cap = min(DUMP_BYTES_PER_ARRAY, DUMP_BYTES // max(1, len(arrays)))
+    written = {}
+    for k, v in arrays.items():
+        a = v.detach().to("cpu", torch.float64 if v.dtype == torch.float64 else torch.float32)
+        if a.dim() == 0:
+            a = a.reshape(1)
+        rows = a.shape[0]
+        row_bytes = max(1, a[0].numel() * a.element_size()) if rows else 1
+        if rows * row_bytes > cap:
+            keep = max(1, cap // row_bytes)
+            idx = torch.randperm(rows, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            a = a[idx]
+        np.save(os.path.join(path, f"{k}.npy"), a.numpy())
+        written[k] = list(a.shape)
+    return written
 
 
 # --------------------------------------------------------------------------------------
@@ -190,6 +231,7 @@ def run_ours(args, rank: int, world: int):
     torch.cuda.synchronize()
     ms = t0.elapsed_time(t1) / K
     launches = _lib.PROF.launches
+    dumped = dump_outputs(out, args.dump_outputs) if args.dump_outputs else None  # before later legs reuse the graph's buffers
     # ---- leg 2: same K steps with per-kernel CUDA events (roofline of the dominant kernel) ----
     _lib.PROF.reset()
     _lib.PROF.enabled = True
@@ -235,30 +277,16 @@ def run_ours(args, rank: int, world: int):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
     n_l = len(times[dom_tp]) / K
     avg_ms = per_kernel[dom_tp] / n_l
     bpe = algorithmic_bytes_per_edge(dom_tp, core)
     achieved = bpe * n_edges / (avg_ms * 1e-3) / 1e9
-    # DRAM traffic of that kernel from the latest committed `ncu --set full` capture (tools/ncu_summary.py writes
-    # profiles/ncu_traffic.json: dram__bytes_read.sum + dram__bytes_write.sum per launch, measured at the c2 shapes)
-    traffic = traffic_src = None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        pat = {"tp_bwd@bwd.L0": "tp_bwd3_kernel", "tp_fwd@fwd.L0": "tp_stream_kernel<float, float, 9, 9, 1, 0,",
-               "tp_bwd@bwd.L1": "tp_smem_kernel<float, float, 9, 1,",
-               "env_bwd@bwd.L0": "env_bwd_stream_kernel<float, 2,", "env_bwd@bwd.L1": "env_bwd_stream_kernel<float, 2,"}.get(dom_tp)
-        if cfg == "c2" and dtype == "float32" and pat:
-            for kname, rec in tj["per_kernel"].items():
-                if pat in kname:
-                    traffic = rec["dram_bytes_per_launch"]
-                    traffic_src = f"profiles/{tj['tag']}_ncu_full_summary.md ({tj['source']}: ncu --set full, dram__bytes_read+write per launch)"
-    except Exception:
-        pass
     roofline = {
         "kernel": dom_tp, "bound": "hbm", "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s",
-        "frac": round(achieved / peak, 4), "traffic": traffic, "traffic_source": traffic_src,
-        "launches_per_call": int(round(n_l)), "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)",
+        "frac": round(achieved / peak, 4),
+        "launches_per_call": int(round(n_l)),
+        "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "H100 SXM data sheet HBM3 bandwidth 3350 GB/s",
         "algorithmic_bytes_per_edge": bpe, "avg_launch_ms": round(avg_ms, 5), "share_of_kernel_time": round(per_kernel[dom_tp] / kernel_total, 4),
     }
     res = {
@@ -268,7 +296,8 @@ def run_ours(args, rank: int, world: int):
         "config": {"workload": f"{cfg}: {systems.CONFIGS[cfg]['system']}, {n_atoms} atoms, {n_edges} edges, l_max={kw['l_max']}, "
                                f"n_layers={kw['num_layers']}, S={kw['num_scalar_features']}, U={kw['num_tensor_features']}, r_max={kw['r_max']}",
                    "global_atoms": n_atoms, "parallelism": "1 GPU", "cuda_graph": graphed is not None, "timing": "CUDA events, inputs larger than L2 (per-step working set "
-                   f"~{n_edges * 5e3 / 1e9:.1f} GB >> 126 MB L2), neighbour list resident"},
+                   f"~{n_edges * 5e3 / 1e9:.1f} GB >> 50 MB L2), neighbour list resident"},
+        "gpu": gpu_info(dev.index or 0),
         "ns_per_day_at_1fs": 1e3 / ms * 0.0864,
         "clocks": clocks,
         "e2e": {"value": n_atoms * 1e3 / ms_e2e, "unit": UNIT, "ms_per_step": ms_e2e,
@@ -281,6 +310,8 @@ def run_ours(args, rank: int, world: int):
         "kernel_time_ms_per_step": round(kernel_total, 4),
         "dominant_kernel": dom,
     }
+    if dumped is not None:
+        res["dumped_outputs"] = {"dir": args.dump_outputs, "arrays": dumped}
     if not args.no_cpu_baseline:
         res["cpu_baseline"] = cpu_baseline(cfg, steps=3)
     print(json.dumps(res))
@@ -483,6 +514,7 @@ def _measure_multi(args, rank, world, dev, cfg, K, W):
                        "host_cpus_visible": len(os.sched_getaffinity(0))},
             "ns_per_day_at_1fs": 1e3 / ms * 0.0864,
             "clocks": clocks,
+            "gpu": gpu_info(dev.index or 0),
             "e2e": {"value": n_global * 1e3 / ms_e2e, "unit": UNIT, "ms_per_step": ms_e2e,
                     "h2d_bytes_per_step": pos_host.numel() * 8 * world, "d2h_bytes_per_step": (f_host.numel() * f_host.element_size() + 8) * world},
             "gpu_launches": launches,
@@ -563,9 +595,9 @@ def run_reference(args, rank: int, world: int):
 
 def run_reference_gpu(args, rank: int, world: int, triton: bool = False):
     """GPU baseline (SURVEY 8d "GPU reference baseline"): the oracle -- a plain-PyTorch restatement of the reference's
-    default path, autograd forces -- evaluated on one B200 at the full benchmark size, fp32, eager.  With ``triton``
-    every eligible Contracter is replaced by the reference's own TritonContracter (oracle/_ref, staged verbatim from
-    /root/reference by oracle/build_ref.py), i.e. the reference's accelerated inference path."""
+    default path, autograd forces -- evaluated on one GPU at the full benchmark size, fp32, eager.  With ``triton``
+    every eligible Contracter is replaced by the reference's own TritonContracter (oracle/_ref, staged from the
+    reference checkout by oracle/build_ref.py), i.e. the reference's accelerated inference path."""
     if rank != 0:
         return
     from allegro_b200 import data as D
@@ -613,9 +645,9 @@ def run_reference_gpu(args, rank: int, world: int, triton: bool = False):
     ms = t0.elapsed_time(t1) / K
     res = {"impl": args.impl, "metric": METRIC, "value": n * 1e3 / ms, "unit": UNIT, "n_gpus": 1, "steps": K, "warmup": W, "ms_per_step": ms,
            "higher_is_better": True, "dtype": "f32", "data": "synthetic",
-           "config": {"workload": f"{cfg}: {n} atoms, {e} edges (full size)", "what": "oracle/ (plain PyTorch restatement of the reference, autograd forces) on 1 B200, eager"
+           "config": {"workload": f"{cfg}: {n} atoms, {e} edges (full size)", "what": "oracle/ (plain PyTorch restatement of the reference, autograd forces) on 1 GPU, eager"
                       + (f", {swapped} Contracter(s) replaced by the reference's TritonContracter" if triton else ""),
-                      "peak_mem_gb": round(torch.cuda.max_memory_allocated() / 2**30, 1)}}
+                      "peak_mem_gb": round(torch.cuda.max_memory_allocated() / 2**30, 1)}, "gpu": gpu_info(dev.index or 0)}
     print(json.dumps(res))
 
 
@@ -625,19 +657,24 @@ def main():
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference", "reference-gpu", "reference-gpu-triton"],
-                    help="reference = CPU oracle (the driver's reference arm); reference-gpu(-triton) = the same oracle on the B200 "
+                    help="reference = CPU oracle; reference-gpu(-triton) = the same oracle on the GPU "
                          "(eager PyTorch; -triton swaps in the reference's own Triton tensor-product kernel staged under oracle/_ref): "
-                         "the GPU baseline of the >=10x target, NOT the driver's anchor")
+                         "the GPU baseline of the >=10x target")
     ap.add_argument("--config", default="c2")
     ap.add_argument("--dtype", default="float32", choices=["float64", "float32", "bfloat16"],
-                    help="activation storage; default float32 (GEMMs on tcgen05 as split-bf16, fp32-accurate): bfloat16 storage, the dtype BASELINE names for c2, measured 4e-3/4e-2 (E/F) against the fp64 oracle, outside the 1e-3 parity bar")
+                    help="activation storage; default float32 (GEMMs on wgmma as split-bf16, fp32-accurate): bfloat16 storage is the dtype BASELINE names for c2")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity-check", action="store_true", help="skip the pre-timing E/F check against the CPU oracle sub-sample")
     ap.add_argument("--halo", default="p2p", choices=["p2p", "nccl"], help="N>1: ghost-atom exchange over NVLink peer memory (default) or NCCL")
     ap.add_argument("--reps", type=int, default=0, help="N>1: lattice repetitions per box edge instead of the config's own (smaller boxes for tests)")
     ap.add_argument("--no-c4", action="store_true", help="N=8: skip the extra 1M-atom c4 measurement")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel from Python instead of replaying a CUDA graph")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="1 GPU: after the timed steps write the outputs of the last timed step as DIR/<name>.npy (float32 / float64; "
+                         "arrays over 8 MB as a fixed seeded row sample)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.gpus > 1 or args.impl != "ours"):
+        ap.error("--dump-outputs is supported for the single-GPU run of this framework")
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
     if args.impl == "reference":

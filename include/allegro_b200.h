@@ -1,4 +1,4 @@
-/* allegro_b200 C ABI -- B200 (sm_100a) kernels for Allegro's per-edge hot path.
+/* allegro_b200 C ABI -- H100 (sm_90a) kernels for Allegro's per-edge hot path.
  *
  * The reference (mir-group/allegro v0.7.1) is pure Python; its "FFI" for this path is the
  * kernel plug-in point Contracter.forward(x1, x2, idxs, scatter_dim_size)
@@ -36,11 +36,11 @@ enum { AB2_EPI_NONE = 0, AB2_EPI_MUL_DSILU = 1 };
 
 const char* ab2_last_error(void);
 int ab2_version(void);
-/* 1 if a CUDA device with compute capability 10.x is current, else 0 (no error). */
+/* 1 if a CUDA device with compute capability 9.0 is current, else 0 (no error). */
 int ab2_device_ok(void);
 /* Kernel-selection switches (for A/B tests and tuning; process-global, not thread-safe):
  *   "tp_fast"    1 shared-memory / register-tiled tensor product (default), 2 register-M variants, 0 shape-generic kernels
- *   "linear_tc"  1 tcgen05 tensor-core linear (default), 0 CUDA-core tile kernel
+ *   "linear_tc"  1 wgmma tensor-core linear (default), 0 CUDA-core tile kernel
  *   "tp_variant" 1: 3 CTAs/SM (default), 0: 2 CTAs/SM for the shared-memory tensor-product kernel
  *   "tp_stream"  1 TMA-staged streaming tensor product where instantiated (default), 0 round-1 kernels;
  *                "tp_stream_te" edges per stage (0 = 8), "tp_stream_cps" cap on CTAs per SM (0 = occupancy limit),
@@ -51,7 +51,7 @@ int ab2_device_ok(void);
  *   "env_stream" 1 streaming adjoint of the environment sum (default), 0 round-1 kernel
  *   "linear_tma" 1 TMA-producer variant of the tensor-core linear where eligible (default), 0 cp.async producers
  *   "env_split"  warps per (centre, channel chunk) in ab2_env_sum / ab2_env_bwd: 0 auto (default), 1, 2, 4
- *   "tc_debug"   stage knock-out mask of the tcgen05 linear (bit0 no stores, bit1 no loads, bit2 no MMA); results are
+ *   "tc_debug"   stage knock-out mask of the wgmma linear (bit0 no stores, bit1 no loads, bit2 no MMA); results are
  *                wrong when non-zero -- for tools/exp_env.py only
  * Returns 1 (and sets ab2_last_error) for an unknown key. */
 int ab2_set_option(const char* key, int value);
@@ -110,15 +110,15 @@ int ab2_linear(int dtype, int64_t M, int K, int N, int n_a, const void* const* a
                const int64_t* a_ld_host, const int32_t* a_width_host,
                const void* const* a_aux_ptr_host /* nullable */, const int64_t* a_aux_ld_host,
                int act, const void* W,
-               const void* W_packed /* nullable: image from ab2_linear_pack -> tcgen05 path */,
+               const void* W_packed /* nullable: image from ab2_linear_pack -> wgmma path */,
                int n_o, void* const* o_ptr_host, const int64_t* o_ld_host,
                const int32_t* o_width_host, const int32_t* o_accum_host, int epi, const void* aux,
                int64_t aux_ld, void* stream);
 
-/* Tensor-core (tcgen05) path of ab2_linear.  ab2_linear_packed_bytes returns the size of the
- * packed weight image (bf16 hi + lo parts in the UMMA canonical K-major core-matrix layout) or 0
+/* Tensor-core (wgmma) path of ab2_linear.  ab2_linear_packed_bytes returns the size of the
+ * packed weight image (bf16 hi + lo parts in the GMMA canonical K-major core-matrix layout) or 0
  * if (dtype, K, N) is not eligible (fp64, K % 16 != 0, K > 512); ab2_linear_pack builds it on the
- * device from W[K][N].  Any N is accepted: outputs wider than 256 columns, or whose W image does not
+ * device from W[K][N].  Any N is accepted: outputs wider than 128 columns, or whose W image does not
  * fit the shared-memory budget (128 KB), run as column slices (one launch per slice, W slice resident).
  * With fp32 storage the kernel computes A_hi W_hi + A_lo W_hi + A_hi W_lo in bf16 MMAs with fp32
  * accumulation (~2^-16 relative). */

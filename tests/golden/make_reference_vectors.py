@@ -10,10 +10,12 @@ exactly what that does and does not pin).  The reference's package `__init__` (w
 nequip-compile tooling) is bypassed by registering a bare parent package; every `allegro.nn` /
 `allegro.model` module is executed as is.
 
-Outputs (committed, small):
-  tests/golden/ref_models.pt   whole-model cases: ctor kwargs, inputs, reference state_dict, outputs
-  tests/golden/ref_ops.pt      operator cases: Contracter / MakeWeightedChannels inputs+outputs,
-                               per-layer irreps of Allegro_Module for a grid of (l_max, parity, L)
+Outputs (committed, each shard under 1 MB; tests/golden_util.py loads them):
+  tests/golden/ref_models.<i>.pt   whole-model cases: ctor kwargs, inputs, reference state_dict, outputs
+  tests/golden/ref_ops.<i>.pt      operator cases: Contracter / MakeWeightedChannels inputs+outputs,
+                                   per-layer irreps of Allegro_Module for a grid of (l_max, parity, L)
+  tests/golden/ref_modifier.pt     one model built by the reference's AllegroModel: kwargs, state_dict and the
+                                   constructor state of every Contracter (tests/test_reference_modifier.py)
 """
 import os
 import sys
@@ -25,6 +27,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 REF = "/root/reference"
 sys.path.insert(0, os.path.join(HERE, "_stubs"))
+sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 
 if not os.path.isdir(os.path.join(REF, "allegro")):
@@ -40,6 +43,7 @@ from e3nn.o3 import Irreps  # noqa: E402  (stand-in)
 
 from allegro_b200 import data as D  # noqa: E402
 from allegro_b200 import systems  # noqa: E402
+from golden_util import save_sharded  # noqa: E402
 
 BESSEL = {"_target_": "allegro.nn.TwoBodyBesselScalarEmbed", "num_bessels": 8, "polynomial_cutoff_p": 6}
 
@@ -150,7 +154,7 @@ def run_models():
         out.append(rec)
         print(f"{name:28s} atoms {data['pos'].shape[0]:3d} edges {data['edge_index'].shape[1]:5d} E {float(res['total_energy']):+.6f} "
               f"max|F| {float(res['forces'].abs().max()):.4f}")
-    torch.save(out, os.path.join(HERE, "ref_models.pt"))
+    save_sharded(out, "ref_models")
 
 
 def run_ops():
@@ -209,12 +213,28 @@ def run_ops():
                                          int((tp.w3j != 0).sum()), bool(tp.w3j_is_ij_diagonal)) for tp in am.tps],
                                    latent_dims=[tuple(int(w.shape[0]) for w in lat.weights) + (int(lat.weights[-1].shape[1]),) for lat in am.latents]))
     torch.set_default_dtype(prev)
-    torch.save(dict(contracter=contract, channels=channels, layers=layers), os.path.join(HERE, "ref_ops.pt"))
+    save_sharded(dict(contracter=contract, channels=channels, layers=layers), "ref_ops")
     print(f"operators: {len(contract)} Contracter, {len(channels)} MakeWeightedChannels, {len(layers)} layer-irreps cases")
+
+
+def run_modifier():
+    kw = dict(seed=3, model_dtype="float64", r_max=4.0, type_names=["H", "C", "O"], l_max=2, num_layers=3, num_scalar_features=16,
+              num_tensor_features=4, avg_num_neighbors=20.0, radial_chemical_embed={"_target_": "allegro.nn.TwoBodyBesselScalarEmbed"})
+    model = allegro.model.AllegroModel(**kw)
+    tps = list(model.model.allegro.tps)
+    assert all(type(tp) is Contracter for tp in tps)
+    rec = dict(kwargs=kw, state_dict=pack_state_dict(model.model.state_dict()),
+               tps=[dict(irreps=(repr(a.irreps_in1), repr(a.irreps_in2), repr(a.irreps_out)), mul=a.mul, num_paths=a.num_paths,
+                         path_channel_coupling=a.path_channel_coupling, scatter_factor=a.scatter_factor,
+                         w3j_is_ij_diagonal=bool(a.w3j_is_ij_diagonal)) for a in tps])
+    torch.save(rec, os.path.join(HERE, "ref_modifier.pt"))
+    print(f"modifier: {len(tps)} Contracter")
 
 
 if __name__ == "__main__":
     run_models()
     run_ops()
-    for f in ("ref_models.pt", "ref_ops.pt"):
-        print(f, os.path.getsize(os.path.join(HERE, f)) // 1024, "KiB")
+    run_modifier()
+    for f in sorted(os.listdir(HERE)):
+        if f.endswith(".pt"):
+            print(f, os.path.getsize(os.path.join(HERE, f)) // 1024, "KiB")

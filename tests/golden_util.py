@@ -1,5 +1,7 @@
 """Loading helpers for the reference-generated fixtures under tests/golden/ (see
 tests/golden/make_reference_vectors.py for how they were produced)."""
+import glob
+import io
 import os
 
 import torch
@@ -20,12 +22,52 @@ def unpack_state_dict(sd):
     return out
 
 
+SHARD_BYTES = 900_000  # every fixture file stays under 1 MB
+
+
+def save_sharded(obj, stem):
+    """Write a list of records (or a dict of such lists) as tests/golden/<stem>.<i>.pt shards of at most SHARD_BYTES each;
+    load_sharded(stem) restores the object."""
+    items = [(k, r) for k, v in obj.items() for r in v] if isinstance(obj, dict) else [(None, r) for r in obj]
+
+    def pack(part):
+        if isinstance(obj, dict):
+            return {k: [r for kk, r in part if kk == k] for k in obj}
+        return [r for _, r in part]
+
+    def nbytes(part):
+        buf = io.BytesIO()
+        torch.save(pack(part), buf)
+        return buf.tell()
+
+    for f in glob.glob(os.path.join(GOLDEN, f"{stem}.*.pt")):
+        os.remove(f)
+    shards, cur = [], []
+    for it in items:
+        if cur and nbytes(cur + [it]) > SHARD_BYTES:
+            shards.append(cur)
+            cur = []
+        cur.append(it)
+    shards.append(cur)
+    for i, part in enumerate(shards):
+        torch.save(pack(part), os.path.join(GOLDEN, f"{stem}.{i}.pt"))
+    return len(shards)
+
+
+def load_sharded(stem):
+    files = sorted(glob.glob(os.path.join(GOLDEN, f"{stem}.*.pt")), key=lambda f: int(f.rsplit(".", 2)[1]))
+    parts = [torch.load(f, weights_only=False) for f in files]
+    if isinstance(parts[0], dict):
+        return {k: [r for p in parts for r in p[k]] for k in parts[0]}
+    return [r for p in parts for r in p]
+
+
 def load_models():
-    return torch.load(os.path.join(GOLDEN, "ref_models.pt"), weights_only=False)
+    return load_sharded("ref_models")
 
 
 def load_ops():
-    return torch.load(os.path.join(GOLDEN, "ref_ops.pt"), weights_only=False)
+    return load_sharded("ref_ops")
 
 
 def model_case_ids():

@@ -1,4 +1,4 @@
-"""CPU tests: the C-ABI library builds for sm_100a, loads, and exports every symbol that
+"""CPU tests: the C-ABI library builds for sm_90a, loads, and exports every symbol that
 include/allegro_b200.h declares (no compute calls without a GPU); host-side packing logic."""
 import ctypes
 import os

@@ -97,7 +97,7 @@ def test_linear_concat_split_act_epi(dtype, shape):
 @pytest.mark.parametrize("mode", ["plain", "silu_in", "dsilu_epi_accum"])
 @pytest.mark.parametrize("tma", [1, 0], ids=["tma", "cpasync"])
 def test_linear_tensor_core_path(dtype, shape, mode, tma):
-    """tcgen05 path (16-byte aligned segments, K % 16 == 0) against an fp64 reference and against
+    """wgmma path (16-byte aligned segments, K % 16 == 0) against an fp64 reference and against
     the CUDA-core kernel.  fp32 storage uses the 3-term bf16 split: held to 1e-4 (measured ~1e-5)."""
     M, awid, owid = shape
     K, N = sum(awid), sum(owid)

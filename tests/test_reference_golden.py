@@ -1,6 +1,6 @@
 """Oracle and product host logic against vectors produced by the REFERENCE'S OWN CODE.
 
-tests/golden/ref_models.pt / ref_ops.pt were written by tests/golden/make_reference_vectors.py, which
+tests/golden/ref_models.*.pt / ref_ops.*.pt were written by tests/golden/make_reference_vectors.py, which
 executes the unmodified /root/reference allegro/nn + allegro/model modules (third-party e3nn / nequip
 calls resolved to stand-ins backed by the oracle's primitives, tests/golden/_stubs/README.md).  These
 tests therefore pin the oracle's restatement -- and the product's table / irreps / state_dict logic --

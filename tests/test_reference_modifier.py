@@ -1,68 +1,48 @@
-"""The kernel plug-in point on the REAL reference classes (build container only: needs /root/reference; skipped elsewhere).
+"""The kernel plug-in point applied to a whole model, pinned to what the reference's own model builder produced.
 
 `Contracter.enable_B200Contracter(model)` is the analogue of the reference's `enable_TritonContracter` /
-`enable_CuEquivarianceContracter` model modifiers (allegro/nn/_strided/_contract.py:253-310).  Here it is applied to a
-model assembled by the reference's own builders (third-party imports resolved to tests/golden/_stubs): every
-`allegro.nn._strided._contract.Contracter` must be replaced by the B200 operator with identical constructor state and
-`state_dict`, and nothing else may change.  (The forward of the replaced operator needs a GPU: tests/test_zx_gpu_reference_golden.py.)
+`enable_CuEquivarianceContracter` model modifiers (allegro/nn/_strided/_contract.py:253-310).  tests/golden/ref_modifier.pt
+records, for one model built by the reference's own `AllegroModel` (third-party imports resolved to tests/golden/_stubs),
+its constructor kwargs, its `state_dict` and the constructor state of every `Contracter` in it.  The same model is
+assembled here from the oracle's restatement and loaded with the reference's `state_dict`; every `Contracter` must be
+replaced by the B200 operator with the reference's constructor state and `state_dict`, and nothing else may change.
+(The forward of the replaced operator needs a GPU: tests/test_zx_gpu_reference_golden.py.)
 """
 import os
-import sys
-import types
 
 import pytest
 import torch
 
-REF = "/root/reference"
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "allegro")), reason="reference checkout not present")
+from golden_util import GOLDEN, unpack_state_dict
 
 
-@pytest.fixture()
-def reference_allegro():
-    here = os.path.dirname(os.path.abspath(__file__))
-    stubs = os.path.join(here, "golden", "_stubs")
-    saved_path, saved_mods = list(sys.path), {k: v for k, v in sys.modules.items() if k.split(".")[0] in ("allegro", "e3nn", "nequip", "hydra")}
-    sys.path.insert(0, stubs)
-    pkg = types.ModuleType("allegro")
-    pkg.__path__ = [os.path.join(REF, "allegro")]
-    sys.modules["allegro"] = pkg
-    try:
-        import allegro.model
-        import allegro.nn  # noqa: F401
-
-        yield allegro
-    finally:
-        sys.path[:] = saved_path
-        for k in [k for k in sys.modules if k.split(".")[0] in ("allegro", "e3nn", "nequip", "hydra")]:
-            del sys.modules[k]
-        sys.modules.update(saved_mods)
-
-
-def test_enable_b200_contracter_on_reference_model(reference_allegro):
-    from allegro.nn._strided import Contracter as RefContracter  # the reference class
-
+def test_enable_b200_contracter_on_reference_model():
     from allegro_b200.nn import B200Contracter
+    from oracle import nn_ref as R
+    from oracle.model_ref import AllegroOracle
 
-    model = reference_allegro.model.AllegroModel(
-        seed=3, model_dtype="float64", r_max=4.0, type_names=["H", "C", "O"], l_max=2, num_layers=3, num_scalar_features=16,
-        num_tensor_features=4, avg_num_neighbors=20.0, radial_chemical_embed={"_target_": "allegro.nn.TwoBodyBesselScalarEmbed"})
+    rec = torch.load(os.path.join(GOLDEN, "ref_modifier.pt"), weights_only=False)
+    ref_sd = unpack_state_dict(rec["state_dict"])
+    model = AllegroOracle(**rec["kwargs"])
+    model.model.load_state_dict(ref_sd, strict=True)
     before = {k: v.clone() for k, v in model.state_dict().items()}
     old = list(model.model.allegro.tps)
-    assert all(type(tp) is RefContracter for tp in old)
+    assert len(old) == len(rec["tps"]) and all(type(tp) is R.Contracter for tp in old)
     out = B200Contracter.enable_B200Contracter(model)
     assert out is model
     new = list(model.model.allegro.tps)
     assert len(new) == len(old) and all(isinstance(tp, B200Contracter) for tp in new)
-    for a, b in zip(old, new):
-        assert (repr(a.irreps_in1), repr(a.irreps_in2), repr(a.irreps_out)) == (repr(b.irreps_in1), repr(b.irreps_in2), repr(b.irreps_out))
-        assert (a.mul, a.num_paths, a.path_channel_coupling, a.scatter_factor, bool(a.w3j_is_ij_diagonal)) == (
-            b.mul, b.num_paths, b.path_channel_coupling, b.scatter_factor, bool(b.w3j_is_ij_diagonal))
-        assert b.w3j.dtype == a.w3j.dtype and torch.equal(b.w3j, a.w3j) and torch.equal(b.weights, a.weights)
+    for i, (ref, b) in enumerate(zip(rec["tps"], new)):
+        assert (repr(b.irreps_in1), repr(b.irreps_in2), repr(b.irreps_out)) == tuple(ref["irreps"])
+        assert (b.mul, b.num_paths, b.path_channel_coupling, b.scatter_factor, bool(b.w3j_is_ij_diagonal)) == (
+            ref["mul"], ref["num_paths"], ref["path_channel_coupling"], ref["scatter_factor"], ref["w3j_is_ij_diagonal"])
+        w3j, weights = ref_sd[f"allegro.tps.{i}.w3j"], ref_sd[f"allegro.tps.{i}.weights"]
+        assert b.w3j.dtype == w3j.dtype and torch.equal(b.w3j, w3j) and torch.equal(b.weights, weights)
     after = model.state_dict()
     assert list(after.keys()) == list(before.keys())
     assert all(torch.equal(after[k], before[k]) for k in before)
-    # every other module of the reference model is untouched
-    assert type(model.model.allegro).__module__ == "allegro.nn._allegro"
+    # every other module of the model is untouched
+    assert type(model.model.allegro) is R.Allegro_Module
     # the replaced operator refuses CPU tensors instead of silently falling back
     tp = new[0]
     with pytest.raises(RuntimeError):

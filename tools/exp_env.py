@@ -60,7 +60,7 @@ print(f"read  (sum)   {GB / timeit(lambda: x.sum(), 10) * 1e6:7.0f} GB/s", flush
 print(f"copy  (r+w)   {2 * GB / timeit(lambda: y.copy_(x), 10) * 1e6:7.0f} GB/s", flush=True)
 del x, y
 
-# ---- tcgen05 linear stage knock-outs (fp32 split path) ----
+# ---- wgmma linear stage knock-outs (fp32 split path) ----
 M = 461154
 for awid, owid in (([64], [96, 64, 96]), ([64, 64, 64], [64]), ([64], [64]), ([128], [128])):
     K, N = sum(awid), sum(owid)

@@ -1,6 +1,6 @@
 """Per-op roofline table from a bench.py JSON line (its `kernels_ms_per_step` leg) -- post-processing only.
 
-    python tools/roofline_table.py profiles/r1k_bench_f32.json [--peak 6584.8]
+    python tools/roofline_table.py bench_line.json [--peak 3350]
 
 Algorithmic bytes are the unavoidable global traffic of each op of the per-kernel pipeline (DESIGN.md section 4):
 inputs read once, outputs written once, in the storage dtype; epilogue operands (silu' pre-activations, accumulated

@@ -1,5 +1,5 @@
 """GPU baseline for SURVEY row a13: the REFERENCE's own Triton tensor-product kernel (oracle/_ref/ref_triton, staged
-verbatim from /root/reference by oracle/build_ref.py) timed next to this package's kernels on the same B200, same
+verbatim from the reference checkout by oracle/build_ref.py) timed next to this package's kernels on the same GPU, same
 shapes (c2 layer 0: E = 460 992 edges, U = 32, 9 x 9 -> 9), plus a parity check between the two.
 
 What is compared

@@ -1,10 +1,10 @@
-// Micro-benchmarks that size the streaming kernels of allegro_b200 (run on the GPU box through gpurun):
+// Micro-benchmarks that size the streaming kernels of allegro_b200 :
 //   bulk   : persistent CTAs, ONE producer thread issuing cp.async.bulk (global -> shared, mbarrier complete_tx)
 //            into a ring of NS stages of CH bytes; NC consumer warps read every byte from shared memory.
 //            -> achievable HBM read rate of a "TMA-staged CSR row" pipeline vs stage size / depth / CTAs per SM.
 //   ldg    : plain coalesced LDG.128 streaming with U independent loads in flight per thread.
-//   ffma   : FFMA vs FFMA2 (fma.rn.f32x2) issue throughput per SM.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o tools/ubench/ubench tools/ubench/ubench.cu
+//   ffma   : FFMA issue throughput per SM.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o tools/ubench/ubench tools/ubench/ubench.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -112,7 +112,6 @@ __global__ void __launch_bounds__(256) ldg_kernel(const float4* __restrict__ src
 }
 
 // dependent-chain-free FMA loops: 16 independent accumulators (8 pairs)
-template <bool PACKED>
 __global__ void __launch_bounds__(256) ffma_kernel(float* out, int iters, float a, float b) {
     float2 acc[8];
 #pragma unroll
@@ -121,15 +120,8 @@ __global__ void __launch_bounds__(256) ffma_kernel(float* out, int iters, float 
     for (int it = 0; it < iters; ++it) {
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-            if (PACKED) {
-                unsigned long long r, x = *reinterpret_cast<unsigned long long*>(&acc[i]), y = *reinterpret_cast<unsigned long long*>(&m),
-                                      z = *reinterpret_cast<unsigned long long*>(&c);
-                asm volatile("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(x), "l"(y), "l"(z));
-                acc[i] = *reinterpret_cast<float2*>(&r);
-            } else {
-                asm volatile("fma.rn.f32 %0, %0, %1, %2;" : "+f"(acc[i].x) : "f"(m.x), "f"(c.x));
-                asm volatile("fma.rn.f32 %0, %0, %1, %2;" : "+f"(acc[i].y) : "f"(m.y), "f"(c.y));
-            }
+            asm volatile("fma.rn.f32 %0, %0, %1, %2;" : "+f"(acc[i].x) : "f"(m.x), "f"(c.x));
+            asm volatile("fma.rn.f32 %0, %0, %1, %2;" : "+f"(acc[i].y) : "f"(m.y), "f"(c.y));
         }
     }
     float s = 0.f;
@@ -205,21 +197,17 @@ int main() {
         run(bulk_kernel<6>, 6, 1536, 4, 4);
         run(bulk_kernel<6>, 6, 1536, 4, 8);
     }
-    // ---- FFMA vs FFMA2 ----
+    // ---- FFMA ----
     {
         const int iters = 4096;
-        for (int packed = 0; packed < 2; ++packed) {
-            for (int r = 0; r < 3; ++r) {
-                CK(cudaEventRecord(e0));
-                if (packed) ffma_kernel<true><<<nsm * 8, 256>>>(out, iters, 1.0001f, 0.5f);
-                else ffma_kernel<false><<<nsm * 8, 256>>>(out, iters, 1.0001f, 0.5f);
-                CK(cudaEventRecord(e1));
-                CK(cudaEventSynchronize(e1));
-            }
-            const double fma = (double)nsm * 8 * 256 * iters * 16;
-            printf("%s : %.1f TFMA/s (%.1f FMA/clk/SM at 1.9 GHz)\n", packed ? "FFMA2" : "FFMA ", fma / time_ms(e0, e1) / 1e9,
-                   fma / time_ms(e0, e1) / 1e3 / nsm / 1.9e6);
+        for (int r = 0; r < 3; ++r) {
+            CK(cudaEventRecord(e0));
+            ffma_kernel<<<nsm * 8, 256>>>(out, iters, 1.0001f, 0.5f);
+            CK(cudaEventRecord(e1));
+            CK(cudaEventSynchronize(e1));
         }
+        const double fma = (double)nsm * 8 * 256 * iters * 16;
+        printf("FFMA : %.1f TFMA/s (%.1f FMA/clk/SM at 1.98 GHz)\n", fma / time_ms(e0, e1) / 1e9, fma / time_ms(e0, e1) / 1e3 / nsm / 1.98e6);
     }
     return 0;
 }
