@@ -16,6 +16,7 @@ from . import build as _build
 AB2_F64, AB2_F32, AB2_BF16 = 0, 1, 2
 ACT_NONE, ACT_SILU, ACT_MUL_DSILU = 0, 1, 2
 EPI_NONE, EPI_MUL_DSILU = 0, 1
+NOT_ELIGIBLE = -1
 MAX_SEG = 4
 
 DTYPE_ENUM = {torch.float64: AB2_F64, torch.float32: AB2_F32, torch.bfloat16: AB2_BF16}
@@ -39,6 +40,7 @@ _SIGNATURES = {
     "ab2_linear": ([_i32, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _i64, _vp], C.c_int),
     "ab2_linear_packed_bytes": ([_i32, _i32, _i32], C.c_int64),
     "ab2_linear_pack": ([_i32, _i32, _i32, _vp, _vp, _vp], C.c_int),
+    "ab2_mlp2": ([_i32, _i32, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_env_sum": ([_i32, _i32, _i64, _i32, _vp, _vp, _vp, _i64, _dbl, _vp, _vp], C.c_int),
     "ab2_env_bwd": ([_i32, _i32, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _i64, _vp, _dbl, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_tp_fwd": ([_i32, _i32, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp], C.c_int),
@@ -152,6 +154,15 @@ class _timed:
             self.ev[1].record()
             PROF.records.setdefault(self.name + "@" + _TAG[0], []).append(self.ev)
         return False
+
+    def cancel(self):
+        """After the block: the call launched nothing (the kernel declined the case), so it is not counted."""
+        PROF.launches -= self.n
+        if PROF.enabled:
+            key = self.name + "@" + _TAG[0]
+            PROF.records[key].pop()
+            if not PROF.records[key]:
+                del PROF.records[key]
 
 
 def set_option(key: str, value: int):
@@ -269,6 +280,64 @@ def linear(
                 _ptr(aux), aux_ld, _stream(),
             )
         )
+
+
+def mlp2(
+    a_segs: Sequence[torch.Tensor],
+    W1: torch.Tensor,
+    W2: torch.Tensor,
+    o_segs: Sequence[torch.Tensor],
+    pre: torch.Tensor,
+    o_accum: Optional[Sequence[bool]] = None,
+    backward: bool = False,
+    W1_packed: Optional[torch.Tensor] = None,
+    W2_packed: Optional[torch.Tensor] = None,
+) -> bool:
+    """Two-layer SiLU MLP in one kernel (ab2_mlp2), A = cat(a_segs, -1):
+    forward   pre = A @ W1 (written),  Out (+)= silu(pre) @ W2;
+    backward  Out (+)= ((A @ W1) * silu'(pre)) @ W2   (A = Gout, W1 = W2_fwd^T, W2 = W1_fwd^T).
+    A one-column backward (K = 1) takes W1 as it is (rank-1 first stage, no packed image).
+    Returns False, with nothing computed, when the kernel does not take this case: the caller then runs two ``linear``
+    calls."""
+    M = a_segs[0].shape[0]
+    K, H = W1.shape
+    N = W2.shape[1]
+    dt = W1.dtype
+    rank1 = backward and K == 1
+    if W2_packed is None or (W1_packed is None and not rank1):
+        return False
+    na, no = len(a_segs), len(o_segs)
+    a_ptr = (C.c_void_p * na)()
+    a_ld = (C.c_int64 * na)()
+    a_w = (C.c_int32 * na)()
+    for s, t in enumerate(a_segs):
+        t, ld = _row_strided(t, f"A segment {s}") if t.shape[1] > 1 else (t, int(t.stride(0)))
+        assert t.dtype == dt and t.shape[0] == M
+        a_ptr[s], a_ld[s], a_w[s] = t.data_ptr(), ld, t.shape[1]
+        _ptr(t)
+    o_ptr = (C.c_void_p * no)()
+    o_ld = (C.c_int64 * no)()
+    o_w = (C.c_int32 * no)()
+    o_acc = (C.c_int32 * no)()
+    for s, t in enumerate(o_segs):
+        t, ld = _row_strided(t, f"output segment {s}")
+        assert t.dtype == dt and t.shape[0] == M
+        o_ptr[s], o_ld[s], o_w[s] = t.data_ptr(), ld, t.shape[1]
+        o_acc[s] = int(bool(o_accum[s])) if o_accum is not None else 0
+        _ptr(t)
+    pre, pre_ld = _row_strided(pre, "pre")
+    assert pre.dtype == dt and tuple(pre.shape) == (M, H)
+    timer = _timed("mlp2", 1)
+    with timer:
+        rc = load().ab2_mlp2(
+            DTYPE_ENUM[dt], int(backward), M, K, H, N, na, a_ptr, a_ld, a_w, _ptr(W1_packed), _ptr(W2_packed),
+            _ptr(_contig(W1, "W1")) if rank1 else None, _ptr(pre), pre_ld, no, o_ptr, o_ld, o_w, o_acc, _stream(),
+        )
+    if rc == NOT_ELIGIBLE:
+        timer.cancel()
+        return False
+    _check(rc)
+    return True
 
 
 def linear_pack(W: torch.Tensor) -> Optional[torch.Tensor]:

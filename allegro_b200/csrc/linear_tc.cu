@@ -161,6 +161,9 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[16 * NCH], uint64_t da, ui
 __device__ __forceinline__ void cp_async16(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
 }
+__device__ __forceinline__ void cp_async4(uint32_t dst_smem, const void* src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst_smem), "l"(src) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
@@ -304,53 +307,76 @@ struct TcCtx {
 // =============================== consumers (2 warpgroups: wgmma + epilogue) ===============================
 // cw: consumer warp 0..7; warpgroup cw / 4 owns rows [64 (cw / 4), 64 (cw / 4) + 64) of each tile, warp cw % 4 of it
 // holds the accumulator rows [16 (cw % 4), 16 (cw % 4) + 16) of that half.
-template <typename TSrc, bool SPLIT, int NCH>
-__device__ __forceinline__ void tc_consumer_role(const TcParams& p, const TcCtx& c, int cw, int lane) {
-    const int wg = cw >> 2, w4 = cw & 3;
+
+// Main loop fed by the ring: acc = A (p.K columns, canonical ring stages) @ W (resident at c.sW).  Each ring slot is
+// released once the wgmma group that read it has retired; stage / phase carry the ring position across tiles.
+template <bool SPLIT, int NCH>
+__device__ __forceinline__ void tc_mma_ring(float (&acc)[16 * NCH], const TcParams& p, const TcCtx& c, int wg, int lane, int& stage,
+                                            uint32_t& phase) {
     const int nkb = c.nkb, stage_bytes = c.stage_bytes, w_half = c.w_half;
     const uint32_t sW_u = smem_u32(c.sW);
     const uint32_t w_sbo = (uint32_t)(p.K / 8) * 128;  // bytes between 8-column (n) groups of W
     constexpr uint32_t A_SBO = (KC / 8) * 128;         // bytes between 8-row groups of a stage
-    float* stg = c.sEpi + cw * 16 * EPI_LD;
-    int stage = 0;
-    uint32_t phase = 0;
-    float acc[16 * NCH];
-    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        int prev = -1;
-        for (int kb = 0; kb < nkb; ++kb) {
-            mbar_wait(c.full_bar(stage), phase);
-            wgmma_fence();
-            const uint32_t a_hi = smem_u32(c.sA + stage * stage_bytes) + (uint32_t)wg * 8 * A_SBO;
-            const int ksteps = min(2, (p.K - kb * KC) / 16);
-            for (int ks = 0; ks < ((p.debug & 4) ? 0 : ksteps); ++ks) {
-                const uint64_t da_hi = make_desc(a_hi + ks * 256, 128, A_SBO);
-                const uint32_t wk = sW_u + (uint32_t)(kb * (KC / 8) + ks * 2) * 128;
-                const uint64_t db_hi = make_desc(wk, 128, w_sbo);
-                wgmma_bf16<NCH>(acc, da_hi, db_hi, (kb | ks) ? 1u : 0u);
-                if constexpr (SPLIT) {
-                    const uint64_t da_lo = make_desc(a_hi + STAGE_HALF + ks * 256, 128, A_SBO);
-                    const uint64_t db_lo = make_desc(wk + w_half, 128, w_sbo);
-                    wgmma_bf16<NCH>(acc, da_lo, db_hi, 1u);
-                    wgmma_bf16<NCH>(acc, da_hi, db_lo, 1u);
-                }
+    int prev = -1;
+    for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(c.full_bar(stage), phase);
+        wgmma_fence();
+        const uint32_t a_hi = smem_u32(c.sA + stage * stage_bytes) + (uint32_t)wg * 8 * A_SBO;
+        const int ksteps = min(2, (p.K - kb * KC) / 16);
+        for (int ks = 0; ks < ((p.debug & 4) ? 0 : ksteps); ++ks) {
+            const uint64_t da_hi = make_desc(a_hi + ks * 256, 128, A_SBO);
+            const uint32_t wk = sW_u + (uint32_t)(kb * (KC / 8) + ks * 2) * 128;
+            const uint64_t db_hi = make_desc(wk, 128, w_sbo);
+            wgmma_bf16<NCH>(acc, da_hi, db_hi, (kb | ks) ? 1u : 0u);
+            if constexpr (SPLIT) {
+                const uint64_t da_lo = make_desc(a_hi + STAGE_HALF + ks * 256, 128, A_SBO);
+                const uint64_t db_lo = make_desc(wk + w_half, 128, w_sbo);
+                wgmma_bf16<NCH>(acc, da_lo, db_hi, 1u);
+                wgmma_bf16<NCH>(acc, da_hi, db_lo, 1u);
             }
-            wgmma_commit();
-            // the group of the previous k block has retired: its ring slot is free (this one stays in flight)
-            if (prev >= 0) {
-                wgmma_wait<1>();
-                if (lane == 0) mbar_arrive(c.empty_bar(prev));
-            }
-            prev = stage;
-            if (++stage == p.nstage) { stage = 0; phase ^= 1; }
         }
-        wgmma_wait<0>();
-        if (lane == 0 && prev >= 0) mbar_arrive(c.empty_bar(prev));
-        if (p.debug & 4) {
+        wgmma_commit();
+        // the group of the previous k block has retired: its ring slot is free (this one stays in flight)
+        if (prev >= 0) {
+            wgmma_wait<1>();
+            if (lane == 0) mbar_arrive(c.empty_bar(prev));
+        }
+        prev = stage;
+        if (++stage == p.nstage) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    if (lane == 0 && prev >= 0) mbar_arrive(c.empty_bar(prev));
+    if (p.debug & 4) {
 #pragma unroll
-            for (int j = 0; j < 16 * NCH; ++j) acc[j] = 0.f;
-        }
+        for (int j = 0; j < 16 * NCH; ++j) acc[j] = 0.f;
+    }
+}
 
-        // ---- epilogue: this warp's 16 rows, one 32-column chunk at a time ----
+// Main loop from a resident operand: acc = A (this warpgroup's 64 x K tile at a_u, bf16 hi image, lo image a_half bytes
+// further) @ W (K x 32 NCH image at w_u, lo image w_half bytes further), both canonical K-major.  The k16 steps and the
+// three split-bf16 products run in the same order as in tc_mma_ring, so the result is bitwise that of the ring-fed loop.
+template <int NCH>
+__device__ __forceinline__ void tc_mma_resident(float (&acc)[16 * NCH], uint32_t a_u, uint32_t a_half, int K, uint32_t w_u, uint32_t w_half) {
+    const uint32_t sbo = (uint32_t)(K / 8) * 128;  // A rows and W columns: 8-groups K / 8 core matrices apart
+    wgmma_fence();
+    for (int ks = 0; ks < K / 16; ++ks) {
+        const uint64_t da_hi = make_desc(a_u + ks * 256, 128, sbo), da_lo = make_desc(a_u + a_half + ks * 256, 128, sbo);
+        const uint64_t db_hi = make_desc(w_u + ks * 256, 128, sbo), db_lo = make_desc(w_u + w_half + ks * 256, 128, sbo);
+        wgmma_bf16<NCH>(acc, da_hi, db_hi, ks ? 1u : 0u);
+        wgmma_bf16<NCH>(acc, da_lo, db_hi, 1u);
+        wgmma_bf16<NCH>(acc, da_hi, db_lo, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+}
+
+// Epilogue of one 64-row half tile from the accumulator registers: this warp's 16 rows, one 32-column chunk at a time,
+// into the output segments of p (chunk table `chunks`, one entry per 32 columns of p).  DSILU = false compiles out the
+// silu' epilogue (p.epi must then be AB2_EPI_NONE).
+template <typename TSrc, int NCH, bool DSILU = true>
+__device__ __forceinline__ void tc_epilogue(const TcParams& p, const ChunkInfo* chunks, float* stg, const float (&acc)[16 * NCH], int64_t tile,
+                                            int wg, int w4, int lane) {
+    {
         const int64_t m_base = tile * BM + wg * 64 + w4 * 16;
         const int64_t left64 = p.M - m_base;  // <= 0: this warp's rows lie beyond M
         const int rows_left = left64 >= 16 ? 16 : (left64 > 0 ? (int)left64 : 0);
@@ -362,7 +388,7 @@ __device__ __forceinline__ void tc_consumer_role(const TcParams& p, const TcCtx&
             float v[16];
 #pragma unroll
             for (int j = 0; j < 16; ++j) v[j] = vin[j];
-            if (p.epi == AB2_EPI_MUL_DSILU) {
+            if (DSILU && p.epi == AB2_EPI_MUL_DSILU) {
                 const TSrc* ax = (const TSrc*)p.aux + m * p.aux_ld + c0;
                 if (sizeof(TSrc) == 4 && c0 + 16 <= p.N && ((reinterpret_cast<uintptr_t>(ax) & 15) == 0)) {
                     const float4* a4 = reinterpret_cast<const float4*>(ax);
@@ -425,7 +451,7 @@ __device__ __forceinline__ void tc_consumer_role(const TcParams& p, const TcCtx&
                 *reinterpret_cast<float2*>(stg + ((lane >> 2) + 8) * EPI_LD + col) = make_float2(acc[16 * ch + 4 * j + 2], acc[16 * ch + 4 * j + 3]);
             }
             __syncwarp();
-            const ChunkInfo ci = c.sChunk[ch];
+            const ChunkInfo ci = chunks[ch];
             if ((p.debug & 1) || rows_left == 0) {
             } else if (ci.ok) {
                 // coalesced path: every global access covers 4 rows x 128 B.
@@ -439,7 +465,7 @@ __device__ __forceinline__ void tc_consumer_role(const TcParams& p, const TcCtx&
                 uint32_t off[4];
 #pragma unroll
                 for (int itr = 0; itr < 4; ++itr) off[itr] = (uint32_t)row_of(itr) * ol;
-                if (p.epi == AB2_EPI_MUL_DSILU) {
+                if (DSILU && p.epi == AB2_EPI_MUL_DSILU) {
                     float4 ax[4];
                     const float* ab = ci.aptr + m_base * p.aux_ld + c4 * 4;
                     const uint32_t al = (uint32_t)p.aux_ld;
@@ -478,6 +504,19 @@ __device__ __forceinline__ void tc_consumer_role(const TcParams& p, const TcCtx&
             }
             __syncwarp();  // staging buffer is rewritten by the next chunk
         }
+    }
+}
+
+template <typename TSrc, bool SPLIT, int NCH>
+__device__ __forceinline__ void tc_consumer_role(const TcParams& p, const TcCtx& c, int cw, int lane) {
+    const int wg = cw >> 2, w4 = cw & 3;
+    float* stg = c.sEpi + cw * 16 * EPI_LD;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[16 * NCH];
+    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        tc_mma_ring<SPLIT, NCH>(acc, p, c, wg, lane, stage, phase);
+        tc_epilogue<TSrc, NCH>(p, c.sChunk, stg, acc, tile, wg, w4, lane);
     }
 }
 
@@ -724,74 +763,65 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
 
+// bf16 hi + lo split of two fp32 values (hi = rn(x), lo = rn(x - hi)), packed as bf16x2 pairs
+__device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uint32_t& lo) {
+    const __nv_bfloat16 h0 = __float2bfloat16_rn(a), h1 = __float2bfloat16_rn(b);
+    __nv_bfloat162 hh;
+    hh.x = h0; hh.y = h1;
+    hi = *reinterpret_cast<uint32_t*>(&hh);
+    lo = pack_bf16x2(a - __bfloat162float(h0), b - __bfloat162float(h1));
+}
+
+// barriers of the TMA-fed ring: canonical full / empty [NSTAGE] at bar0, raw-slot full [8] at rbar0
+__device__ __forceinline__ void tma_init_bars(uint32_t bar0, uint32_t rbar0, int wpg) {
+    for (int s = 0; s < NSTAGE; ++s) {
+        mbar_init(bar0 + 8u * s, wpg * 32);          // canonical stage full: the warps of one converter group
+        mbar_init(bar0 + 8u * (NSTAGE + s), NCONS);  // empty: one arrive per consumer warp
+    }
+    for (int s = 0; s < 8; ++s) mbar_init(rbar0 + 8u * s, 1);  // expect_tx arrive of the issuing lane
+    fence_barrier_init();
+}
+
+// k-chunk table entry i (concat columns [32 i, 32 i + 32)): segment index, column offset inside the segment, has-aux flag
+__device__ __forceinline__ int4 tma_kseg_entry(const TcParams& p, int i) {
+    int kk = i * KC;
+    int4 ent = make_int4(-1, 0, 0, 0);
+#pragma unroll
+    for (int sgi = 0; sgi < AB2_MAX_SEG; ++sgi) {
+        if (sgi < p.n_a && ent.x < 0 && kk < p.K) {
+            if (kk < p.a[sgi].width) ent = make_int4(sgi, kk, p.a[sgi].aux ? 1 : 0, 0);
+            kk -= p.a[sgi].width;
+        }
+    }
+    return ent;
+}
+
+// copy the hi and lo images (w_half bytes each) of a packed W into shared memory, all threads of the CTA
+__device__ __forceinline__ void stage_w(uint8_t* dst, const void* hi, const void* lo, int w_half) {
+    const uint4* src = reinterpret_cast<const uint4*>(hi);
+    uint4* d = reinterpret_cast<uint4*>(dst);
+    for (int e = threadIdx.x; e < w_half / 16; e += NTHREADS) d[e] = __ldg(src + e);
+    const uint4* srcl = reinterpret_cast<const uint4*>(lo);
+    uint4* dl = reinterpret_cast<uint4*>(dst + w_half);
+    for (int e = threadIdx.x; e < w_half / 16; e += NTHREADS) dl[e] = __ldg(srcl + e);
+}
+
+// Converter warps 0-7 (G groups) of the TMA-fed ring: total = work items (tile, k block) of this CTA, sKseg the k-chunk
+// table, rbar0 the raw-slot barriers.
 // G converter groups of 8/G warps.  A raw slot and a canonical stage must always be consumed / produced by the SAME group
 // (NR % G == 0 and nstage % G == 0, checked on the host): a group then never waits more than one mbarrier phase ahead
 // of its own slot.  (With slots shared between groups a group's first wait can be for the SECOND fill of a slot whose
 // first fill has not completed yet -- the parity wait returns immediately and the pipeline falls apart.)
-template <int G, int NCH>
-__global__ void __launch_bounds__(NTHREADS, 1) linear_tma_kernel(const TcParams p, const __grid_constant__ TmaMaps maps, int NR) {
+template <int G>
+__device__ __forceinline__ void tma_converter_role(const TcParams& p, const TmaMaps& maps, int NR, const TcCtx& ctx, uint8_t* sRaw,
+                                                   const int4* sKseg, uint32_t rbar0, int64_t total, int warp, int lane) {
     constexpr int WPG = NPROD / G;      // warps per converter group
     constexpr int RGW = 16 / WPG;       // 8-row groups of a stage handled by one warp
-    using TSrc = float;
-    constexpr bool SPLIT = true;
-    extern __shared__ __align__(1024) uint8_t smem[];
-    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;  // warp-uniform role index
-    const int w_half = p.Npad * p.K * 2;
-    const int w_bytes = 2 * w_half;
-    const int stage_bytes = 2 * STAGE_HALF;
+    const int nkb = ctx.nkb;
     const int raw_slot = TMA_BOX_BYTES * (p.has_aux ? 2 : 1);
-    // plan: raw ring (1024-byte aligned, swizzle atom) | W | canonical ring | epilogue staging | prefetch | tail
-    uint8_t* sRaw = smem + ((1024u - (smem_u32(smem) & 1023u)) & 1023u);
-    uint8_t* sW = sRaw + (size_t)NR * raw_slot;
-    uint8_t* sA = sW + ((w_bytes + 127) & ~127);
-    float* sEpi = reinterpret_cast<float*>(sA + p.nstage * stage_bytes);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sEpi) + EPI_BYTES);
-    ChunkInfo* sChunk = reinterpret_cast<ChunkInfo*>(reinterpret_cast<uint8_t*>(bars) + TAIL_BARS);
-    // k-chunk table (one entry per 32 columns): segment index, column offset inside the segment, has-aux flag
-    int4* sKseg = reinterpret_cast<int4*>(reinterpret_cast<uint8_t*>(sChunk) + TAIL_CHUNK);
-    uint64_t* rbars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sKseg) + (MAX_K / 32) * 16);  // raw_full[8]
-    const uint32_t bar0 = smem_u32(bars), rbar0 = smem_u32(rbars);
+    uint8_t* sA = ctx.sA;
+    const int stage_bytes = ctx.stage_bytes;
     auto rfull_bar = [&](int s) { return rbar0 + 8u * s; };
-    const int nkb = p.K / KC;
-
-    // ---- one-time setup ----
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < NSTAGE; ++s) {
-            mbar_init(bar0 + 8u * s, WPG * 32);          // canonical stage full: the warps of one converter group
-            mbar_init(bar0 + 8u * (NSTAGE + s), NCONS);  // empty: one arrive per consumer warp
-        }
-        for (int s = 0; s < 8; ++s) mbar_init(rfull_bar(s), 1);  // expect_tx arrive of the issuing lane
-        fence_barrier_init();
-    }
-    if (threadIdx.x < MAX_K / 32) {
-        int kk = threadIdx.x * KC;
-        int4 ent = make_int4(-1, 0, 0, 0);
-#pragma unroll
-        for (int sgi = 0; sgi < AB2_MAX_SEG; ++sgi) {
-            if (sgi < p.n_a && ent.x < 0 && kk < p.K) {
-                if (kk < p.a[sgi].width) ent = make_int4(sgi, kk, p.a[sgi].aux ? 1 : 0, 0);
-                kk -= p.a[sgi].width;
-            }
-        }
-        sKseg[threadIdx.x] = ent;
-    } else if (threadIdx.x >= 64 && threadIdx.x < 64 + MAX_CHUNK) {
-        sChunk[threadIdx.x - 64] = tc_chunk_info<TSrc>(p, (threadIdx.x - 64) * 32);
-    }
-    {
-        const uint4* src = reinterpret_cast<const uint4*>(p.Wpacked);
-        uint4* dst = reinterpret_cast<uint4*>(sW);
-        for (int e = threadIdx.x; e < w_half / 16; e += NTHREADS) dst[e] = __ldg(src + e);
-        const uint4* srcl = reinterpret_cast<const uint4*>(p.Wlo);
-        uint4* dstl = reinterpret_cast<uint4*>(sW + w_half);
-        for (int e = threadIdx.x; e < w_half / 16; e += NTHREADS) dstl[e] = __ldg(srcl + e);
-    }
-    fence_proxy_async();
-    __syncthreads();
-    TcCtx ctx;
-    ctx.sW = sW; ctx.sA = sA; ctx.sEpi = sEpi; ctx.sChunk = sChunk; ctx.bar0 = bar0;
-    ctx.nkb = nkb; ctx.stage_bytes = stage_bytes; ctx.w_half = w_half;
-    const int64_t my_tiles = (p.num_tiles > blockIdx.x) ? (p.num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-    const int64_t total = my_tiles * nkb;
 
     // loads of sequence number qs (k block qs % nkb of this CTA's tile qs / nkb) into raw slot rs
     auto tma_issue = [&](int64_t qs, int rs) {
@@ -808,9 +838,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tma_kernel(const TcParams 
         }
     };
 
-    if (warp >= NPROD) {
-        tc_consumer_role<TSrc, SPLIT, NCH>(p, ctx, warp - NPROD, lane);
-    } else {
+    {
         // =============================== converters ===============================
         const int grp = warp / WPG, sub = warp % WPG;
         const int r8 = lane & 7, kc = lane >> 3;
@@ -883,6 +911,229 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tma_kernel(const TcParams 
             rs += G; if (rs >= NR) { rs -= NR; rph ^= 1; }
             cs += G; if (cs >= p.nstage) { cs -= p.nstage; cph ^= 1; }
             kb += G; while (kb >= nkb) kb -= nkb;
+        }
+    }
+}
+
+template <int G, int NCH>
+__global__ void __launch_bounds__(NTHREADS, 1) linear_tma_kernel(const TcParams p, const __grid_constant__ TmaMaps maps, int NR) {
+    constexpr int WPG = NPROD / G;      // warps per converter group
+    using TSrc = float;
+    constexpr bool SPLIT = true;
+    extern __shared__ __align__(1024) uint8_t smem[];
+    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;  // warp-uniform role index
+    const int w_half = p.Npad * p.K * 2;
+    const int w_bytes = 2 * w_half;
+    const int stage_bytes = 2 * STAGE_HALF;
+    const int raw_slot = TMA_BOX_BYTES * (p.has_aux ? 2 : 1);
+    // plan: raw ring (1024-byte aligned, swizzle atom) | W | canonical ring | epilogue staging | prefetch | tail
+    uint8_t* sRaw = smem + ((1024u - (smem_u32(smem) & 1023u)) & 1023u);
+    uint8_t* sW = sRaw + (size_t)NR * raw_slot;
+    uint8_t* sA = sW + ((w_bytes + 127) & ~127);
+    float* sEpi = reinterpret_cast<float*>(sA + p.nstage * stage_bytes);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sEpi) + EPI_BYTES);
+    ChunkInfo* sChunk = reinterpret_cast<ChunkInfo*>(reinterpret_cast<uint8_t*>(bars) + TAIL_BARS);
+    // k-chunk table (one entry per 32 columns): segment index, column offset inside the segment, has-aux flag
+    int4* sKseg = reinterpret_cast<int4*>(reinterpret_cast<uint8_t*>(sChunk) + TAIL_CHUNK);
+    uint64_t* rbars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sKseg) + (MAX_K / 32) * 16);  // raw_full[8]
+    const uint32_t bar0 = smem_u32(bars), rbar0 = smem_u32(rbars);
+    const int nkb = p.K / KC;
+
+    // ---- one-time setup ----
+    if (threadIdx.x == 0) tma_init_bars(bar0, rbar0, WPG);
+    if (threadIdx.x < MAX_K / 32) {
+        sKseg[threadIdx.x] = tma_kseg_entry(p, threadIdx.x);
+    } else if (threadIdx.x >= 64 && threadIdx.x < 64 + MAX_CHUNK) {
+        sChunk[threadIdx.x - 64] = tc_chunk_info<TSrc>(p, (threadIdx.x - 64) * 32);
+    }
+    stage_w(sW, p.Wpacked, p.Wlo, w_half);
+    fence_proxy_async();
+    __syncthreads();
+    TcCtx ctx;
+    ctx.sW = sW; ctx.sA = sA; ctx.sEpi = sEpi; ctx.sChunk = sChunk; ctx.bar0 = bar0;
+    ctx.nkb = nkb; ctx.stage_bytes = stage_bytes; ctx.w_half = w_half;
+    const int64_t my_tiles = (p.num_tiles > blockIdx.x) ? (p.num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+    const int64_t total = my_tiles * nkb;
+
+    if (warp >= NPROD) {
+        tc_consumer_role<TSrc, SPLIT, NCH>(p, ctx, warp - NPROD, lane);
+    } else {
+        tma_converter_role<G>(p, maps, NR, ctx, sRaw, sKseg, rbar0, total, warp, lane);
+    }
+}
+
+// =========================================================================================
+// Two-layer SiLU MLP in one kernel (ab2_mlp2).  Stage 1 is the TMA-fed GEMM of linear_tma_kernel (A @ W1, converter
+// warps unchanged); stage 2 multiplies the hidden layer, kept on chip, by W2.  Per 128-row tile each consumer warpgroup,
+// for its own 64 rows:
+//   stage 1   acc = A @ W1 from the ring (rank-1 backward: acc = gout[m] * w1[j] in fp32, no ring);
+//   between   forward: pre = acc goes to HBM through the epilogue, h = silu(acc); backward: h = acc * silu'(pre).  h is
+//             split into bf16 hi + lo and written to the warpgroup's resident 64 x H tile (canonical K-major), then
+//             fence.proxy.async and a named barrier over the warpgroup's 128 threads.  In the backward, pre is brought in
+//             by cp.async while stage 1 runs, each thread's two pre values into the very hi / lo bytes of the tile that
+//             the thread later overwrites with its own result: no registers held over the main loop, no extra barrier;
+//   stage 2   per column chunk of at most 64: acc2 = h @ W2[:, chunk] from the resident tile, then the epilogue into the
+//             chunk's output segments.
+// W1 and W2 (hi + lo) stay resident.  The hidden layer never goes to HBM, and A is read once however wide the output.
+// The k16 steps, the split products and the SiLU / silu' arithmetic are those of the two ab2_linear launches it
+// replaces, so the results are bitwise theirs (the rank-1 stage 1 is an exact fp32 product instead of a split MMA).
+// =========================================================================================
+constexpr int MLP2_MAX_H = 64;      // wider hidden layers need more than 128 registers per consumer thread (spills)
+constexpr int MLP2_CHUNK = 64;      // stage-2 columns per chunk: the accumulator of stage 2 stays at 32 registers
+constexpr int MLP2_MAX_CHUNKS = 4;  // N <= 256
+constexpr int MLP2_TAIL = TAIL_BARS + (1 + MLP2_MAX_CHUNKS) * TAIL_CHUNK + (MAX_K / 32) * 16 + 8 * 8;
+
+struct Mlp2Params {
+    TcParams s1;                    // stage 1: A segments, K, N = Npad = H, W1 images; forward: o = {pre}
+    TcParams s2[MLP2_MAX_CHUNKS];   // stage-2 column chunks: K = H, N, Npad, the chunk's output segments
+    int n0[MLP2_MAX_CHUNKS];        // first column of each chunk
+    int n2;                         // number of chunks
+    int w2_npad;                    // columns of the whole (padded) W2 image
+    int backward;
+    const float* pre;               // backward: silu' argument [M][H]
+    int64_t pre_ld;
+    const float* gout1;             // rank-1 backward: the single Gout column (row stride gout1_ld); null otherwise
+    int64_t gout1_ld;
+    const float* w1row;             // rank-1 backward: the H entries of the 1 x H first matrix
+};
+
+// stage 2 of one column chunk: acc = h (resident) @ W2 chunk, epilogue into the chunk's output segments
+template <int NCH>
+__device__ __forceinline__ void mlp2_stage2(const TcParams& p2, const ChunkInfo* chunks, float* stg, uint32_t h_u, uint32_t h_half, int H, uint32_t w_u,
+                                            uint32_t w_half, int64_t tile, int wg, int w4, int lane) {
+    float acc[16 * NCH];
+    tc_mma_resident<NCH>(acc, h_u, h_half, H, w_u, w_half);
+    tc_epilogue<float, NCH, false>(p2, chunks, stg, acc, tile, wg, w4, lane);
+}
+
+template <int NCH1>
+__global__ void __launch_bounds__(NTHREADS, 1) mlp2_kernel(const __grid_constant__ Mlp2Params q, const __grid_constant__ TmaMaps maps, int NR) {
+    constexpr int G = 2, WPG = NPROD / G;
+    constexpr int H = 32 * NCH1;
+    const TcParams& p = q.s1;
+    extern __shared__ __align__(1024) uint8_t smem[];
+    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;  // warp-uniform role index
+    const bool rank1 = q.gout1 != nullptr;
+    const int w1_half = rank1 ? 0 : H * p.K * 2;
+    const int w2_half = q.w2_npad * H * 2;
+    const int stage_bytes = 2 * STAGE_HALF;
+    constexpr int h_half = 64 * H * 2;  // one warpgroup's hidden tile, hi or lo image
+    // plan: raw ring (1024-byte aligned) | W1 | W2 | canonical ring | hidden tiles (2 warpgroups x hi, lo) | epilogue staging | tail
+    uint8_t* sRaw = smem + ((1024u - (smem_u32(smem) & 1023u)) & 1023u);
+    uint8_t* sW1 = sRaw + (size_t)NR * TMA_BOX_BYTES;
+    uint8_t* sW2 = sW1 + 2 * w1_half;
+    uint8_t* sA = sW2 + 2 * w2_half;
+    uint8_t* sH = sA + p.nstage * stage_bytes;
+    float* sEpi = reinterpret_cast<float*>(sH + 4 * h_half);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sEpi) + EPI_BYTES);
+    // chunk tables: stage 1 (pre), then one per stage-2 chunk, MAX_CHUNK entries each
+    ChunkInfo* sChunk = reinterpret_cast<ChunkInfo*>(reinterpret_cast<uint8_t*>(bars) + TAIL_BARS);
+    int4* sKseg = reinterpret_cast<int4*>(reinterpret_cast<uint8_t*>(sChunk) + (1 + MLP2_MAX_CHUNKS) * TAIL_CHUNK);
+    uint64_t* rbars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sKseg) + (MAX_K / 32) * 16);
+    const uint32_t bar0 = smem_u32(bars), rbar0 = smem_u32(rbars);
+    const int nkb = p.K / KC;
+
+    // ---- one-time setup ----
+    if (threadIdx.x == 0) tma_init_bars(bar0, rbar0, WPG);
+    if (threadIdx.x < MAX_K / 32) {
+        sKseg[threadIdx.x] = tma_kseg_entry(p, threadIdx.x);
+    } else if (threadIdx.x >= 64 && threadIdx.x < 64 + (1 + MLP2_MAX_CHUNKS) * MAX_CHUNK) {
+        const int i = threadIdx.x - 64, t = i / MAX_CHUNK, c0 = (i % MAX_CHUNK) * 32;
+        ChunkInfo ci{nullptr, nullptr, 0, 0, 0};
+        if (t == 0) ci = tc_chunk_info<float>(p, c0);
+        else if (t - 1 < q.n2) ci = tc_chunk_info<float>(q.s2[t - 1], c0);
+        sChunk[i] = ci;
+    }
+    if (!rank1) stage_w(sW1, p.Wpacked, p.Wlo, w1_half);
+    stage_w(sW2, q.s2[0].Wpacked, q.s2[0].Wlo, w2_half);
+    fence_proxy_async();
+    __syncthreads();
+    TcCtx ctx;
+    ctx.sW = sW1; ctx.sA = sA; ctx.sEpi = sEpi; ctx.sChunk = sChunk; ctx.bar0 = bar0;
+    ctx.nkb = nkb; ctx.stage_bytes = stage_bytes; ctx.w_half = w1_half;
+
+    if (warp < NPROD) {
+        if (!rank1) {
+            const int64_t my_tiles = (p.num_tiles > blockIdx.x) ? (p.num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+            tma_converter_role<G>(p, maps, NR, ctx, sRaw, sKseg, rbar0, my_tiles * nkb, warp, lane);
+        }
+        return;
+    }
+    // =============================== consumers ===============================
+    const int cw = warp - NPROD, wg = cw >> 2, w4 = cw & 3;
+    float* stg = sEpi + cw * 16 * EPI_LD;
+    uint8_t* hid = sH + wg * 2 * h_half;  // this warpgroup's hidden tile: hi, then lo
+    const uint32_t hid_u = smem_u32(hid);
+    const int r8 = lane >> 2, cq = 2 * (lane & 3);  // fragment: rows 16 w4 + r8 (+ 8), columns 8 j + cq (+ 1)
+    const uint32_t wg_bar = 8 + wg;                 // named barrier of this warpgroup (ids 1..G are the converter groups')
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        // canonical K-major: byte offset of (row, k) = ((row / 8) (H / 8) + k / 8) 128 + (row % 8) 16 + (k % 8) 2
+        const uint32_t off_a = (uint32_t)(threadIdx.x & 96) * (H / 8) * 8 + r8 * 16 + cq * 2, off_b = off_a + (H / 8) * 128;
+        // fragment rows (rows beyond M read row M - 1: their results are never stored)
+        const int64_t m0 = tile * BM + wg * 64 + w4 * 16 + r8;
+        const int64_t ma = m0 < p.M ? m0 : p.M - 1, mb = m0 + 8 < p.M ? m0 + 8 : p.M - 1;
+        // every warp of the warpgroup is done with the previous tile's stage-2 reads of the hidden tile
+        asm volatile("bar.sync %0, %1;" ::"r"(wg_bar), "r"(128) : "memory");
+        if (q.backward) {  // pre (r, c) -> hi slot of (r, c..c+1), pre (r, c + 1) -> its lo slot
+            const float* ra = q.pre + ma * q.pre_ld + cq;
+            const float* rb = q.pre + mb * q.pre_ld + cq;
+#pragma unroll
+            for (int j = 0; j < 4 * NCH1; ++j) {
+                cp_async4(hid_u + off_a + j * 128, ra + 8 * j);
+                cp_async4(hid_u + h_half + off_a + j * 128, ra + 8 * j + 1);
+                cp_async4(hid_u + off_b + j * 128, rb + 8 * j);
+                cp_async4(hid_u + h_half + off_b + j * 128, rb + 8 * j + 1);
+            }
+            cp_async_commit();
+        }
+        // hidden value i = 4 j + e of this thread's fragment -> bf16 hi + lo in the tile.  In the backward the slot still
+        // holds pre (see above) and is read just before it is overwritten.  (Values are formed on the way to shared
+        // memory: registers an MMA accumulates into are never written by other instructions, which would make ptxas
+        // serialise the wgmma pipeline.)
+        auto slot = [&](int i) { return hid + ((i & 2) ? off_b : off_a) + (i >> 2) * 128 + ((i & 1) ? h_half : 0); };
+        auto pre_at = [&](int i) { return *reinterpret_cast<const float*>(slot(i)); };
+        auto store_hidden = [&](auto&& h) {
+#pragma unroll
+            for (int j = 0; j < 4 * NCH1; ++j) {
+                const float h0 = h(4 * j), h1 = h(4 * j + 1), h2 = h(4 * j + 2), h3 = h(4 * j + 3);
+                uint32_t hi, lo;
+                split_bf16x2(h0, h1, hi, lo);
+                *reinterpret_cast<uint32_t*>(slot(4 * j)) = hi;
+                *reinterpret_cast<uint32_t*>(slot(4 * j + 1)) = lo;
+                split_bf16x2(h2, h3, hi, lo);
+                *reinterpret_cast<uint32_t*>(slot(4 * j + 2)) = hi;
+                *reinterpret_cast<uint32_t*>(slot(4 * j + 3)) = lo;
+            }
+        };
+        if (rank1) {
+            const float ga = __ldg(q.gout1 + ma * q.gout1_ld), gb = __ldg(q.gout1 + mb * q.gout1_ld);
+            cp_async_wait<0>();  // this thread's own copies: visible to it once complete
+            store_hidden([&](int i) {
+                const float w = __ldg(q.w1row + 8 * (i >> 2) + cq + (i & 1));
+                return ((i & 2) ? gb : ga) * w * dsilu_fast(pre_at(i));
+            });
+        } else {
+            float acc[16 * NCH1];
+            tc_mma_ring<true, NCH1>(acc, p, ctx, wg, lane, stage, phase);
+            if (!q.backward) {
+                tc_epilogue<float, NCH1, false>(p, sChunk, stg, acc, tile, wg, w4, lane);  // pre
+                store_hidden([&](int i) { return silu_fast(acc[i]); });
+            } else {
+                cp_async_wait<0>();
+                store_hidden([&](int i) { return acc[i] * dsilu_fast(pre_at(i)); });
+            }
+        }
+        fence_proxy_async();  // generic-proxy writes, read by wgmma through the async proxy
+        asm volatile("bar.sync %0, %1;" ::"r"(wg_bar), "r"(128) : "memory");
+#pragma unroll 1
+        for (int c = 0; c < q.n2; ++c) {
+            const TcParams& p2 = q.s2[c];
+            const ChunkInfo* ch = sChunk + (1 + c) * MAX_CHUNK;
+            const uint32_t w_u = smem_u32(sW2) + (uint32_t)q.n0[c] * H * 2;
+            if (p2.Npad == 32) mlp2_stage2<1>(p2, ch, stg, hid_u, h_half, H, w_u, w2_half, tile, wg, w4, lane);
+            else mlp2_stage2<2>(p2, ch, stg, hid_u, h_half, H, w_u, w2_half, tile, wg, w4, lane);
         }
     }
 }
@@ -1009,6 +1260,19 @@ static int tc_launch_tma(TcParams& p, int w_bytes, int stage_bytes, int max_smem
     return -1;
 }
 
+// SM count and opt-in shared memory per block of the current device (queried once)
+static void tc_device_limits(int& num_sms, int& max_smem) {
+    static int sms = 0, smem = 0;
+    if (sms == 0) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    }
+    num_sms = sms;
+    max_smem = smem;
+}
+
 // One column slice [n0, n0 + N) of the GEMM with its W images resident in shared memory.
 static int tc_launch_slice(int dtype, int64_t M, int K, int N, int n_a, const void* const* a_ptr, const int64_t* a_ld,
                            const int32_t* a_width, const void* const* a_aux, const int64_t* a_aux_ld, int act, const void* Whi, const void* Wlo,
@@ -1016,14 +1280,8 @@ static int tc_launch_slice(int dtype, int64_t M, int K, int N, int n_a, const vo
                            const void* aux, int64_t aux_ld, cudaStream_t st, bool dry = false) {
     const int has_aux = (act == AB2_ACT_MUL_DSILU && a_aux) ? 1 : 0;
     if (tc_npad(N) > MAX_N) return -1;
-    static int num_sms = 0;
-    static int max_smem = 0;
-    if (num_sms == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-        cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    }
+    int num_sms = 0, max_smem = 0;
+    tc_device_limits(num_sms, max_smem);
     TcParams p;
     memset(&p, 0, sizeof(p));
     p.M = M; p.K = K; p.N = N; p.Npad = tc_npad(N); p.n_a = n_a; p.act = act; p.Wpacked = Whi; p.Wlo = Wlo; p.n_o = n_o;
@@ -1140,4 +1398,125 @@ int ab2_linear_tc_try(int dtype, int64_t M, int K, int N, int n_a, const void* c
         if (rc != 0) return n0 == 0 ? -1 : 1;  // a later slice failing would leave a half-written output: report an error
     }
     return 0;
+}
+
+// Fused two-layer SiLU MLP (mlp2_kernel); contract in include/allegro_b200.h.  Returns AB2_NOT_ELIGIBLE, with nothing
+// enqueued and no error set, for a case the kernel does not take: the caller then runs two ab2_linear launches.
+extern "C" int ab2_mlp2(int dtype, int backward, int64_t M, int K, int H, int N, int n_a, const void* const* a_ptr, const int64_t* a_ld,
+                        const int32_t* a_width, const void* W1_packed, const void* W2_packed, const void* w1_row, void* pre, int64_t pre_ld, int n_o,
+                        void* const* o_ptr, const int64_t* o_ld, const int32_t* o_width, const int32_t* o_accum, void* stream) {
+    AB2_CHECK_ARG(n_a >= 1 && n_a <= AB2_MAX_SEG && n_o >= 1 && n_o <= AB2_MAX_SEG, "segment count");
+    AB2_CHECK_ARG(K > 0 && H > 0 && N > 0 && pre && pre_ld >= H, "shape");
+    int ks = 0, ns = 0;
+    for (int s = 0; s < n_a; ++s) {
+        AB2_CHECK_ARG(a_ptr[s] && a_width[s] > 0 && a_ld[s] >= a_width[s], "A segment");
+        ks += a_width[s];
+    }
+    for (int s = 0; s < n_o; ++s) {
+        AB2_CHECK_ARG(o_ptr[s] && o_width[s] > 0 && o_ld[s] >= o_width[s], "output segment");
+        ns += o_width[s];
+    }
+    AB2_CHECK_ARG(ks == K, "A segment widths must sum to K");
+    AB2_CHECK_ARG(ns == N, "output segment widths must sum to N");
+    const bool rank1 = w1_row != nullptr;
+    AB2_CHECK_ARG(!rank1 || (backward && K == 1 && n_a == 1), "rank-1 mode is the backward of a single output column");
+    if (M == 0) return 0;
+    // ---- eligibility ----
+    auto al16 = [](const void* ptr, int64_t ld) { return (reinterpret_cast<uintptr_t>(ptr) % 16) == 0 && (ld * 4) % 16 == 0; };
+    if (dtype != AB2_F32 || !g_ab2_opt_linear_tc || !g_ab2_opt_linear_tma || !tc_encode_fn()) return AB2_NOT_ELIGIBLE;
+    if (H % 32 != 0 || H > MLP2_MAX_H || !W2_packed || M >= ((int64_t)1 << 31) || !al16(pre, pre_ld)) return AB2_NOT_ELIGIBLE;
+    if (rank1) {
+        if (reinterpret_cast<uintptr_t>(w1_row) % 16 != 0) return AB2_NOT_ELIGIBLE;
+    } else {
+        if (!W1_packed || K % KC != 0 || K > MAX_K) return AB2_NOT_ELIGIBLE;
+        for (int s = 0; s < n_a; ++s)
+            if (a_width[s] % KC != 0 || !al16(a_ptr[s], a_ld[s])) return AB2_NOT_ELIGIBLE;
+    }
+    // stage-2 column chunks: equal, multiples of 32, <= MLP2_CHUNK
+    const int nchunks = (N + MLP2_CHUNK - 1) / MLP2_CHUNK;
+    if (nchunks > MLP2_MAX_CHUNKS) return AB2_NOT_ELIGIBLE;
+    const int cwidth = ((N + nchunks - 1) / nchunks + 31) / 32 * 32;
+    const int w2_npad = tc_npad(N);
+    // shared-memory plan: 2 converter groups, deepest {NR raw slots, cn canonical stages} that fits
+    int num_sms = 0, max_smem = 0;
+    tc_device_limits(num_sms, max_smem);
+    const size_t fixed = 1024 + (rank1 ? 0 : (size_t)2 * H * K * 2) + (size_t)2 * w2_npad * H * 2 + (size_t)4 * 64 * H * 2 + EPI_BYTES + MLP2_TAIL;
+    const int plans[4][2] = {{4, 4}, {2, 4}, {4, 2}, {2, 2}};  // {NR, cn}
+    // (rank-1: no ring at all, NR = nstage = 0 -- the kernel lays out W1, W2, ... behind NR raw slots and nstage stages)
+    int NR = 0, nstage = 0;
+    size_t smem = rank1 ? fixed : 0;
+    for (int q = 0; q < 4 && !rank1 && !NR; ++q) {
+        const size_t need = fixed + (size_t)(plans[q][0] * TMA_BOX_BYTES + plans[q][1] * 2 * STAGE_HALF);
+        if (need <= (size_t)max_smem) { NR = plans[q][0]; nstage = plans[q][1]; smem = need; }
+    }
+    if (smem == 0 || smem > (size_t)max_smem) return AB2_NOT_ELIGIBLE;
+
+    Mlp2Params q;
+    memset(&q, 0, sizeof(q));
+    TmaMaps maps;
+    memset(&maps, 0, sizeof(maps));
+    const int64_t num_tiles = (M + BM - 1) / BM;
+    TcParams& p = q.s1;
+    p.M = M; p.K = K; p.N = H; p.Npad = H; p.n_a = n_a; p.act = AB2_ACT_NONE; p.epi = AB2_EPI_NONE;
+    p.num_tiles = num_tiles; p.nstage = nstage;
+    for (int s = 0; s < n_a; ++s) { p.a[s].ptr = a_ptr[s]; p.a[s].ld = a_ld[s]; p.a[s].width = a_width[s]; }
+    if (rank1) {
+        q.gout1 = reinterpret_cast<const float*>(a_ptr[0]);
+        q.gout1_ld = a_ld[0];
+        q.w1row = reinterpret_cast<const float*>(w1_row);
+    } else {
+        p.Wpacked = W1_packed;
+        p.Wlo = reinterpret_cast<const uint8_t*>(W1_packed) + (size_t)H * K * 2;
+        for (int s = 0; s < n_a; ++s)
+            if (!tc_make_map(&maps.a[s], a_ptr[s], a_ld[s], a_width[s], M)) return AB2_NOT_ELIGIBLE;
+    }
+    if (backward) {
+        q.backward = 1;
+        q.pre = reinterpret_cast<const float*>(pre);
+        q.pre_ld = pre_ld;
+    } else {
+        p.n_o = 1;
+        p.o[0].ptr = pre; p.o[0].ld = pre_ld; p.o[0].width = H;
+    }
+    q.w2_npad = w2_npad;
+    q.n2 = 0;
+    for (int n0 = 0; n0 < N; n0 += cwidth, ++q.n2) {
+        const int nc = (N - n0 < cwidth) ? (N - n0) : cwidth;
+        TcParams& p2 = q.s2[q.n2];
+        p2.M = M; p2.K = H; p2.N = nc; p2.Npad = tc_npad(nc); p2.epi = AB2_EPI_NONE; p2.num_tiles = num_tiles;
+        q.n0[q.n2] = n0;
+        // output segments covered by [n0, n0 + nc)
+        int seg_lo = 0;
+        for (int s = 0; s < n_o; ++s) {
+            const int seg_hi = seg_lo + o_width[s];
+            const int a = n0 > seg_lo ? n0 : seg_lo, b = (n0 + nc) < seg_hi ? (n0 + nc) : seg_hi;
+            if (a < b) {
+                TcSeg& o = p2.o[p2.n_o++];
+                o.ptr = reinterpret_cast<float*>(o_ptr[s]) + (a - seg_lo);
+                o.ld = o_ld[s];
+                o.width = b - a;
+                o.accum = o_accum ? o_accum[s] : 0;
+            }
+            seg_lo = seg_hi;
+        }
+    }
+    q.s2[0].Wpacked = W2_packed;  // the whole W2 image (hi, then lo) is staged once
+    q.s2[0].Wlo = reinterpret_cast<const uint8_t*>(W2_packed) + (size_t)w2_npad * H * 2;
+
+    const unsigned grid = (unsigned)((num_tiles < num_sms) ? num_tiles : num_sms);
+    cudaStream_t st = (cudaStream_t)stream;
+    auto go = [&](auto kern) -> int {
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+            cudaGetLastError();
+            return AB2_NOT_ELIGIBLE;
+        }
+        kern<<<grid, NTHREADS, smem, st>>>(q, maps, NR);
+        AB2_CUDA_LAUNCH_CHECK();
+        return 0;
+    };
+    switch (H / 32) {
+        case 1: return go(mlp2_kernel<1>);
+        case 2: return go(mlp2_kernel<2>);
+    }
+    return AB2_NOT_ELIGIBLE;
 }

@@ -132,6 +132,10 @@ class PackedMLP:
     def forward(self, in_segs: Sequence[torch.Tensor], out_segs: Sequence[torch.Tensor]) -> List[torch.Tensor]:
         """Returns the list of stored pre-activations (needed by backward)."""
         M = in_segs[0].shape[0]
+        if self.is_two_layer_silu:  # one kernel, the hidden layer stays on chip (falls through where not eligible)
+            h = torch.empty(M, self.dims[1], dtype=self.dtype, device=self.device)
+            if _lib.mlp2(list(in_segs), self.W[0], self.W[1], list(out_segs), h, W1_packed=self.Wp[0], W2_packed=self.Wp[1]):
+                return [h]
         pre: List[torch.Tensor] = []
         cur = list(in_segs)
         for k in range(self.n_layers):
@@ -148,6 +152,9 @@ class PackedMLP:
 
     def backward(self, gout_segs: Sequence[torch.Tensor], pre: List[torch.Tensor], gin_segs: Sequence[torch.Tensor], gin_accum: Sequence[bool]):
         M = gout_segs[0].shape[0]
+        if self.is_two_layer_silu and _lib.mlp2(list(gout_segs), self.WT[1], self.WT[0], list(gin_segs), pre[0], o_accum=list(gin_accum),
+                                                backward=True, W1_packed=self.WTp[1], W2_packed=self.WTp[0]):
+            return
         cur = list(gout_segs)
         WT, WTp = list(self.WT), list(self.WTp)
         if self.out_pad is not None and self.out_pad_p is not None and len(cur) == 1 and cur[0].is_contiguous():

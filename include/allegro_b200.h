@@ -125,6 +125,28 @@ int ab2_linear(int dtype, int64_t M, int K, int N, int n_a, const void* const* a
 int64_t ab2_linear_packed_bytes(int dtype, int K, int N);
 int ab2_linear_pack(int dtype, int K, int N, const void* W, void* packed, void* stream);
 
+/* Two-layer SiLU MLP in one tensor-core kernel (the latent and readout MLPs, _allegro.py:278; allegro_models.py:231-241),
+ * with the hidden layer kept on chip:
+ *   backward == 0:  pre = A @ W1 (written, [M][H]),       Out (+)= silu(pre) @ W2
+ *   backward != 0:  pre is read,                           Out (+)= ((A @ W1) * silu'(pre)) @ W2
+ * A: n_a row segments (ptr, leading dim, width) whose widths sum to K; Out: n_o column segments summing to N, each with
+ * its own accumulate flag.  W1 [K][H] and W2 [H][N] are given as ab2_linear_pack images.  For the MLP backward pass
+ * A = Gout, W1 = W2_fwd^T, W2 = W1_fwd^T and Out = Gin.
+ * Rank-1 backward (w1_row != NULL): K = 1, A is the single gradient column and w1_row the H fp32 entries of the 1 x H
+ * matrix W1; the first stage is then an exact fp32 product (no packed W1).
+ * Numerics: the same split-bf16 MMAs, k order and SiLU / silu' arithmetic as the two ab2_linear launches it replaces, so
+ * the results are bitwise theirs, except in rank-1 mode, whose first stage is more accurate than the split MMA.
+ * Returns AB2_NOT_ELIGIBLE (nothing enqueued, no error set) for what the kernel does not take: dtype other than AB2_F32,
+ * A segments not multiples of 32 columns (except the rank-1 column) or not 16-byte aligned, H other than 32 or 64, N above
+ * 256, or W1 + W2 + pipeline exceeding the shared memory of one SM.  The caller then runs the MLP as
+ * two ab2_linear calls. */
+#define AB2_NOT_ELIGIBLE (-1)
+int ab2_mlp2(int dtype, int backward, int64_t M, int K, int H, int N, int n_a, const void* const* a_ptr_host,
+             const int64_t* a_ld_host, const int32_t* a_width_host, const void* W1_packed, const void* W2_packed,
+             const void* w1_row /* nullable: rank-1 backward */, void* pre, int64_t pre_ld, int n_o,
+             void* const* o_ptr_host, const int64_t* o_ld_host, const int32_t* o_width_host,
+             const int32_t* o_accum_host, void* stream);
+
 /* _channels.py:44-57 + _contract.py:195-204 fused: gamma[c][j][u] =
  *   sf * sum_{z in row c} Y[z][j] * w[z][irrep(j)][u]      (a4, a7; deterministic, no atomics) */
 int ab2_env_sum(int dtype, int lmax, int64_t N, int U, const int32_t* row_ptr, const void* Y,
