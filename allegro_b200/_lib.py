@@ -40,6 +40,7 @@ _SIGNATURES = {
     "ab2_linear": ([_i32, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _i64, _vp], C.c_int),
     "ab2_linear_packed_bytes": ([_i32, _i32, _i32], C.c_int64),
     "ab2_linear_pack": ([_i32, _i32, _i32, _vp, _vp, _vp], C.c_int),
+    "ab2_mlp2_readout": ([_i32, _i32, _i64, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _vp], C.c_int),
     "ab2_mlp2": ([_i32, _i32, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_env_sum": ([_i32, _i32, _i64, _i32, _vp, _vp, _vp, _i64, _dbl, _vp, _vp], C.c_int),
     "ab2_env_bwd": ([_i32, _i32, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _i64, _vp, _dbl, _vp, _i64, _vp, _vp], C.c_int),
@@ -332,6 +333,67 @@ def mlp2(
         rc = load().ab2_mlp2(
             DTYPE_ENUM[dt], int(backward), M, K, H, N, na, a_ptr, a_ld, a_w, _ptr(W1_packed), _ptr(W2_packed),
             _ptr(_contig(W1, "W1")) if rank1 else None, _ptr(pre), pre_ld, no, o_ptr, o_ld, o_w, o_acc, _stream(),
+        )
+    if rc == NOT_ELIGIBLE:
+        timer.cancel()
+        return False
+    _check(rc)
+    return True
+
+
+def mlp2_readout(
+    backward: bool,
+    x: torch.Tensor,
+    s: torch.Tensor,
+    xl: Optional[torch.Tensor],
+    pre_l: torch.Tensor,
+    pre_r: torch.Tensor,
+    ez: torch.Tensor,
+    w2_ro: torch.Tensor,
+    W_packed: Sequence[Optional[torch.Tensor]],
+    S: int,
+) -> bool:
+    """Last latent MLP + readout MLP in one kernel (ab2_mlp2_readout), P = x.shape[1], U = s.shape[1], S the width of
+    x_L, H the hidden width of both MLPs:
+    forward   reads x = X[:, :P] and s; writes pre_l, xl = X[:, P:P+S], pre_r and ez = Ez;
+              W_packed = packed (W1_lat [P+U][H], W2_lat [H][S], W1_ro[:P] [P][H], W1_ro[P:] [S][H]);
+    backward  reads ez = gEz, pre_l and pre_r; writes x = gX[:, :P] and s = gs (xl is None);
+              W_packed = packed (W1_ro^T [H][P+S], W2_lat^T [S][H], W1_lat^T [H][P+U]).
+    w2_ro: the readout's H x 1 output layer.  Returns False, with nothing computed, when the kernel does not take this
+    case (among others: latent and readout hidden widths that differ): the caller then runs the two MLPs separately."""
+    if any(w is None for w in W_packed):
+        return False
+    M, P = x.shape
+    U = s.shape[1]
+    H = pre_l.shape[1]
+    if pre_r.shape[1] != H or w2_ro.numel() != H:
+        return False  # the kernel takes one hidden width for both MLPs
+    if not backward and xl.shape[1] != S:
+        raise ValueError(f"mlp2_readout: x_L has {xl.shape[1]} columns, S = {S}")
+    # the packed images must be those of the shapes the library is told: it sizes every copy from P, S, U and H
+    kn = [(H, P + S), (S, H), (H, P + U)] if backward else [(P + U, H), (H, S), (P, H), (S, H)]
+    if len(W_packed) != len(kn):
+        raise ValueError(f"mlp2_readout: {len(W_packed)} packed images, expected {len(kn)}")
+    for i, ((k, n), w) in enumerate(zip(kn, W_packed)):
+        if w.numel() * w.element_size() != (n + 31) // 32 * 32 * k * 4:
+            raise ValueError(f"mlp2_readout: packed image {i} is not that of a [{k}][{n}] matrix")
+    dt = x.dtype
+    views = {}
+    for name, t in (("x", x), ("s", s), ("xl", xl), ("pre_l", pre_l), ("pre_r", pre_r), ("ez", ez)):
+        if t is None:
+            views[name] = (None, 0)
+            continue
+        assert t.dtype == dt and t.shape[0] == M
+        views[name] = (_ptr(t), int(t.stride(0))) if name == "ez" else (_ptr(_row_strided(t, name)[0]), int(t.stride(0)))
+    assert ez.shape[1] == 1
+    wp = (C.c_void_p * len(W_packed))(*[w.data_ptr() for w in W_packed])
+    for w in W_packed:
+        _ptr(w)
+    timer = _timed("mlp2_readout", 1)
+    with timer:
+        rc = load().ab2_mlp2_readout(
+            DTYPE_ENUM[dt], int(backward), M, P, S, U, H, *views["x"], *views["s"], *views["xl"], *views["pre_l"], *views["pre_r"],
+            *views["ez"], wp, _ptr(_contig(w2_ro, "w2_ro")), _stream(),
         )
     if rc == NOT_ELIGIBLE:
         timer.cancel()

@@ -308,11 +308,17 @@ struct TcCtx {
 // cw: consumer warp 0..7; warpgroup cw / 4 owns rows [64 (cw / 4), 64 (cw / 4) + 64) of each tile, warp cw % 4 of it
 // holds the accumulator rows [16 (cw % 4), 16 (cw % 4) + 16) of that half.
 
+struct NoExtraMma {
+    __device__ __forceinline__ void operator()(int, int, uint64_t, uint64_t) const {}
+};
+
 // Main loop fed by the ring: acc = A (p.K columns, canonical ring stages) @ W (resident at c.sW).  Each ring slot is
 // released once the wgmma group that read it has retired; stage / phase carry the ring position across tiles.
-template <bool SPLIT, int NCH>
+// extra(kb, ks, da_hi, da_lo) is called after the products of each k16 step, inside the same wgmma group: it may issue
+// further wgmmas that read the same A stage into another accumulator.
+template <bool SPLIT, int NCH, typename Extra = NoExtraMma>
 __device__ __forceinline__ void tc_mma_ring(float (&acc)[16 * NCH], const TcParams& p, const TcCtx& c, int wg, int lane, int& stage,
-                                            uint32_t& phase) {
+                                            uint32_t& phase, const Extra& extra = Extra{}) {
     const int nkb = c.nkb, stage_bytes = c.stage_bytes, w_half = c.w_half;
     const uint32_t sW_u = smem_u32(c.sW);
     const uint32_t w_sbo = (uint32_t)(p.K / 8) * 128;  // bytes between 8-column (n) groups of W
@@ -328,12 +334,13 @@ __device__ __forceinline__ void tc_mma_ring(float (&acc)[16 * NCH], const TcPara
             const uint32_t wk = sW_u + (uint32_t)(kb * (KC / 8) + ks * 2) * 128;
             const uint64_t db_hi = make_desc(wk, 128, w_sbo);
             wgmma_bf16<NCH>(acc, da_hi, db_hi, (kb | ks) ? 1u : 0u);
+            const uint64_t da_lo = make_desc(a_hi + STAGE_HALF + ks * 256, 128, A_SBO);
             if constexpr (SPLIT) {
-                const uint64_t da_lo = make_desc(a_hi + STAGE_HALF + ks * 256, 128, A_SBO);
                 const uint64_t db_lo = make_desc(wk + w_half, 128, w_sbo);
                 wgmma_bf16<NCH>(acc, da_lo, db_hi, 1u);
                 wgmma_bf16<NCH>(acc, da_hi, db_lo, 1u);
             }
+            extra(kb, ks, da_hi, da_lo);
         }
         wgmma_commit();
         // the group of the previous k block has retired: its ring slot is free (this one stays in flight)
@@ -355,14 +362,16 @@ __device__ __forceinline__ void tc_mma_ring(float (&acc)[16 * NCH], const TcPara
 // Main loop from a resident operand: acc = A (this warpgroup's 64 x K tile at a_u, bf16 hi image, lo image a_half bytes
 // further) @ W (K x 32 NCH image at w_u, lo image w_half bytes further), both canonical K-major.  The k16 steps and the
 // three split-bf16 products run in the same order as in tc_mma_ring, so the result is bitwise that of the ring-fed loop.
+// accumulate: continue the k sum already in acc (the k steps of a longer ring-fed loop that follow those in acc).
 template <int NCH>
-__device__ __forceinline__ void tc_mma_resident(float (&acc)[16 * NCH], uint32_t a_u, uint32_t a_half, int K, uint32_t w_u, uint32_t w_half) {
+__device__ __forceinline__ void tc_mma_resident(float (&acc)[16 * NCH], uint32_t a_u, uint32_t a_half, int K, uint32_t w_u, uint32_t w_half,
+                                                bool accumulate = false) {
     const uint32_t sbo = (uint32_t)(K / 8) * 128;  // A rows and W columns: 8-groups K / 8 core matrices apart
     wgmma_fence();
     for (int ks = 0; ks < K / 16; ++ks) {
         const uint64_t da_hi = make_desc(a_u + ks * 256, 128, sbo), da_lo = make_desc(a_u + a_half + ks * 256, 128, sbo);
         const uint64_t db_hi = make_desc(w_u + ks * 256, 128, sbo), db_lo = make_desc(w_u + w_half + ks * 256, 128, sbo);
-        wgmma_bf16<NCH>(acc, da_hi, db_hi, ks ? 1u : 0u);
+        wgmma_bf16<NCH>(acc, da_hi, db_hi, (ks || accumulate) ? 1u : 0u);
         wgmma_bf16<NCH>(acc, da_lo, db_hi, 1u);
         wgmma_bf16<NCH>(acc, da_hi, db_lo, 1u);
     }
@@ -372,8 +381,9 @@ __device__ __forceinline__ void tc_mma_resident(float (&acc)[16 * NCH], uint32_t
 
 // Epilogue of one 64-row half tile from the accumulator registers: this warp's 16 rows, one 32-column chunk at a time,
 // into the output segments of p (chunk table `chunks`, one entry per 32 columns of p).  DSILU = false compiles out the
-// silu' epilogue (p.epi must then be AB2_EPI_NONE).
-template <typename TSrc, int NCH, bool DSILU = true>
+// silu' epilogue (p.epi must then be AB2_EPI_NONE).  GENERIC = false compiles out the per-element path: every chunk must
+// then be on the coalesced path (ChunkInfo::ok, checked by the caller's host code).
+template <typename TSrc, int NCH, bool DSILU = true, bool GENERIC = true>
 __device__ __forceinline__ void tc_epilogue(const TcParams& p, const ChunkInfo* chunks, float* stg, const float (&acc)[16 * NCH], int64_t tile,
                                             int wg, int w4, int lane) {
     {
@@ -489,7 +499,7 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, const ChunkInfo* 
 #pragma unroll
                 for (int itr = 0; itr < 4; ++itr)
                     if (itr * 4 + rsub < rows_left) stg128(tb + off[itr], x[itr]);
-            } else {
+            } else if constexpr (GENERIC) {
                 // generic path: lane -> (row lane % 16, columns c0 + 16 (lane / 16) .. + 16)
                 const int r = lane & 15, h = lane >> 4;
                 if (r < rows_left && c0 + 16 * h < p.N) {
@@ -1138,6 +1148,307 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp2_kernel(const __grid_constant
     }
 }
 
+// =========================================================================================
+// Last latent MLP + readout MLP in one kernel (ab2_mlp2_readout).  The readout reads X[:, :P + S] = [X[:, :P] | x_L]
+// and the last latent MLP reads [X[:, :P] | s] and writes x_L = X[:, P:P+S], so one kernel streams X[:, :P] once and
+// keeps x_L (forward) and its gradient (backward) on chip.  W1_ro = [W1_ro_a ; W1_ro_b] split by rows at P; w2_ro is
+// the readout's H x 1 output layer (fp32).  H = S = 64.  Per 128-row tile each consumer warpgroup, for its own 64 rows:
+//   forward   ring over A = [X[:, :P] | s]: acc = A @ W1_lat and, over the first P columns only, acc_r = A @ W1_ro_a;
+//             pre_L = acc to HBM; h = silu(acc) to the on-chip tile T; x = h @ W2_lat to HBM (x_L) and, split into
+//             bf16 hi + lo as the converters split it, to T; acc_r += x @ W1_ro_b, which continues the readout's k16
+//             order over K = P + S, so pre_r = acc_r is bitwise the readout's; pre_r to HBM;
+//             Ez = sum_j silu(pre_r[j]) w2_ro[j] in fp32 (a quad shuffle; the readout MMA's split-bf16 w2_ro is
+//             replaced by the exact fp32 product).
+//   backward  g_r = gEz w2_ro silu'(pre_r) in fp32 (the rank-1 stage of mlp2_kernel) to T_r; g_x = g_r @ W1_ro^T[:, P:]
+//             to T_x (never to HBM); g_h = (g_x @ W2_lat^T) silu'(pre_L) to T_h; then per column chunk (<= 64) of
+//             [gX[:, :P] | gs]: T_h @ W1_lat^T[:, chunk] (+ T_r @ W1_ro^T[:, chunk] for the gX chunks, added once in
+//             fp32: the readout's gX written and then accumulated into, without the round trip).  pre_r and pre_L
+//             arrive by cp.async as in mlp2_kernel.  No ring: the converter warps only stage the weights.
+// Everything other than Ez is bitwise the two mlp2_kernel launches it replaces.
+// =========================================================================================
+constexpr int RO_H = 64;                    // hidden width of both MLPs and the width S of x_L
+constexpr int RO_TILE = 64 * RO_H * 2;      // one warpgroup's 64 x 64 on-chip operand, hi or lo image (8 KB)
+constexpr int RO_MAX_CHUNKS = 4;            // backward output chunks: P + U <= 256
+constexpr int RO_TAIL = TAIL_BARS + RO_MAX_CHUNKS * TAIL_CHUNK + (MAX_K / 32) * 16 + 8 * 8 + RO_H * 4;
+
+struct Mlp2RoParams {
+    TcParams s1;                  // forward: ring GEMM over [X[:, :P] | s] (K = P + U, N = H) with o = {pre_L}; backward: M, num_tiles
+    TcParams o[RO_MAX_CHUNKS];    // forward: {x_L, pre_r}; backward: the column chunks of [gX[:, :P] | gs]
+    int n0[RO_MAX_CHUNKS];        // backward: first column of each chunk
+    int n_chunks;
+    int P;
+    const void* w[4];             // packed images, forward: W1_lat, W2_lat, W1_ro_a, W1_ro_b; backward: W1_ro^T, W2_lat^T, W1_lat^T
+    int w_half[4];                // bytes of each hi (= lo) image
+    const float* w2ro;            // H fp32
+    float* ez;                    // forward: Ez (written); backward: gEz (read)
+    int64_t ez_ld;
+    const float* pre_l;           // backward: silu' arguments
+    int64_t pre_l_ld;
+    const float* pre_r;
+    int64_t pre_r_ld;
+};
+
+// this thread's 32 accumulator values (fragment of rows r8, r8 + 8 and columns 8 j + cq (+ 1)) -> bf16 hi + lo images of a
+// warpgroup's 64 x 64 canonical K-major tile, as the converters split; h(i) gives value i
+template <typename F>
+__device__ __forceinline__ void ro_store_tile(uint8_t* t, uint32_t off_a, uint32_t off_b, F&& h) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        uint32_t hi, lo;
+        split_bf16x2(h(4 * j), h(4 * j + 1), hi, lo);
+        *reinterpret_cast<uint32_t*>(t + off_a + j * 128) = hi;
+        *reinterpret_cast<uint32_t*>(t + RO_TILE + off_a + j * 128) = lo;
+        split_bf16x2(h(4 * j + 2), h(4 * j + 3), hi, lo);
+        *reinterpret_cast<uint32_t*>(t + off_b + j * 128) = hi;
+        *reinterpret_cast<uint32_t*>(t + RO_TILE + off_b + j * 128) = lo;
+    }
+}
+
+// pre (r, c) -> hi slot of (r, c..c+1), pre (r, c + 1) -> its lo slot, for this thread's fragment (see mlp2_kernel)
+__device__ __forceinline__ void ro_fetch_pre(uint32_t t_u, uint32_t off_a, uint32_t off_b, const float* ra, const float* rb) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        cp_async4(t_u + off_a + j * 128, ra + 8 * j);
+        cp_async4(t_u + RO_TILE + off_a + j * 128, ra + 8 * j + 1);
+        cp_async4(t_u + off_b + j * 128, rb + 8 * j);
+        cp_async4(t_u + RO_TILE + off_b + j * 128, rb + 8 * j + 1);
+    }
+    cp_async_commit();
+}
+
+__device__ __forceinline__ float ro_pre_at(const uint8_t* t, uint32_t off_a, uint32_t off_b, int i) {
+    return *reinterpret_cast<const float*>(t + ((i & 2) ? off_b : off_a) + (i >> 2) * 128 + ((i & 1) ? RO_TILE : 0));
+}
+
+// shared-memory plan of mlp2_readout_fwd_kernel: raw ring (1024-byte aligned) | W1_lat | W2_lat | W1_ro_a | W1_ro_b |
+// canonical ring | tiles (2 warpgroups x hi, lo) | epilogue staging | tail (barriers, chunk tables pre_L / x_L / pre_r,
+// k-chunk table, raw-slot barriers, w2_ro)
+struct RoFwdPlan {
+    uint8_t* raw;
+    uint8_t* w[4];
+    uint8_t* a;
+    uint8_t* t;
+    float* epi;
+    uint64_t* bars;
+    ChunkInfo* chunk;
+    int4* kseg;
+    uint64_t* rbars;
+    float* w2ro;
+    __device__ __forceinline__ RoFwdPlan(uint8_t* smem, const Mlp2RoParams& q, int NR) {
+        raw = smem + ((1024u - (smem_u32(smem) & 1023u)) & 1023u);
+        w[0] = raw + (size_t)NR * TMA_BOX_BYTES;
+#pragma unroll
+        for (int i = 1; i < 4; ++i) w[i] = w[i - 1] + 2 * q.w_half[i - 1];
+        a = w[3] + 2 * q.w_half[3];
+        t = a + q.s1.nstage * 2 * STAGE_HALF;
+        epi = reinterpret_cast<float*>(t + 4 * RO_TILE);
+        bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(epi) + EPI_BYTES);
+        chunk = reinterpret_cast<ChunkInfo*>(reinterpret_cast<uint8_t*>(bars) + TAIL_BARS);
+        kseg = reinterpret_cast<int4*>(reinterpret_cast<uint8_t*>(chunk) + RO_MAX_CHUNKS * TAIL_CHUNK);
+        rbars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(kseg) + (MAX_K / 32) * 16);
+        w2ro = reinterpret_cast<float*>(rbars + 8);
+    }
+    __device__ __forceinline__ TcCtx ctx(const Mlp2RoParams& q) const {
+        TcCtx c;
+        c.sW = w[0]; c.sA = a; c.sEpi = epi; c.sChunk = chunk; c.bar0 = smem_u32(bars);
+        c.nkb = q.s1.K / KC; c.stage_bytes = 2 * STAGE_HALF; c.w_half = q.w_half[0];
+        return c;
+    }
+};
+
+__global__ void __launch_bounds__(NTHREADS, 1) mlp2_readout_fwd_kernel(const __grid_constant__ Mlp2RoParams q, const __grid_constant__ TmaMaps maps,
+                                                                        int NR) {
+    constexpr int G = 2, WPG = NPROD / G;
+    const TcParams& p = q.s1;
+    extern __shared__ __align__(1024) uint8_t smem[];
+    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);  // warp-uniform role index
+
+    // ---- one-time setup ----
+    {
+        const RoFwdPlan sp(smem, q, NR);
+        if (threadIdx.x == 0) tma_init_bars(smem_u32(sp.bars), smem_u32(sp.rbars), WPG);
+        if (threadIdx.x < MAX_K / 32) {
+            sp.kseg[threadIdx.x] = tma_kseg_entry(p, threadIdx.x);
+        } else if (threadIdx.x >= 64 && threadIdx.x < 64 + 3 * MAX_CHUNK) {
+            const int i = threadIdx.x - 64, t = i / MAX_CHUNK, c0 = (i % MAX_CHUNK) * 32;
+            sp.chunk[i] = tc_chunk_info<float>(t == 0 ? p : q.o[t - 1], c0);
+        } else if (threadIdx.x >= 128 && threadIdx.x < 128 + RO_H) {
+            sp.w2ro[threadIdx.x - 128] = q.w2ro[threadIdx.x - 128];
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) stage_w(sp.w[i], q.w[i], reinterpret_cast<const uint8_t*>(q.w[i]) + q.w_half[i], q.w_half[i]);
+        fence_proxy_async();
+        __syncthreads();
+        if (warp < NPROD) {
+            const int64_t my_tiles = (p.num_tiles > blockIdx.x) ? (p.num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+            tma_converter_role<G>(p, maps, NR, sp.ctx(q), sp.raw, sp.kseg, smem_u32(sp.rbars), my_tiles * (p.K / KC), warp, threadIdx.x & 31);
+            return;
+        }
+    }
+    // =============================== consumers ===============================
+    const int cw = warp - NPROD, wg = cw >> 2, w4 = cw & 3;
+    const uint32_t wg_bar = 8 + wg;  // named barrier of this warpgroup (ids 1..G are the converter groups')
+    const int nkb_r = q.P / KC;
+    auto wg_sync = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(wg_bar), "r"(128) : "memory"); };
+    int stage = 0;
+    uint32_t phase = 0;
+    const RoFwdPlan sp(smem, q, NR);
+    const TcCtx ctx = sp.ctx(q);
+    float* stg = sp.epi + cw * 16 * EPI_LD;
+    uint8_t* tl = sp.t + wg * 2 * RO_TILE;  // this warpgroup's tile: hi, then lo
+    const uint32_t tl_u = smem_u32(tl);
+    const uint32_t wa_u = smem_u32(sp.w[2]), wa_half = q.w_half[2], wa_sbo = (uint32_t)(q.P / 8) * 128;
+    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        // The lane index is re-read per tile: the lane-dependent addresses of the three epilogues are then formed inside
+        // the loop.  Hoisted out of it they stay live next to the 64 accumulator registers of the ring and spill.
+        int lane;
+        asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
+        const int r8 = lane >> 2, cq = 2 * (lane & 3);  // fragment: rows 16 w4 + r8 (+ 8), columns 8 j + cq (+ 1)
+        // canonical K-major: byte offset of (row, k) = ((row / 8) (H / 8) + k / 8) 128 + (row % 8) 16 + (k % 8) 2
+        const uint32_t off_a = (uint32_t)w4 * 32 * (RO_H / 8) * 8 + r8 * 16 + cq * 2, off_b = off_a + (RO_H / 8) * 128;
+        wg_sync();  // every warp of the warpgroup is done with the previous tile's reads of T
+        float acc[32], acc_r[32];
+        // acc_r = X[:, :P] @ W1_ro_a from the same ring stages, with the products in the order of the readout's ring
+        tc_mma_ring<true, 2>(acc, p, ctx, wg, lane, stage, phase, [&](int kb, int ks, uint64_t da_hi, uint64_t da_lo) {
+            if (kb < nkb_r) {
+                const uint32_t wk = wa_u + (uint32_t)(kb * (KC / 8) + ks * 2) * 128;
+                const uint64_t db_hi = make_desc(wk, 128, wa_sbo), db_lo = make_desc(wk + wa_half, 128, wa_sbo);
+                wgmma_bf16<2>(acc_r, da_hi, db_hi, (kb | ks) ? 1u : 0u);
+                wgmma_bf16<2>(acc_r, da_lo, db_hi, 1u);
+                wgmma_bf16<2>(acc_r, da_hi, db_lo, 1u);
+            }
+        });
+        tc_epilogue<float, 2, false, false>(p, sp.chunk, stg, acc, tile, wg, w4, lane);  // pre_L
+        ro_store_tile(tl, off_a, off_b, [&](int i) { return silu_fast(acc[i]); });
+        fence_proxy_async();  // generic-proxy writes, read by wgmma through the async proxy
+        wg_sync();
+        {
+            float x[32];
+            tc_mma_resident<2>(x, tl_u, RO_TILE, RO_H, smem_u32(sp.w[1]), q.w_half[1]);
+            wg_sync();  // every warp's wgmma reads of h have completed before T is overwritten
+            tc_epilogue<float, 2, false, false>(q.o[0], sp.chunk + MAX_CHUNK, stg, x, tile, wg, w4, lane);  // x_L
+            ro_store_tile(tl, off_a, off_b, [&](int i) { return x[i]; });
+        }
+        fence_proxy_async();
+        wg_sync();
+        tc_mma_resident<2>(acc_r, tl_u, RO_TILE, RO_H, smem_u32(sp.w[3]), q.w_half[3], /*accumulate=*/true);
+        tc_epilogue<float, 2, false, false>(q.o[1], sp.chunk + 2 * MAX_CHUNK, stg, acc_r, tile, wg, w4, lane);  // pre_r
+        // Ez: this thread's 16 columns of rows r8 and r8 + 8, then the sum over the 4 lanes of the quad
+        float ea = 0.f, eb = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float2 w = *reinterpret_cast<const float2*>(sp.w2ro + 8 * j + cq);
+            ea = fmaf(silu_fast(acc_r[4 * j]), w.x, ea);
+            ea = fmaf(silu_fast(acc_r[4 * j + 1]), w.y, ea);
+            eb = fmaf(silu_fast(acc_r[4 * j + 2]), w.x, eb);
+            eb = fmaf(silu_fast(acc_r[4 * j + 3]), w.y, eb);
+        }
+        ea += __shfl_xor_sync(0xffffffffu, ea, 1);
+        eb += __shfl_xor_sync(0xffffffffu, eb, 1);
+        ea += __shfl_xor_sync(0xffffffffu, ea, 2);
+        eb += __shfl_xor_sync(0xffffffffu, eb, 2);
+        const int64_t m0 = tile * BM + wg * 64 + w4 * 16 + r8;
+        if ((lane & 3) == 0) {
+            if (m0 < p.M) q.ez[m0 * q.ez_ld] = ea;
+            if (m0 + 8 < p.M) q.ez[(m0 + 8) * q.ez_ld] = eb;
+        }
+    }
+}
+
+// backward output chunk c: acc = T_h @ W1_lat^T[:, chunk] (+ T_r @ W1_ro^T[:, chunk]), epilogue into the chunk's output
+template <int NCH>
+__device__ __forceinline__ void ro_bwd_chunk(const TcParams& pc, const ChunkInfo* chunks, float* stg, uint32_t th_u, uint32_t wl_u, uint32_t wl_half,
+                                             uint32_t tr_u, uint32_t wr_u, uint32_t wr_half, bool with_ro, int64_t tile, int wg, int w4, int lane) {
+    float acc[16 * NCH];
+    tc_mma_resident<NCH>(acc, th_u, RO_TILE, RO_H, wl_u, wl_half);
+    if (with_ro) {
+        float acc2[16 * NCH], sum[16 * NCH];
+        tc_mma_resident<NCH>(acc2, tr_u, RO_TILE, RO_H, wr_u, wr_half);
+#pragma unroll
+        for (int i = 0; i < 16 * NCH; ++i) sum[i] = acc[i] + acc2[i];
+        tc_epilogue<float, NCH, false>(pc, chunks, stg, sum, tile, wg, w4, lane);
+    } else {
+        tc_epilogue<float, NCH, false>(pc, chunks, stg, acc, tile, wg, w4, lane);
+    }
+}
+
+__global__ void __launch_bounds__(NTHREADS, 1) mlp2_readout_bwd_kernel(const __grid_constant__ Mlp2RoParams q) {
+    const TcParams& p = q.s1;
+    extern __shared__ __align__(1024) uint8_t smem[];
+    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;  // warp-uniform role index
+    // plan: W1_ro^T | W2_lat^T | W1_lat^T | tiles T_r, T_x, T_h (2 warpgroups x hi, lo each) | epilogue staging | tail
+    uint8_t* sWi[3];
+    sWi[0] = smem;
+    for (int i = 1; i < 3; ++i) sWi[i] = sWi[i - 1] + 2 * q.w_half[i - 1];
+    uint8_t* sT = sWi[2] + 2 * q.w_half[2];
+    float* sEpi = reinterpret_cast<float*>(sT + 3 * 4 * RO_TILE);
+    ChunkInfo* sChunk = reinterpret_cast<ChunkInfo*>(reinterpret_cast<uint8_t*>(sEpi) + EPI_BYTES + TAIL_BARS);
+    if (threadIdx.x < RO_MAX_CHUNKS * MAX_CHUNK) {
+        const int t = threadIdx.x / MAX_CHUNK;
+        ChunkInfo ci{nullptr, nullptr, 0, 0, 0};
+        if (t < q.n_chunks) ci = tc_chunk_info<float>(q.o[t], (threadIdx.x % MAX_CHUNK) * 32);
+        sChunk[threadIdx.x] = ci;
+    }
+    for (int i = 0; i < 3; ++i) stage_w(sWi[i], q.w[i], reinterpret_cast<const uint8_t*>(q.w[i]) + q.w_half[i], q.w_half[i]);
+    fence_proxy_async();
+    __syncthreads();
+    if (warp < NPROD) return;
+    // =============================== consumers ===============================
+    const int cw = warp - NPROD, wg = cw >> 2, w4 = cw & 3;
+    float* stg = sEpi + cw * 16 * EPI_LD;
+    uint8_t* t_r = sT + wg * 2 * RO_TILE;  // this warpgroup's tiles (hi, then lo): T_r, T_x, T_h
+    uint8_t* t_x = t_r + 4 * RO_TILE;
+    uint8_t* t_h = t_x + 4 * RO_TILE;
+    const uint32_t tr_u = smem_u32(t_r), tx_u = smem_u32(t_x), th_u = smem_u32(t_h);
+    const uint32_t wr_u = smem_u32(sWi[0]), wl_u = smem_u32(sWi[2]);
+    const int r8 = lane >> 2, cq = 2 * (lane & 3);
+    const uint32_t wg_bar = 8 + wg;
+    const uint32_t off_a = (uint32_t)(threadIdx.x & 96) * (RO_H / 8) * 8 + r8 * 16 + cq * 2, off_b = off_a + (RO_H / 8) * 128;
+    auto wg_sync = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(wg_bar), "r"(128) : "memory"); };
+    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        const int64_t m0 = tile * BM + wg * 64 + w4 * 16 + r8;  // rows beyond M read row M - 1: their results are never stored
+        const int64_t ma = m0 < p.M ? m0 : p.M - 1, mb = m0 + 8 < p.M ? m0 + 8 : p.M - 1;
+        wg_sync();  // every warp of the warpgroup is done with the previous tile's reads of T_r, T_x, T_h
+        ro_fetch_pre(tr_u, off_a, off_b, q.pre_r + ma * q.pre_r_ld + cq, q.pre_r + mb * q.pre_r_ld + cq);
+        ro_fetch_pre(th_u, off_a, off_b, q.pre_l + ma * q.pre_l_ld + cq, q.pre_l + mb * q.pre_l_ld + cq);
+        const float ga = __ldg(q.ez + ma * q.ez_ld), gb = __ldg(q.ez + mb * q.ez_ld);
+        cp_async_wait<1>();  // pre_r (this thread's own copies: visible to it once complete)
+        ro_store_tile(t_r, off_a, off_b, [&](int i) {
+            const float w = __ldg(q.w2ro + 8 * (i >> 2) + cq + (i & 1));
+            return ((i & 2) ? gb : ga) * w * dsilu_fast(ro_pre_at(t_r, off_a, off_b, i));
+        });
+        fence_proxy_async();
+        wg_sync();
+        {
+            float gx[32];  // g_x = g_r @ W1_ro^T[:, P:P+S]
+            tc_mma_resident<2>(gx, tr_u, RO_TILE, RO_H, wr_u + (uint32_t)q.P * RO_H * 2, q.w_half[0]);
+            ro_store_tile(t_x, off_a, off_b, [&](int i) { return gx[i]; });
+        }
+        fence_proxy_async();
+        wg_sync();
+        {
+            float gh[32];  // g_h = (g_x @ W2_lat^T) silu'(pre_L)
+            tc_mma_resident<2>(gh, tx_u, RO_TILE, RO_H, smem_u32(sWi[1]), q.w_half[1]);
+            cp_async_wait<0>();
+            ro_store_tile(t_h, off_a, off_b, [&](int i) { return gh[i] * dsilu_fast(ro_pre_at(t_h, off_a, off_b, i)); });
+        }
+        fence_proxy_async();
+        wg_sync();
+#pragma unroll 1
+        for (int c = 0; c < q.n_chunks; ++c) {
+            const TcParams& pc = q.o[c];
+            const uint32_t n0 = (uint32_t)q.n0[c];
+            const bool with_ro = (int)n0 < q.P;
+            if (pc.Npad == 32)
+                ro_bwd_chunk<1>(pc, sChunk + c * MAX_CHUNK, stg, th_u, wl_u + n0 * RO_H * 2, q.w_half[2], tr_u, wr_u + n0 * RO_H * 2, q.w_half[0],
+                                with_ro, tile, wg, w4, lane);
+            else
+                ro_bwd_chunk<2>(pc, sChunk + c * MAX_CHUNK, stg, th_u, wl_u + n0 * RO_H * 2, q.w_half[2], tr_u, wr_u + n0 * RO_H * 2, q.w_half[0],
+                                with_ro, tile, wg, w4, lane);
+        }
+    }
+}
+
 // W[K][N] (row-major TSrc) -> canonical K-major no-swizzle bf16 images (hi, lo), Npad rows:
 //   byte offset of (n, k) = ((n/8)*(K/8) + k/8)*128 + (n%8)*16 + (k%8)*2
 template <typename TSrc>
@@ -1519,4 +1830,103 @@ extern "C" int ab2_mlp2(int dtype, int backward, int64_t M, int K, int H, int N,
         case 2: return go(mlp2_kernel<2>);
     }
     return AB2_NOT_ELIGIBLE;
+}
+
+// Last latent MLP + readout MLP (mlp2_readout_fwd_kernel / mlp2_readout_bwd_kernel); contract in include/allegro_b200.h.
+// Returns AB2_NOT_ELIGIBLE, with nothing enqueued and no error set, for a case the kernels do not take: the caller then
+// runs the two MLPs as two ab2_mlp2 (or ab2_linear) calls.
+extern "C" int ab2_mlp2_readout(int dtype, int backward, int64_t M, int P, int S, int U, int H, void* x, int64_t x_ld, void* s, int64_t s_ld,
+                                void* xl, int64_t xl_ld, void* pre_l, int64_t pre_l_ld, void* pre_r, int64_t pre_r_ld, void* ez, int64_t ez_ld,
+                                const void* const* w_packed, const void* w2_ro, void* stream) {
+    AB2_CHECK_ARG(P > 0 && S > 0 && U > 0 && H > 0 && M >= 0, "shape");
+    AB2_CHECK_ARG(x && s && pre_l && pre_r && ez && w2_ro && w_packed && (backward || xl), "null pointer");
+    AB2_CHECK_ARG(x_ld >= P && s_ld >= U && (backward || xl_ld >= S) && pre_l_ld >= H && pre_r_ld >= H && ez_ld >= 1, "leading dimension");
+    if (M == 0) return 0;
+    // ---- eligibility ----
+    const int n_w = backward ? 3 : 4;
+    auto al16 = [](const void* ptr, int64_t ld) { return (reinterpret_cast<uintptr_t>(ptr) % 16) == 0 && (ld * 4) % 16 == 0; };
+    if (dtype != AB2_F32 || !g_ab2_opt_linear_tc || !g_ab2_opt_linear_tma || (!backward && !tc_encode_fn())) return AB2_NOT_ELIGIBLE;
+    if (H != RO_H || S != RO_H || P % KC != 0 || U % KC != 0 || P + U > MAX_K || M >= ((int64_t)1 << 31)) return AB2_NOT_ELIGIBLE;
+    if (!al16(x, x_ld) || !al16(s, s_ld) || (!backward && !al16(xl, xl_ld)) || !al16(pre_l, pre_l_ld) || !al16(pre_r, pre_r_ld) ||
+        reinterpret_cast<uintptr_t>(w2_ro) % 16 != 0)
+        return AB2_NOT_ELIGIBLE;
+    for (int i = 0; i < n_w; ++i)
+        if (!w_packed[i]) return AB2_NOT_ELIGIBLE;
+
+    Mlp2RoParams q;
+    memset(&q, 0, sizeof(q));
+    const int64_t num_tiles = (M + BM - 1) / BM;
+    q.P = P;
+    q.w2ro = reinterpret_cast<const float*>(w2_ro);
+    q.ez = reinterpret_cast<float*>(ez);
+    q.ez_ld = ez_ld;
+    for (int i = 0; i < n_w; ++i) q.w[i] = w_packed[i];
+    TcParams& p = q.s1;
+    p.M = M; p.num_tiles = num_tiles;
+    auto out1 = [&](TcParams& o, void* ptr, int64_t ld, int n) {  // one output segment of n columns, plain stores
+        o.M = M; o.K = H; o.N = n; o.Npad = n; o.epi = AB2_EPI_NONE; o.num_tiles = num_tiles;
+        o.n_o = 1; o.o[0].ptr = ptr; o.o[0].ld = ld; o.o[0].width = n;
+    };
+    int num_sms = 0, max_smem = 0;
+    tc_device_limits(num_sms, max_smem);
+    const unsigned grid = (unsigned)((num_tiles < num_sms) ? num_tiles : num_sms);
+    cudaStream_t st = (cudaStream_t)stream;
+    auto go = [&](auto kern, size_t smem, auto... args) -> int {
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+            cudaGetLastError();
+            return AB2_NOT_ELIGIBLE;
+        }
+        kern<<<grid, NTHREADS, smem, st>>>(q, args...);
+        AB2_CUDA_LAUNCH_CHECK();
+        return 0;
+    };
+
+    if (backward) {
+        // output chunks of [gX[:, :P] | gs]: the prefix, then gs, each in pieces of at most 64 columns
+        for (int seg = 0; seg < 2; ++seg) {
+            const int lo = seg ? P : 0, hi = seg ? P + U : P;
+            for (int n0 = lo; n0 < hi; n0 += 64) {
+                if (q.n_chunks == RO_MAX_CHUNKS) return AB2_NOT_ELIGIBLE;
+                const int nc = hi - n0 < 64 ? hi - n0 : 64;
+                float* base = seg ? reinterpret_cast<float*>(s) + (n0 - P) : reinterpret_cast<float*>(x) + n0;
+                out1(q.o[q.n_chunks], base, seg ? s_ld : x_ld, nc);
+                q.n0[q.n_chunks++] = n0;
+            }
+        }
+        q.w_half[0] = (P + S) * H * 2;  // W1_ro^T: K = H, N = P + S
+        q.w_half[1] = H * S * 2;        // W2_lat^T: K = S, N = H
+        q.w_half[2] = (P + U) * H * 2;  // W1_lat^T: K = H, N = P + U
+        q.pre_l = reinterpret_cast<const float*>(pre_l); q.pre_l_ld = pre_l_ld;
+        q.pre_r = reinterpret_cast<const float*>(pre_r); q.pre_r_ld = pre_r_ld;
+        const size_t smem = (size_t)2 * (q.w_half[0] + q.w_half[1] + q.w_half[2]) + (size_t)12 * RO_TILE + EPI_BYTES + RO_TAIL;
+        if (smem > (size_t)max_smem) return AB2_NOT_ELIGIBLE;
+        return go(mlp2_readout_bwd_kernel, smem);
+    }
+
+    p.K = P + U; p.N = H; p.Npad = H; p.n_a = 2; p.act = AB2_ACT_NONE; p.epi = AB2_EPI_NONE;
+    p.a[0].ptr = x; p.a[0].ld = x_ld; p.a[0].width = P;
+    p.a[1].ptr = s; p.a[1].ld = s_ld; p.a[1].width = U;
+    p.Wpacked = w_packed[0];
+    p.n_o = 1; p.o[0].ptr = pre_l; p.o[0].ld = pre_l_ld; p.o[0].width = H;
+    out1(q.o[0], xl, xl_ld, S);
+    out1(q.o[1], pre_r, pre_r_ld, H);
+    q.w_half[0] = H * (P + U) * 2;  // W1_lat: K = P + U, N = H
+    q.w_half[1] = S * H * 2;        // W2_lat: K = H, N = S
+    q.w_half[2] = H * P * 2;        // W1_ro[:P]: K = P, N = H
+    q.w_half[3] = H * S * 2;        // W1_ro[P:]: K = S, N = H
+    p.Wlo = reinterpret_cast<const uint8_t*>(w_packed[0]) + q.w_half[0];
+    // shared-memory plan: 2 converter groups, deepest {NR raw slots, cn canonical stages} that fits
+    const size_t fixed = 1024 + (size_t)2 * (q.w_half[0] + q.w_half[1] + q.w_half[2] + q.w_half[3]) + (size_t)4 * RO_TILE + EPI_BYTES + RO_TAIL;
+    const int plans[4][2] = {{4, 4}, {2, 4}, {4, 2}, {2, 2}};  // {NR, cn}
+    int NR = 0;
+    size_t smem = 0;
+    for (int i = 0; i < 4 && !NR; ++i) {
+        const size_t need = fixed + (size_t)(plans[i][0] * TMA_BOX_BYTES + plans[i][1] * 2 * STAGE_HALF);
+        if (need <= (size_t)max_smem) { NR = plans[i][0]; p.nstage = plans[i][1]; smem = need; }
+    }
+    if (!NR) return AB2_NOT_ELIGIBLE;
+    TmaMaps maps;
+    memset(&maps, 0, sizeof(maps));
+    if (!tc_make_map(&maps.a[0], x, x_ld, P, M) || !tc_make_map(&maps.a[1], s, s_ld, U, M)) return AB2_NOT_ELIGIBLE;
+    return go(mlp2_readout_fwd_kernel, smem, maps, NR);
 }

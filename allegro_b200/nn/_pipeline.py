@@ -92,6 +92,15 @@ class AllegroCore:
             assert tp.base_dim2 == self.D
         self.readout = PackedMLP(edge_readout, dtype, device)
         self.nw = nw
+        # the last latent MLP and the readout in one kernel per direction (ab2_mlp2_readout); the readout's first layer
+        # is packed once more split by rows into the x_0..x_{L-1} block and the x_L block
+        last = self.layers[-1]["mlp"]
+        self.ro_fused = last.is_two_layer_silu and self.readout.is_two_layer_silu and last.dims[1] == self.readout.dims[1]
+        if self.ro_fused:
+            P = S * self.L
+            W1r = self.readout.W[0]
+            self.ro_fwd_p = [last.Wp[0], last.Wp[1], _lib.linear_pack(W1r[:P].contiguous()), _lib.linear_pack(W1r[P:].contiguous())]
+            self.ro_bwd_p = [self.readout.WTp[0], last.WTp[1], last.WTp[0]]
         # "plain GEMM" backward plan (all latent/readout MLPs are 2-layer SiLU): the gradient of the
         # densenet block x_b is ONE GEMM over all its consumers (readout, latents m >= b), concatenated
         # along K, each consumer's g_h scaled by silu'(pre) in the GEMM prologue -- no accumulation.
@@ -138,6 +147,8 @@ class AllegroCore:
             self.embed.forward([x_emb], [w0, X[:, :S], omega[0]])
         V: List[Optional[torch.Tensor]] = [None]
         gammas, pre_lat = [], []
+        Ez = torch.empty(E, 1, dtype=dt, device=dev)
+        pre_read = None
         for l, ly in enumerate(self.layers):
             _lib.set_tag(f"fwd.L{l}")
             gamma = _lib.env_sum(dt, self.lmax, N, U, csr.row_ptr, Y, omega[l], self.sf)
@@ -149,12 +160,20 @@ class AllegroCore:
             if not ly["last"]:
                 omega.append(torch.empty(E, self.nw, dtype=dt, device=dev))
                 outs.append(omega[l + 1])
-            pre_lat.append(ly["mlp"].forward([X[:, : S * (l + 1)], s], outs))
+            if ly["last"] and self.ro_fused:
+                P = S * L
+                pre_l = torch.empty(E, ly["mlp"].dims[1], dtype=dt, device=dev)
+                pre_r = torch.empty(E, self.readout.dims[1], dtype=dt, device=dev)
+                if _lib.mlp2_readout(False, X[:, :P], s, X[:, P:], pre_l, pre_r, Ez, self.readout.W[1], self.ro_fwd_p, S):
+                    pre_lat.append([pre_l])
+                    pre_read = [pre_r]
+            if pre_read is None:
+                pre_lat.append(ly["mlp"].forward([X[:, : S * (l + 1)], s], outs))
             V.append(Vn)
             gammas.append(gamma)
-        _lib.set_tag("fwd.readout")
-        Ez = torch.empty(E, 1, dtype=dt, device=dev)
-        pre_read = self.readout.forward([X], [Ez])
+        if pre_read is None:
+            _lib.set_tag("fwd.readout")
+            pre_read = self.readout.forward([X], [Ez])
         Ei = _lib.edge_sum(Ez.view(E).to(self.acc), csr.row_ptr, self.factor)
         sv.Y, sv.w0, sv.omega, sv.V, sv.gamma, sv.pre_lat, sv.pre_read, sv.X = Y, w0, omega, V, gammas, pre_lat, pre_read, X
         return Ei, X, Ez, sv
@@ -234,7 +253,15 @@ class AllegroCore:
         _lib.set_tag("bwd.readout")
         gEz = _lib.edge_sum_bwd(gEi.contiguous(), csr.ctr, self.factor).to(dt).view(E, 1)
         gX = torch.empty(E, S * (L + 1), dtype=dt, device=dev)
-        self.readout.backward([gEz], sv.pre_read, [gX], [False])
+        last = self.layers[-1]
+        gV_last = torch.empty(E, last["d_out"], U, dtype=dt, device=dev)
+        if last["d_out"] > 1:
+            gV_last.zero_()
+        # readout and last latent MLP in one kernel: gX[:, :S L] and gs of the last layer (gX[:, S L:] is not formed)
+        fused = self.ro_fused and _lib.mlp2_readout(True, gX[:, : S * L], gV_last.view(E, -1)[:, :U], None, sv.pre_lat[-1][0],
+                                                     sv.pre_read[0], gEz, self.readout.W[1], self.ro_bwd_p, S)
+        if not fused:
+            self.readout.backward([gEz], sv.pre_read, [gX], [False])
         gY = torch.zeros(E, D, dtype=self.acc, device=dev)
         gV_next: Optional[torch.Tensor] = None   # grad wrt V_{l+1}
         gomega_next: Optional[torch.Tensor] = None  # grad wrt omega_{l+1}
@@ -243,9 +270,7 @@ class AllegroCore:
             ly = self.layers[l]
             _lib.set_tag(f"bwd.L{l}")
             if ly["last"]:
-                gV_next = torch.empty(E, ly["d_out"], U, dtype=dt, device=dev)
-                if ly["d_out"] > 1:
-                    gV_next.zero_()
+                gV_next = gV_last
                 gs_acc = False
             else:
                 gs_acc = True
@@ -253,7 +278,8 @@ class AllegroCore:
             gouts = [gX[:, S * (l + 1) : S * (l + 2)]]
             if not ly["last"]:
                 gouts.append(gomega_next)
-            ly["mlp"].backward(gouts, sv.pre_lat[l], [gX[:, : S * (l + 1)], gs], [True, gs_acc])
+            if not (ly["last"] and fused):
+                ly["mlp"].backward(gouts, sv.pre_lat[l], [gX[:, : S * (l + 1)], gs], [True, gs_acc])
             ggamma = torch.empty(N, D, U, dtype=self.acc, device=dev)
             if l == 0:
                 gw0 = torch.empty(E, self.nw, dtype=dt, device=dev)

@@ -147,6 +147,27 @@ int ab2_mlp2(int dtype, int backward, int64_t M, int K, int H, int N, int n_a, c
              void* const* o_ptr_host, const int64_t* o_ld_host, const int32_t* o_width_host,
              const int32_t* o_accum_host, void* stream);
 
+/* Last latent MLP + readout MLP in one tensor-core kernel per direction (two-layer SiLU MLPs, hidden width H).  The
+ * readout reads X[:, :P + S] and the last latent MLP reads [X[:, :P] | s] and writes x_L = X[:, P:P+S], with P = S L;
+ * x_L and its gradient stay on chip.  W1_ro = [W1_ro_a ; W1_ro_b] is the readout's first layer split by rows at P, w2_ro
+ * its H x 1 output layer (H fp32 values).
+ *   backward == 0:  reads x = X[:, :P] and s [M][U]; writes pre_l = [x | s] @ W1_lat, xl = x_L = silu(pre_l) @ W2_lat,
+ *                   pre_r = x @ W1_ro_a + x_L @ W1_ro_b and ez = Ez = silu(pre_r) @ w2_ro.
+ *                   w_packed = {W1_lat [P+U][H], W2_lat [H][S], W1_ro_a [P][H], W1_ro_b [S][H]}.
+ *   backward != 0:  reads ez = gEz [M][1], pre_l and pre_r; g_r = gEz w2_ro^T * silu'(pre_r),
+ *                   g_h = ((g_r @ W1_ro^T[:, P:]) @ W2_lat^T) * silu'(pre_l); writes x = gX[:, :P] =
+ *                   g_h @ W1_lat^T[:, :P] + g_r @ W1_ro^T[:, :P] and s = gs = g_h @ W1_lat^T[:, P:].  gX[:, P:] is not
+ *                   formed.  xl is unused.  w_packed = {W1_ro^T [H][P+S], W2_lat^T [S][H], W1_lat^T [H][P+U]}.
+ * All matrices are ab2_linear_pack images.  Numerics: pre_l, x_L, pre_r, gX[:, :P] and gs are bitwise those of the two
+ * ab2_mlp2 calls this replaces (forward: last latent, then readout; backward: rank-1 readout, then last latent).  Ez is
+ * an fp32 dot product of silu(pre_r) and w2_ro instead of the split-bf16 MMA, so it differs in the last bits.
+ * Returns AB2_NOT_ELIGIBLE (nothing enqueued, no error set) for dtype other than AB2_F32, H or S other than 64, P or U
+ * not multiples of 32, P + U above 512 (backward: above 256), operands not 16-byte aligned, a missing packed image, or a
+ * shared-memory plan that does not fit one SM.  The caller then runs the two MLPs separately. */
+int ab2_mlp2_readout(int dtype, int backward, int64_t M, int P, int S, int U, int H, void* x, int64_t x_ld, void* s, int64_t s_ld,
+                     void* xl, int64_t xl_ld, void* pre_l, int64_t pre_l_ld, void* pre_r, int64_t pre_r_ld, void* ez, int64_t ez_ld,
+                     const void* const* w_packed_host, const void* w2_ro, void* stream);
+
 /* _channels.py:44-57 + _contract.py:195-204 fused: gamma[c][j][u] =
  *   sf * sum_{z in row c} Y[z][j] * w[z][irrep(j)][u]      (a4, a7; deterministic, no atomics) */
 int ab2_env_sum(int dtype, int lmax, int64_t N, int U, const int32_t* row_ptr, const void* Y,

@@ -82,6 +82,12 @@ def main():
         dims = [S * (l + 1) + U, W, S + (0 if last else nw)]
         ops[f"linear@fwd.L{l}"] = mlp_fwd(E, b, dims)
         ops[f"linear@bwd.L{l}"] = mlp_bwd(E, b, dims, accum_in=S * (l + 1) + (0 if last else U))
+    # last latent MLP + readout in one kernel (ab2_mlp2_readout), P = S L, both hidden widths W:
+    #   forward  reads X[:, :P], s; writes pre_L, x_L, pre_r, Ez
+    #   backward reads gEz, pre_r, pre_L; writes gX[:, :P], gs
+    P = S * L
+    ops["mlp2_readout@fwd.L%d" % (L - 1)] = E * b * (P + U + W + S + W + 1)
+    ops["mlp2_readout@bwd.readout"] = E * b * (1 + W + W + P + U)
     k = d["kernels_ms_per_step"]
     rows, tot_ms, tot_b = [], 0.0, 0
     for name, ms in sorted(k.items(), key=lambda kv: -kv[1]):

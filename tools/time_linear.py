@@ -1,6 +1,7 @@
 """Micro-benchmark of ab2_linear on the GPU (tensor-core vs CUDA-core path, stage knock-outs).
 
     python tools/time_linear.py --mlp2   # ab2_mlp2 against the two launches it replaces, c2 shapes
+    python tools/time_linear.py --mlp2-readout   # ab2_mlp2_readout against the two ab2_mlp2 calls it replaces, c2 shapes
 """
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -97,6 +98,48 @@ def run_mlp2(name, backward, awid, H, owid, accum):
     print(f"mlp2 {name:12s} K={K:3d} H={H} N={N:3d}: two launches {t_pair*1e3:6.0f}us  fused {t_fused*1e3:6.0f}us "
           f"({M * floats * 4 / t_fused / 1e6:5.0f}GB/s)  {t_pair / t_fused:4.2f}x", flush=True)
 
+
+def run_mlp2_readout(S=64, U=32, H=64, L=2):
+    """ab2_mlp2_readout (last latent MLP + readout) against the two ab2_mlp2 calls it replaces, each direction."""
+    P = S * L
+    X = torch.randn(M, P + S, device=dev)
+    s = torch.randn(M, 3 * U, device=dev)[:, :U]
+    W1l, W2l, W1r, w2r = (torch.randn(P + U, H, device=dev) * 0.1, torch.randn(H, S, device=dev) * 0.1,
+                          torch.randn(P + S, H, device=dev) * 0.1, torch.randn(H, 1, device=dev) * 0.1)
+    W1rT, W2lT, W1lT = W1r.T.contiguous(), W2l.T.contiguous(), W1l.T.contiguous()
+    pk = _lib.linear_pack
+    fwd_p = [pk(W1l), pk(W2l), pk(W1r[:P].contiguous()), pk(W1r[P:].contiguous())]
+    bwd_p = [pk(W1rT), pk(W2lT), pk(W1lT)]
+    p1l, p2l, p1r, p2r, pT1r, pT2l, pT1l = pk(W1l), pk(W2l), pk(W1r), pk(w2r), pk(W1rT), pk(W2lT), pk(W1lT)
+    pre_l, pre_r, Ez, gEz = torch.randn(M, H, device=dev), torch.randn(M, H, device=dev), torch.empty(M, 1, device=dev), torch.randn(M, 1, device=dev)
+    gX, gs = torch.empty(M, P + S, device=dev), torch.empty(M, 3 * U, device=dev)[:, :U]
+    w2rT = w2r.T.contiguous()
+
+    def fwd_pair():
+        assert _lib.mlp2([X[:, :P], s], W1l, W2l, [X[:, P:]], pre_l, W1_packed=p1l, W2_packed=p2l)
+        assert _lib.mlp2([X], W1r, w2r, [Ez], pre_r, W1_packed=p1r, W2_packed=p2r)
+
+    def fwd_fused():
+        assert _lib.mlp2_readout(False, X[:, :P], s, X[:, P:], pre_l, pre_r, Ez, w2r, fwd_p, S)
+
+    def bwd_pair():
+        assert _lib.mlp2([gEz], w2rT, W1rT, [gX], pre_r, backward=True, W2_packed=pT1r)
+        assert _lib.mlp2([gX[:, P:]], W2lT, W1lT, [gX[:, :P], gs], pre_l, o_accum=[True, False], backward=True, W1_packed=pT2l, W2_packed=pT1l)
+
+    def bwd_fused():
+        assert _lib.mlp2_readout(True, gX[:, :P], gs, None, pre_l, pre_r, gEz, w2r, bwd_p, S)
+
+    # fused kernels' HBM traffic in floats per row (forward: X[:, :P], s in; pre_L, x_L, pre_r, Ez out;
+    # backward: gEz, pre_r, pre_L in; gX[:, :P], gs out)
+    for name, pair, fused, floats in (("fwd", fwd_pair, fwd_fused, P + U + H + S + H + 1), ("bwd", bwd_pair, bwd_fused, 1 + 2 * H + P + U)):
+        t_pair, t_fused = time_ms(pair), time_ms(fused)
+        print(f"mlp2_readout {name} P={P} S={S} U={U} H={H}: two mlp2 {t_pair*1e3:6.0f}us  fused {t_fused*1e3:6.0f}us "
+              f"({M * floats * 4 / t_fused / 1e6:5.0f}GB/s)  {t_pair / t_fused:4.2f}x", flush=True)
+
+
+if "--mlp2-readout" in sys.argv:
+    run_mlp2_readout()
+    sys.exit(0)
 
 if "--mlp2" in sys.argv:
     for shp in mlp2_shapes:
