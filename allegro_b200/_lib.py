@@ -46,6 +46,8 @@ _SIGNATURES = {
     "ab2_env_bwd": ([_i32, _i32, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _i64, _vp, _dbl, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_tp_fwd": ([_i32, _i32, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_tp_bwd": ([_i32, _i32, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp], C.c_int),
+    "ab2_tp_chain_fwd": ([_i32, _i32, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_tp_chain_bwd": ([_i32, _i32, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_edge_sum": ([_i32, _i64, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_edge_sum_bwd": ([_i32, _i64, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_force_scatter": ([_i32, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
@@ -465,6 +467,71 @@ def tp_bwd(dtype, lmax, N, E, U, d_in, d_out, tab, cgw, row_ptr, ctr, gamma, Vin
                 _ptr(gw0) if implicit else None, gw0_ld, _ptr(gY) if implicit else None, _ptr(ggamma), _stream(),
             )
         )
+
+
+def tp_chain_takes(dtype, U: int) -> bool:
+    """The storage types and widths ab2_tp_chain_fwd / ab2_tp_chain_bwd are built for: fp32, U = 32 or 64."""
+    return dtype == torch.float32 and U in (32, 64)
+
+
+def tp_chain_plan(dtype, U: int, cgw0: torch.Tensor, cgw1: torch.Tensor):
+    """What ab2_tp_chain_fwd / ab2_tp_chain_bwd need besides the per-call tensors: the two layers' coupling weights as
+    dense fp32 [nnz][U] device tensors.  None when the kernels do not take the case (``tp_chain_takes``, weights not on
+    a CUDA device); decided on the host, without the library.  The caller has checked that both tables have the baked
+    structure (Tab9x9x9, Tab9x9x1)."""
+    if not tp_chain_takes(dtype, U) or not cgw0.is_cuda:
+        return None
+    return {"cgw0": cgw0.to(torch.float32).contiguous(), "cgw1": cgw1.to(torch.float32).contiguous(), "U": U}
+
+
+def _chain_dense(t: torch.Tensor, shape, name: str):
+    if tuple(t.shape) != tuple(shape) or t.dtype != torch.float32:
+        raise ValueError(f"tp_chain: {name} is {tuple(t.shape)} {t.dtype}, expected {tuple(shape)} float32")
+    return _ptr(_contig(t, name))
+
+
+def tp_chain_fwd(plan, last: bool, row_ptr, ctr, gamma0, gamma1, Y, w0, s) -> bool:
+    """Composed tensor product, forward (ab2_tp_chain_fwd): s [E][U] = the layer-0 scalar V_1[:, 0] (last = False) or
+    the layer-1 output (last = True) from Y, w0 and the centres' gamma rows, without V_1.  Returns False, with nothing
+    computed, when ``plan`` is None or the library declines."""
+    if plan is None:
+        return False
+    E, U = s.shape
+    N = gamma0.shape[0]
+    args = [_chain_dense(gamma0, (N, 9, U), "gamma0"), _chain_dense(gamma1, (N, 9, U), "gamma1") if last else None,
+            _chain_dense(Y, (E, 9), "Y"), _chain_dense(w0, (E, 3 * U), "w0"), _chain_dense(s, (E, U), "s")]
+    timer = _timed("tp_chain_fwd", 1)
+    with timer:
+        rc = load().ab2_tp_chain_fwd(AB2_F32, int(last), N, E, U, _ptr(row_ptr), _ptr(ctr), _ptr(plan["cgw0"]), _ptr(plan["cgw1"]),
+                                     *args, _stream())
+    if rc == NOT_ELIGIBLE:
+        timer.cancel()
+        return False
+    _check(rc)
+    return True
+
+
+def tp_chain_bwd(plan, first: bool, row_ptr, ctr, gamma0, gamma1, Y, w0, g1, g2, gw0, gY, ggamma) -> bool:
+    """Composed tensor product, backward (ab2_tp_chain_bwd).  first = False: ggamma = the gradient of gamma1 from g2.
+    first = True: gw0, gY (+=) and ggamma = the gradient of gamma0 from g1 and g2.  Returns False, with nothing
+    computed, when ``plan`` is None or the library declines."""
+    if plan is None:
+        return False
+    E, U = g2.shape
+    N = gamma0.shape[0]
+    args = [_chain_dense(gamma0, (N, 9, U), "gamma0"), _chain_dense(gamma1, (N, 9, U), "gamma1") if first else None,
+            _chain_dense(Y, (E, 9), "Y"), _chain_dense(w0, (E, 3 * U), "w0"), _chain_dense(g1, (E, U), "g1") if first else None,
+            _chain_dense(g2, (E, U), "g2"), _chain_dense(gw0, (E, 3 * U), "gw0") if first else None,
+            _chain_dense(gY, (E, 9), "gY") if first else None, _chain_dense(ggamma, (N, 9, U), "ggamma")]
+    timer = _timed("tp_chain_bwd", 1)
+    with timer:
+        rc = load().ab2_tp_chain_bwd(AB2_F32, int(first), N, E, U, _ptr(row_ptr), _ptr(ctr), _ptr(plan["cgw0"]), _ptr(plan["cgw1"]),
+                                     *args, _stream())
+    if rc == NOT_ELIGIBLE:
+        timer.cancel()
+        return False
+    _check(rc)
+    return True
 
 
 def edge_sum(Ez: torch.Tensor, row_ptr: torch.Tensor, factor: float) -> torch.Tensor:

@@ -39,7 +39,21 @@ def _env_perm(U: int, n_ir: int, individual: bool = True) -> torch.Tensor:
 
 
 class _Saved:
-    __slots__ = ("csr", "vec", "Y", "w0", "omega", "V", "gamma", "pre_lat", "pre_read", "X", "fold")
+    __slots__ = ("csr", "vec", "Y", "w0", "omega", "V", "gamma", "pre_lat", "pre_read", "X", "fold", "chain")
+
+
+_BAKED_TABLES = {}
+
+
+def _baked_table(d_out: int) -> torch.Tensor:
+    """(i, j, k) structure of the l_max = 2 coupling tables baked into the composed tensor-product kernels
+    (Tab9x9x9 / Tab9x9x1 in csrc/tp_tables_generated.cuh, generated from the same Contracter)."""
+    if d_out not in _BAKED_TABLES:
+        from ._contract import Contracter
+
+        ir = "1x0e+1x1o+1x2e"
+        _BAKED_TABLES[d_out] = Contracter(ir, ir, ir if d_out == 9 else "1x0e", mul=1).sparse_table()[0].cpu()
+    return _BAKED_TABLES[d_out]
 
 
 class AllegroCore:
@@ -123,6 +137,16 @@ class AllegroCore:
                 Ws = self.layers[l]["mlp"].WT[0][:, S * (l + 1) : S * (l + 1) + U].contiguous()
                 self.gsW.append(Ws)
                 self.gsWp.append(_lib.linear_pack(Ws))
+        # the two tensor products composed per centre (ab2_tp_chain_*, DESIGN.md section 4.1): a two-layer l_max = 2
+        # model whose tables have the baked structure, default backward, and (tp_chain_plan) fp32 with U = 32 or 64.
+        # Then the forward keeps the compact scalars s_1, s_2 instead of V_1, and the backward passes the compact
+        # gradients g1, g2 instead of gV_1.
+        self.chain = None
+        l0, l1 = (self.layers + [None, None])[:2]
+        if (self.L == 2 and not self.plain_ok and self.D == 9
+                and (l0["d_in"], l0["d_out"], l1["d_in"], l1["d_out"]) == (9, 9, 9, 1)
+                and torch.equal(l0["tab"].cpu(), _baked_table(9)) and torch.equal(l1["tab"].cpu(), _baked_table(1))):
+            self.chain = _lib.tp_chain_plan(dtype, U, l0["cgw"], l1["cgw"])
 
     # ------------------------------------------------------------------------------------
     def forward(self, csr: EdgeCSR, vec: torch.Tensor, x_emb: Optional[torch.Tensor], keep: bool = True, fill_embed=None):
@@ -149,13 +173,23 @@ class AllegroCore:
         gammas, pre_lat = [], []
         Ez = torch.empty(E, 1, dtype=dt, device=dev)
         pre_read = None
+        chain = self.chain
         for l, ly in enumerate(self.layers):
             _lib.set_tag(f"fwd.L{l}")
             gamma = _lib.env_sum(dt, self.lmax, N, U, csr.row_ptr, Y, omega[l], self.sf)
-            Vn = torch.empty(E, ly["d_out"], U, dtype=dt, device=dev)
-            _lib.tp_fwd(dt, self.lmax, N, E, U, ly["d_in"], ly["d_out"], ly["tab"], ly["cgw"], csr.row_ptr, csr.ctr, gamma,
-                        V[l], Y, w0 if l == 0 else None, Vn)
-            s = Vn.view(E, ly["d_out"] * U)[:, :U]  # scalar (k=0) slab, _allegro.py:272-275
+            Vn = None
+            if chain is not None:
+                # composed path: s_1 = V_1[:, 0] from gamma_0, then s_2 from gamma_0 and gamma_1; V_1 is not formed
+                s = torch.empty(E, U, dtype=dt, device=dev)
+                if not _lib.tp_chain_fwd(chain, ly["last"], csr.row_ptr, csr.ctr, gammas[0] if l else gamma, gamma if l else None, Y, w0, s):
+                    if l:
+                        raise RuntimeError("tp_chain_fwd declined the last layer after taking the first")
+                    chain = None  # declined (e.g. no edges): this call takes the stored-V path throughout
+            if chain is None:
+                Vn = torch.empty(E, ly["d_out"], U, dtype=dt, device=dev)
+                _lib.tp_fwd(dt, self.lmax, N, E, U, ly["d_in"], ly["d_out"], ly["tab"], ly["cgw"], csr.row_ptr, csr.ctr, gamma,
+                            V[l], Y, w0 if l == 0 else None, Vn)
+                s = Vn.view(E, ly["d_out"] * U)[:, :U]  # scalar (k=0) slab, _allegro.py:272-275
             outs = [X[:, S * (l + 1) : S * (l + 2)]]
             if not ly["last"]:
                 omega.append(torch.empty(E, self.nw, dtype=dt, device=dev))
@@ -176,6 +210,7 @@ class AllegroCore:
             pre_read = self.readout.forward([X], [Ez])
         Ei = _lib.edge_sum(Ez.view(E).to(self.acc), csr.row_ptr, self.factor)
         sv.Y, sv.w0, sv.omega, sv.V, sv.gamma, sv.pre_lat, sv.pre_read, sv.X = Y, w0, omega, V, gammas, pre_lat, pre_read, X
+        sv.chain = chain
         return Ei, X, Ez, sv
 
     # ------------------------------------------------------------------------------------
@@ -266,6 +301,8 @@ class AllegroCore:
         gV_next: Optional[torch.Tensor] = None   # grad wrt V_{l+1}
         gomega_next: Optional[torch.Tensor] = None  # grad wrt omega_{l+1}
         gw0 = None
+        chain = sv.chain
+        g1 = None  # composed path: d/ds_1 [E][U]; d/ds_2 is gV_last
         for l in range(L - 1, -1, -1):
             ly = self.layers[l]
             _lib.set_tag(f"bwd.L{l}")
@@ -274,14 +311,27 @@ class AllegroCore:
                 gs_acc = False
             else:
                 gs_acc = True
-            gs = gV_next.view(E, ly["d_out"] * U)[:, :U]
+            if chain is not None and not ly["last"]:
+                g1 = torch.empty(E, U, dtype=dt, device=dev)
+                gs, gs_acc = g1, False
+            else:
+                gs = gV_next.view(E, ly["d_out"] * U)[:, :U]
             gouts = [gX[:, S * (l + 1) : S * (l + 2)]]
             if not ly["last"]:
                 gouts.append(gomega_next)
             if not (ly["last"] and fused):
                 ly["mlp"].backward(gouts, sv.pre_lat[l], [gX[:, : S * (l + 1)], gs], [True, gs_acc])
             ggamma = torch.empty(N, D, U, dtype=self.acc, device=dev)
-            if l == 0:
+            if chain is not None:
+                # last layer: gamma_1's gradient from g2; first layer: gw0, gY and gamma_0's gradient from g1 and g2
+                if l == 0:
+                    gw0 = torch.empty(E, self.nw, dtype=dt, device=dev)
+                ok = _lib.tp_chain_bwd(chain, l == 0, csr.row_ptr, csr.ctr, sv.gamma[0], sv.gamma[1] if l == 0 else None, sv.Y, sv.w0, g1,
+                                       gV_last.view(E, U), gw0, gY if l == 0 else None, ggamma)
+                if not ok:
+                    raise RuntimeError("tp_chain_bwd declined a case its forward took")
+                gV_in = None
+            elif l == 0:
                 gw0 = torch.empty(E, self.nw, dtype=dt, device=dev)
                 _lib.tp_bwd(dt, self.lmax, N, E, U, ly["d_in"], ly["d_out"], ly["tab"], ly["cgw"], csr.row_ptr, csr.ctr,
                             sv.gamma[l], None, sv.Y, sv.w0, gV_next, None, gw0, gY, ggamma)

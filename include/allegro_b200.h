@@ -202,6 +202,33 @@ int ab2_tp_bwd(int dtype, int lmax, int64_t N, int64_t E, int U, int d_in, int d
                int64_t w0_ld, const void* gVout, void* gVin, void* gw0, int64_t gw0_ld, void* gY,
                void* ggamma, void* stream);
 
+/* The two tensor products of a two-layer l_max = 2 model composed per centre, so that the layer-1 features V_1 and
+ * their gradient are never formed (_allegro.py:237-301 with nothing between the layers on the tensor track).
+ * Layer 0 is 9 x 9 -> 9 with implicit V_0, layer 1 is 9 x 9 -> 1; cgw0 [83][U] and cgw1 [9][U] are in the order of
+ * the baked structures Tab9x9x9 / Tab9x9x1 (tp_tables_generated.cuh), which the caller checks on the host.  Per
+ * channel u, with v0[i] = Y[z][i] w0[z][l(i)][u]:
+ *   M0_c[i][k] = sum_{(i,j,k) in tab0} cgw0 gamma0[c][j],   M1_c[k] = sum_{(k,j,0) in tab1} cgw1 gamma1[c][j]
+ *   A_c[i] = M0_c[i][0],   B_c[i] = sum_k M0_c[i][k] M1_c[k]
+ * Forward:  last = 0: s[z][u] = sum_i A_c[i] v0[i]  (= V_1[z][0][u]);  last = 1: s[z][u] = sum_i B_c[i] v0[i]
+ *           (= the layer-1 output);  gamma1 / cgw1 are only read when last = 1.
+ * Backward, g1 = d/ds_1 and g2 = d/ds_2 as [E][U]:
+ *   first = 0: ggamma[c][j] = gamma1's gradient = sum_{(k,j,0) in tab1} cgw1 sum_i M0_c[i][k] G_c[i],
+ *              G_c[i] = sum_{z in c} g2[z] v0[i]   (reads Y, w0, g2; g1 / gw0 / gY unused)
+ *   first = 1: gv0[i] = A_c[i] g1 + B_c[i] g2;  gw0[z][l][u] = sum_{i in l} Y[z][i] gv0[i];
+ *              gY[z][i] += sum_u w0[z][l(i)][u] gv0[i];
+ *              ggamma[c][j] = gamma0's gradient = sum_{(i,j,k) in tab0} cgw0 (delta_k0 H_c[i] + M1_c[k] G_c[i]),
+ *              H_c[i] = sum_{z in c} g1[z] v0[i]
+ * ggamma is written once per centre (zero for centres without edges), in a fixed order, no atomics.  All buffers are
+ * fp32 and dense: Y / gY [E][9], w0 / gw0 [E][3U], s / g1 / g2 [E][U], gamma0 / gamma1 / ggamma [N][9][U].  Returns
+ * AB2_NOT_ELIGIBLE (nothing enqueued, no error set) for dtype other than AB2_F32, U other than 32 or 64, E >= 2^31, or
+ * a gamma / w0 / g1 / g2 base that is null or not 16-byte aligned. */
+int ab2_tp_chain_fwd(int dtype, int last, int64_t N, int64_t E, int U, const int32_t* row_ptr, const int32_t* ctr,
+                     const void* cgw0, const void* cgw1, const void* gamma0, const void* gamma1, const void* Y,
+                     const void* w0, void* s, void* stream);
+int ab2_tp_chain_bwd(int dtype, int first, int64_t N, int64_t E, int U, const int32_t* row_ptr, const int32_t* ctr,
+                     const void* cgw0, const void* cgw1, const void* gamma0, const void* gamma1, const void* Y,
+                     const void* w0, const void* g1, const void* g2, void* gw0, void* gY, void* ggamma, void* stream);
+
 /* edgewise.py:40-60 (a12): Ei[c] = factor * sum_{z in row c} Ez[z]   (TAcc, deterministic). */
 int ab2_edge_sum(int acc_dtype, int64_t N, const int32_t* row_ptr, const void* Ez, double factor,
                  void* Ei, void* stream);

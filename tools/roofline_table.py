@@ -88,6 +88,13 @@ def main():
     P = S * L
     ops["mlp2_readout@fwd.L%d" % (L - 1)] = E * b * (P + U + W + S + W + 1)
     ops["mlp2_readout@bwd.readout"] = E * b * (1 + W + W + P + U)
+    # two-layer models: the tensor products composed per centre (ab2_tp_chain_*), no V_1 / gV_1; per edge Y, w0 and the
+    # compact [E][U] scalars or their gradients, per centre the gamma rows read and (backward) ggamma written
+    per_edge_chain = b * nw + acc * D + 4
+    ops["tp_chain_fwd@fwd.L0"] = E * (per_edge_chain + b * U) + N * acc * D * U
+    ops["tp_chain_fwd@fwd.L1"] = E * (per_edge_chain + b * U) + 2 * N * acc * D * U
+    ops["tp_chain_bwd@bwd.L1"] = E * (per_edge_chain + b * U) + 2 * N * acc * D * U
+    ops["tp_chain_bwd@bwd.L0"] = E * (2 * b * nw + 3 * acc * D + 4 + 2 * b * U) + 3 * N * acc * D * U
     k = d["kernels_ms_per_step"]
     rows, tot_ms, tot_b = [], 0.0, 0
     for name, ms in sorted(k.items(), key=lambda kv: -kv[1]):
