@@ -337,62 +337,6 @@ def test_tp_fwd_bwd_implicit_v0(lmax, dtype, U, tp_fast):
     assert _rel(ggam.transpose(1, 2), ggam_ref) < (tol if dtype != torch.bfloat16 else 1e-5)
 
 
-@pytest.mark.parametrize("s3,gyt", [(1, 1), (0, 1), (0, 0)], ids=["stream3", "stream", "stream_shfl"])
-def test_tp_stream_ragged_rows(s3, gyt):
-    """Layer-0 streaming kernels on a ragged CSR with more centres than CTAs: empty centres (also leading / trailing), rows of
-    1-3 edges (several centres begin inside one 8-edge stage), rows far longer than a stage.  Reference: the shape-generic
-    kernels on the same device data (themselves held to the oracle above); ggamma of empty centres must come back zero and
-    two runs must agree bitwise (every reduction is fixed-order)."""
-    g = torch.Generator().manual_seed(11)
-    N, U, lmax, Dd, n_ir = 3000, 32, 2, 9, 3
-    deg = torch.randint(0, 4, (N,), generator=g)
-    deg[torch.randint(0, N, (300,), generator=g)] = 0
-    deg[torch.randint(0, N, (40,), generator=g)] = torch.randint(60, 200, (40,), generator=g)
-    deg[:5] = 0
-    deg[-7:] = 0
-    ctr = torch.repeat_interleave(torch.arange(N), deg)
-    E = int(ctr.numel())
-    csr = D.build_csr(torch.stack([ctr, torch.randint(0, N, (E,), generator=g)]).to(DEV), N)
-    _, b = _tp_case(lmax, 0, 2, U, True, torch.float32)
-    ijk, _, _ = b.sparse_table()
-    tab, cgw = ijk.to(DEV), b.cgw(torch.float32, DEV)
-    Y = torch.randn(E, Dd, generator=g).to(DEV)
-    w0 = torch.randn(E, n_ir * U, generator=g).to(DEV)
-    gam = torch.randn(N, Dd, U, generator=g).to(DEV)
-    gout = torch.randn(E, Dd, U, generator=g).to(DEV)
-
-    def run():
-        Vout = torch.empty(E, Dd, U, device=DEV)
-        gw0 = torch.full((E, n_ir * U), float("nan"), device=DEV)
-        gY = torch.ones(E, Dd, device=DEV)  # accumulated into
-        ggam = torch.full((N, Dd, U), float("nan"), device=DEV)
-        _lib.tp_fwd(torch.float32, lmax, N, E, U, Dd, Dd, tab, cgw, csr.row_ptr, csr.ctr, gam, None, Y, w0, Vout)
-        _lib.tp_bwd(torch.float32, lmax, N, E, U, Dd, Dd, tab, cgw, csr.row_ptr, csr.ctr, gam, None, Y, w0, gout, None, gw0, gY, ggam)
-        torch.cuda.synchronize()
-        return Vout, gw0, gY, ggam
-
-    try:
-        _lib.set_option("tp_fast", 0)
-        _lib.set_option("tp_stream", 0)
-        ref = run()
-        _lib.set_option("tp_fast", 1)
-        _lib.set_option("tp_stream", 1)
-        _lib.set_option("tp_stream3", s3)
-        _lib.set_option("tp_stream_gytile", gyt)
-        got, again = run(), run()
-    finally:
-        _lib.set_option("tp_fast", 1)
-        _lib.set_option("tp_stream", 1)
-        _lib.set_option("tp_stream3", 1)
-        _lib.set_option("tp_stream_gytile", 1)
-    for name, a, r in zip(("Vout", "gw0", "gY", "ggamma"), got, ref):
-        assert bool(torch.isfinite(a).all()), name
-        assert _rel(a, r) < 2e-5, name
-    assert bool((got[3][deg == 0] == 0).all())
-    for name, a, c in zip(("Vout", "gw0", "ggamma"), (got[0], got[1], got[3]), (again[0], again[1], again[3])):
-        assert torch.equal(a, c), name
-
-
 @pytest.mark.parametrize("layer", [0, 1, 2])
 @pytest.mark.parametrize("implicit", [False, True])
 def test_tp_baked64_matches_generic(layer, implicit):
