@@ -72,6 +72,11 @@ _SIGNATURES = {
     "ab2_nl_count": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_nl_fill": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_radial_bwd": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_nl_frames_count": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
+    "ab2_nl_frames_fill": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_frame_scratch_elems": ([_i64, _i64], C.c_int64),
+    "ab2_frame_sum": ([_i32, _i64, _i64, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
+    "ab2_frame_virial": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
 }
 
 
@@ -701,3 +706,60 @@ def radial_pq_bwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table,
         _check(load().ab2_radial_pq_bwd(DTYPE_ENUM[dtype], E, S, bessel_w.numel(), float(p_cut), _ptr(vec), _ptr(ctr), _ptr(nbr), _ptr(types),
                                         _ptr(rmax_table), rmax_table.shape[0], _ptr(bessel_w), _ptr(_contig(PQ, "PQ")), _ptr(_contig(g_out, "g_out")),
                                         _ptr(_contig(aux, "aux")) if aux is not None else None, _ptr(gvec), _stream()))
+
+
+# --------------------------------------------------------------------------- #
+# batches of frames (many small frames concatenated into one graph)
+# --------------------------------------------------------------------------- #
+def nl_frames(pos: torch.Tensor, frame_ptr: torch.Tensor, cell: torch.Tensor, inv_cell: torch.Tensor, pbc: torch.Tensor, r_max: float):
+    """All-pairs search per frame (ab2_nl_frames_count / fill) -> (row_ptr [n+1] int32, nbr [E] int32, shift_vec [E,3] pos
+    dtype).  frame_ptr [B+1] int32, cell / inv_cell [B,3,3] in the positions' dtype, pbc [B,3] int32, all on the device.
+    Rows are ordered by neighbour, then by image (x, y, z) lexicographically."""
+    n, B = pos.shape[0], frame_ptr.shape[0] - 1
+    dt = DTYPE_ENUM[pos.dtype]
+    pos = _contig(pos, "pos")
+    args = (_ptr(_contig(frame_ptr, "frame_ptr")), _ptr(pos), _ptr(_contig(cell, "cell")), _ptr(_contig(inv_cell, "inv_cell")),
+            _ptr(_contig(pbc, "pbc")), float(r_max))
+    counts = torch.empty(n, dtype=torch.int32, device=pos.device)
+    with _timed("nl_frames_count"):
+        _check(load().ab2_nl_frames_count(dt, n, B, *args, _ptr(counts), _stream()))
+    row_ptr = torch.zeros(n + 1, dtype=torch.int32, device=pos.device)
+    row_ptr[1:] = torch.cumsum(counts, 0).to(torch.int32)
+    E = int(row_ptr[-1])
+    nbr = torch.empty(E, dtype=torch.int32, device=pos.device)
+    shift = torch.empty(E, 3, dtype=pos.dtype, device=pos.device)
+    if E:
+        with _timed("nl_frames_fill"):
+            _check(load().ab2_nl_frames_fill(dt, n, B, *args, _ptr(row_ptr), _ptr(nbr), _ptr(shift), _stream()))
+    return row_ptr, nbr, shift
+
+
+def _frame_scratch(total: int, B: int, width: int, device):
+    m = int(load().ab2_frame_scratch_elems(int(total), int(B))) * width
+    return torch.empty(max(m, 1), dtype=torch.float64, device=device), m
+
+
+def frame_sum(x: torch.Tensor, frame_ptr: torch.Tensor) -> torch.Tensor:
+    """out[b] = sum of x over the atoms [frame_ptr[b], frame_ptr[b+1])  (ab2_frame_sum; fixed order, no atomics)."""
+    B = frame_ptr.shape[0] - 1
+    n = x.numel()
+    out = torch.empty(B, dtype=x.dtype, device=x.device)
+    scratch, m = _frame_scratch(n, B, 1, x.device)
+    with _timed("frame_sum", 2):
+        _check(load().ab2_frame_sum(DTYPE_ENUM[x.dtype], n, B, _ptr(_contig(frame_ptr, "frame_ptr")), _ptr(_contig(x, "x")), _ptr(scratch), m,
+                                    _ptr(out), _stream()))
+    return out
+
+
+def frame_virial(vec: torch.Tensor, gvec: torch.Tensor, frame_ptr: torch.Tensor, row_ptr: torch.Tensor) -> torch.Tensor:
+    """W[b] = sum over frame b's edges [row_ptr[frame_ptr[b]], row_ptr[frame_ptr[b+1]]) of vec (x) gvec -> [B,3,3] in
+    vec's dtype  (ab2_frame_virial; fixed order, no atomics)."""
+    B = frame_ptr.shape[0] - 1
+    E = vec.shape[0]
+    assert gvec.dtype == vec.dtype and gvec.shape == vec.shape
+    W = torch.empty(B, 3, 3, dtype=vec.dtype, device=vec.device)
+    scratch, m = _frame_scratch(E, B, 9, vec.device)
+    with _timed("frame_virial", 2):
+        _check(load().ab2_frame_virial(DTYPE_ENUM[vec.dtype], E, B, _ptr(_contig(frame_ptr, "frame_ptr")), _ptr(_contig(row_ptr, "row_ptr")),
+                                       _ptr(_contig(vec, "vec")), _ptr(_contig(gvec, "gvec")), _ptr(scratch), m, _ptr(W), _stream()))
+    return W

@@ -294,3 +294,68 @@ def neighbor_csr(pos: torch.Tensor, r_max: float, cell: torch.Tensor, pbc=(True,
     ctr = torch.repeat_interleave(torch.arange(nc, device=pos.device, dtype=torch.int32), counts.long())
     maxdeg = int(counts.max()) if nc > 0 else 0
     return EdgeCSR(nc, ctr.contiguous(), nbr, row_ptr, None, maxdeg), shift
+
+
+# Largest frame neighbor_csr_frames takes: its search is all-pairs per frame, O(N_b^2 * images).  Larger frames belong to
+# neighbor_csr (cell list) or neighbor_list.
+FRAMES_MAX_ATOMS = 4096
+
+
+def _frames_pbc(pbc, B: int, device) -> torch.Tensor:
+    if pbc is None:
+        return torch.zeros(B, 3, dtype=torch.bool, device=device)
+    if isinstance(pbc, bool):
+        pbc = (pbc,) * 3
+    t = torch.as_tensor(pbc, dtype=torch.bool, device=device)
+    if t.dim() == 1:
+        t = t.expand(B, 3)
+    if tuple(t.shape) != (B, 3):
+        raise ValueError(f"pbc has shape {tuple(t.shape)}, expected (3,) or ({B}, 3)")
+    return t
+
+
+def neighbor_csr_frames(pos: torch.Tensor, frame_ptr, cell: Optional[torch.Tensor], pbc, r_max: float):
+    """Neighbour lists of a batch of small frames in one pass on the device (ab2_nl_frames_count / fill), straight into the
+    kernels' format -> (EdgeCSR over all atoms of the batch, shift_vec [E,3] in the positions' dtype).
+
+    ``frame_ptr`` [B+1]: the atoms of frame b are [frame_ptr[b], frame_ptr[b+1]).  ``cell`` [B,3,3] (or None: no frame is
+    periodic), ``pbc`` [B,3] or (3,) booleans.  Any cell ``neighbor_list`` takes: triclinic, narrower than r_max, mixed
+    periodicity; a frame with no periodic axis is a molecule (its cell is not used).  Rows are those of
+    ``neighbor_list(frame, method="brute")`` in the same order (by neighbour, then by image), with the frame's atom offset
+    added;  r = pos[nbr] + shift - pos[ctr]  holds for the raw positions.  Frames above FRAMES_MAX_ATOMS atoms are rejected:
+    the search is all-pairs per frame."""
+    from . import _lib
+
+    dev = pos.device
+    fp = torch.as_tensor(frame_ptr).reshape(-1).to(device="cpu", dtype=torch.int64)
+    B = fp.shape[0] - 1
+    n = pos.shape[0]
+    if B < 1 or int(fp[0]) != 0 or int(fp[-1]) != n or bool((fp[1:] < fp[:-1]).any()):
+        raise ValueError(f"frame_ptr must rise from 0 to the number of atoms ({n})")
+    big = int((fp[1:] - fp[:-1]).max())
+    if big > FRAMES_MAX_ATOMS:
+        raise ValueError(f"neighbor_csr_frames takes frames of at most {FRAMES_MAX_ATOMS} atoms (got {big}); "
+                         "use neighbor_csr or neighbor_list for large frames")
+    pbc_t = _frames_pbc(pbc, B, dev)
+    periodic = pbc_t.any(dim=1)
+    if cell is None:
+        if bool(periodic.any()):
+            raise ValueError("periodic frames need a cell")
+        cell64 = torch.zeros(B, 3, 3, dtype=torch.float64, device=dev)
+    else:
+        if cell.numel() != 9 * B:
+            raise ValueError(f"cell has {cell.numel()} entries for {B} frames")
+        cell64 = cell.reshape(B, 3, 3).to(device=dev, dtype=torch.float64)
+    # a frame with no periodic axis is searched as it is: its cell never enters (zeros keep the shift vectors exactly 0)
+    cell64 = torch.where(periodic.view(B, 1, 1), cell64, torch.zeros_like(cell64))
+    eye = torch.eye(3, dtype=torch.float64, device=dev).expand(B, 3, 3)
+    det = torch.linalg.det(torch.where(periodic.view(B, 1, 1), cell64, eye))
+    if not bool(torch.isfinite(det).all()) or bool((det == 0).any()):
+        raise ValueError("a periodic frame has a singular cell")
+    inv64 = torch.where(periodic.view(B, 1, 1), torch.linalg.inv(torch.where(periodic.view(B, 1, 1), cell64, eye)), torch.zeros_like(cell64))
+    row_ptr, nbr, shift = _lib.nl_frames(pos.contiguous(), fp.to(device=dev, dtype=torch.int32), cell64.to(pos.dtype).contiguous(),
+                                         inv64.to(pos.dtype).contiguous(), pbc_t.to(torch.int32).contiguous(), float(r_max))
+    counts = row_ptr[1:] - row_ptr[:-1]
+    ctr = torch.repeat_interleave(torch.arange(n, device=dev, dtype=torch.int32), counts.long())
+    maxdeg = int(counts.max()) if n > 0 else 0
+    return EdgeCSR(n, ctr.contiguous(), nbr, row_ptr, None, maxdeg), shift

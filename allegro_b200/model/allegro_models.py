@@ -190,10 +190,12 @@ class FusedAllegroEnergy(torch.nn.Module):
         summed into one total energy."""
         b = data.get(D.BATCH_KEY)
         if b is not None and b.numel() > 0 and int(b.max()) > 0:
-            raise NotImplementedError("allegro_b200: batched frames are not supported on the fused path; evaluate frames one at a time")
+            raise NotImplementedError("allegro_b200: batched frames are not supported by the single-frame entry points; "
+                                      "use energy_and_forces_frames")
         c = data.get(D.CELL_KEY)
         if c is not None and c.numel() != 9:
-            raise NotImplementedError("allegro_b200: more than one cell in `data` (batched frames) is not supported")
+            raise NotImplementedError("allegro_b200: more than one cell in `data` (batched frames) is not supported by the "
+                                      "single-frame entry points; use energy_and_forces_frames")
 
     def _energy_and_forces(self, data: D.Type, stress: bool) -> D.Type:
         self._single_frame(data)
@@ -249,6 +251,135 @@ class FusedAllegroEnergy(torch.nn.Module):
             sym = 0.5 * (virial + virial.T)
             out[D.STRESS_KEY] = (sym / volume).to(pos.dtype).unsqueeze(0)
             out[D.VIRIAL_KEY] = (-sym).to(pos.dtype).unsqueeze(0)
+        return out
+
+    # ------------------------------------------------------------------------------------
+    # many frames per call
+    # ------------------------------------------------------------------------------------
+    def energy_and_forces_frames(self, data: D.Type, stress: bool = False) -> D.Type:
+        """Energies and forces of a BATCH of frames in one pass: the frames are one larger graph to the kernels (every
+        reduction on the path is per centre or per atom), and the per-frame sums are fixed-order segmented reductions
+        (ab2_frame_sum / ab2_frame_virial), so a frame's results do not depend on the rest of the batch.
+
+        ``data`` is nequip's batched layout: ``pos``, ``atom_types``, ``batch`` [N] (non-decreasing), ``num_atoms`` [B] and
+        either ``edge_index`` with global atom indices (+ ``cell`` [B,3,3] and ``edge_cell_shift``), or the prepared
+        ``edge_csr`` + ``edge_shift_vec`` of ``data.neighbor_csr_frames`` (``batch.collate`` builds either).  Writes
+        ``atomic_energy`` [N,1], ``forces`` [N,3], ``edge_energy`` / ``edge_features`` (input edge order) and
+        ``total_energy`` [B,1]; with ``stress=True`` also ``stress`` / ``virial`` [B,3,3], which need a non-singular cell
+        on every frame."""
+        pos = data[D.POSITIONS_KEY]
+        if not pos.is_cuda:
+            raise RuntimeError("allegro_b200: inputs must be CUDA tensors (no CPU fallback on the hot path)")
+        return self._energy_and_forces_frames(data, stress)
+
+    @staticmethod
+    def _frame_layout(batch: torch.Tensor, num: Optional[torch.Tensor], csr: D.EdgeCSR, n: int):
+        """Host validation of a batch (once per neighbour list) -> (frame_ptr [B+1] int32 on the device, B)."""
+        batch = batch.reshape(-1)
+        if batch.shape[0] != n:
+            raise ValueError(f"`batch` has {batch.shape[0]} entries for {n} atoms")
+        if n > 1 and bool((batch[1:] < batch[:-1]).any()):
+            raise ValueError("`batch` must be non-decreasing: the atoms of a frame must be contiguous")
+        if num is not None:
+            B = int(num.numel())
+        elif n > 0:
+            B = int(batch.max()) + 1
+        else:
+            raise ValueError("an empty batch needs `num_atoms`")
+        if B < 1:
+            raise ValueError("a batch needs at least one frame")
+        if n > 0 and (int(batch[0]) < 0 or int(batch[-1]) >= B):
+            raise ValueError(f"`batch` indexes frames outside [0, {B})")
+        counts = torch.bincount(batch.long(), minlength=B)
+        if num is not None and not torch.equal(counts.cpu(), num.reshape(-1).long().cpu()):
+            raise ValueError("`num_atoms` disagrees with `batch`")
+        if csr.num_atoms != n:
+            raise ValueError(f"the neighbour list has rows for {csr.num_atoms} of {n} atoms; a batch needs a row per atom")
+        if csr.num_edges:
+            if int(csr.nbr.max()) >= n or int(csr.nbr.min()) < 0:
+                raise ValueError("edge neighbour index out of range")
+            b64 = batch.long()
+            if bool((b64[csr.ctr.long()] != b64[csr.nbr.long()]).any()):
+                raise ValueError("an edge joins atoms of two different frames")
+        frame_ptr = torch.zeros(B + 1, dtype=torch.int32, device=csr.row_ptr.device)
+        frame_ptr[1:] = torch.cumsum(counts, 0).to(device=frame_ptr.device, dtype=torch.int32)
+        return frame_ptr, B
+
+    def _energy_and_forces_frames(self, data: D.Type, stress: bool) -> D.Type:
+        pos = data[D.POSITIONS_KEY]
+        core = self.core()
+        n = pos.shape[0]
+        if D.BATCH_KEY not in data:
+            raise ValueError("energy_and_forces_frames needs `batch` (and `num_atoms`): see allegro_b200.batch.collate")
+        batch, num = data[D.BATCH_KEY], data.get(D.NUM_NODES_KEY)
+        prepared = D.CSR_KEY in data
+        if prepared:
+            csr = data[D.CSR_KEY]
+            lsrc = (csr.row_ptr, csr.nbr)
+        else:
+            ei = data[D.EDGE_INDEX_KEY]
+            csr = self._cached("frames_csr", (ei,), (tuple(ei.shape), n), lambda: D.build_csr(ei, n))
+            lsrc = (ei,)
+        frame_ptr, B = self._cached("frames_layout", (batch,) + ((num,) if num is not None else ()) + lsrc, (n, id(csr)),
+                                    lambda: self._frame_layout(batch, num, csr, n))
+        shift_vec = None
+        cell = data.get(D.CELL_KEY)
+        if cell is not None and cell.numel() != 9 * B:
+            raise ValueError(f"`cell` has {cell.numel()} entries for {B} frames (expected [B,3,3])")
+        if prepared:
+            shift_vec = data.get(D.EDGE_SHIFT_VEC_KEY)
+            if shift_vec is not None:
+                shift_vec = shift_vec.to(pos.dtype).contiguous()
+        elif D.EDGE_CELL_SHIFT_KEY in data and cell is not None:
+            sh = data[D.EDGE_CELL_SHIFT_KEY]
+
+            def _shift():
+                s = sh if csr.perm is None else sh[csr.perm]
+                cb = cell.reshape(B, 3, 3).to(pos.dtype)[batch.reshape(-1).long()[csr.ctr.long()]]   # cell of each edge's frame
+                return (s.to(pos.dtype).unsqueeze(1) @ cb).squeeze(1).contiguous()
+
+            shift_vec = self._cached("frames_shift", (sh, cell, batch), (id(csr), pos.dtype), _shift)
+        volume = None
+        if stress:
+            if cell is None:
+                raise ValueError("stress=True needs a cell on every frame")
+
+            def _volume():
+                c = cell.reshape(B, 3, 3).to(core.acc)
+                v = (c[:, 0] * torch.linalg.cross(c[:, 1], c[:, 2])).sum(-1).abs()
+                if bool((v == 0).any()):
+                    raise ValueError("stress=True needs a non-singular cell on every frame")
+                return v
+
+            volume = self._cached("frames_volume", (cell,), (B, core.acc), _volume)
+        types_in = data[D.ATOM_TYPE_KEY]
+        types = types_in.reshape(-1)
+        if types.shape[0] != n:
+            raise ValueError(f"atom_types has {types.shape[0]} entries for {n} atoms")
+        types_i32 = self._cached("frames_types", (types_in,), (n,), lambda: types.to(torch.int32).contiguous())
+        ss = self.per_type_energy_scale_shift
+        gscale = ss.scales[types].to(core.acc)
+        pair = None
+        if self.pair_potential is not None:
+            pair = (self.pair_potential, self.edge_norm.rmax_table.to(device=pos.device, dtype=core.acc))
+        Ei, F, X, Ez, virial, Ei_pair = energy_forces(core, self._upstream, csr, pos.detach().contiguous(), types_i32, shift_vec,
+                                                      gscale, bool(stress), pair=pair, frame_ptr=frame_ptr)
+        e_atom = ss(Ei.unsqueeze(-1), types)
+        if Ei_pair is not None:
+            e_atom = e_atom + Ei_pair.unsqueeze(-1).to(e_atom.dtype)
+        out = dict(data)
+        if csr.perm is not None:
+            inv = torch.empty_like(csr.perm)
+            inv[csr.perm] = torch.arange(csr.perm.shape[0], device=csr.perm.device)
+            X, Ez = X[inv], Ez[inv]
+        out[D.EDGE_FEATURES_KEY], out[D.EDGE_ENERGY_KEY] = X, Ez
+        out[D.PER_ATOM_ENERGY_KEY] = e_atom
+        out[D.TOTAL_ENERGY_KEY] = _lib.frame_sum(e_atom.reshape(-1).contiguous(), frame_ptr).unsqueeze(-1)
+        out[D.FORCE_KEY] = F.to(pos.dtype)
+        if stress:
+            sym = 0.5 * (virial + virial.transpose(1, 2))
+            out[D.STRESS_KEY] = (sym / volume.to(sym.dtype).view(B, 1, 1)).to(pos.dtype)
+            out[D.VIRIAL_KEY] = (-sym).to(pos.dtype)
         return out
 
     def _csr(self, edge_index: torch.Tensor, n: int):
@@ -317,6 +448,10 @@ class ForceStressOutput(torch.nn.Module):
         out[D.FORCE_KEY] = -g
         out[D.POSITIONS_KEY] = pos.detach()
         return {k: (v.detach() if isinstance(v, torch.Tensor) else v) for k, v in out.items()}
+
+    def energy_and_forces_frames(self, data: D.Type, stress: bool = False) -> D.Type:
+        """A batch of frames in one call: ``FusedAllegroEnergy.energy_and_forces_frames``."""
+        return self.model.energy_and_forces_frames(data, stress)
 
 
 def _builder_common(kwargs: Dict):

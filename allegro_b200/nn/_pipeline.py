@@ -455,14 +455,17 @@ class UpstreamPack:
 
 
 def energy_forces(core: "AllegroCore", up: UpstreamPack, csr: EdgeCSR, pos: torch.Tensor, types_i32: torch.Tensor,
-                  shift_vec: Optional[torch.Tensor], gEi_scale: Optional[torch.Tensor], want_virial: bool = False, pair=None):
+                  shift_vec: Optional[torch.Tensor], gEi_scale: Optional[torch.Tensor], want_virial: bool = False, pair=None,
+                  frame_ptr: Optional[torch.Tensor] = None):
     """Whole path with no torch autograd: positions -> (Ei [N], forces [n_atoms,3], X, Ez, virial).
     ``gEi_scale`` = d E_total / d Ei (per-type scales), None = ones.  ``virial`` (only if asked for) is
     sum_z r_z (x) dE/dr_z [3,3] = dE/d(strain) before symmetrisation, from the per-edge gradients the
     force scatter consumes anyway.  ``pair`` = (ZBL module, r_max table) adds the pair potential's gradient to the
     per-edge gradients and returns its per-atom energies as a sixth value (added AFTER the per-type scale/shift,
-    allegro_models.py:270-288)."""
+    allegro_models.py:270-288).  ``frame_ptr`` [B+1] int32 (a batch of frames concatenated into one graph): the virial is
+    then per frame, [B,3,3] (ab2_frame_virial)."""
     dt, acc = core.dtype, core.acc
+    vshape = (3, 3) if frame_ptr is None else (frame_ptr.shape[0] - 1, 3, 3)
     E = csr.num_edges
     if E == 0:
         # a frame without a single edge (every atom isolated): zero energies before scale/shift, zero forces, empty
@@ -470,7 +473,7 @@ def energy_forces(core: "AllegroCore", up: UpstreamPack, csr: EdgeCSR, pos: torc
         dev = pos.device
         return (torch.zeros(csr.num_atoms, dtype=acc, device=dev), torch.zeros(pos.shape[0], 3, dtype=acc, device=dev),
                 torch.empty(0, core.S * (core.L + 1), dtype=dt, device=dev), torch.empty(0, 1, dtype=dt, device=dev),
-                torch.zeros(3, 3, dtype=acc, device=dev) if want_virial else None,
+                torch.zeros(vshape, dtype=acc, device=dev) if want_virial else None,
                 torch.zeros(csr.num_atoms, dtype=acc, device=dev) if pair is not None else None)
     _lib.set_tag("fwd.radial")
     vec = _lib.edge_vec(pos, csr.ctr, csr.nbr, shift_vec, acc)
@@ -490,7 +493,9 @@ def energy_forces(core: "AllegroCore", up: UpstreamPack, csr: EdgeCSR, pos: torc
     if pair is not None:
         Ez_pair = pair[0].edge_energy_and_grad(vec, csr, types_i32, pair[1], gvec)
         Ei_pair = _lib.edge_sum(Ez_pair, csr.row_ptr, 1.0)
-    virial = (vec.T @ gvec.to(vec.dtype)) if want_virial else None
+    virial = None
+    if want_virial:
+        virial = (vec.T @ gvec.to(vec.dtype)) if frame_ptr is None else _lib.frame_virial(vec, gvec.to(vec.dtype), frame_ptr, csr.row_ptr)
     F = _lib.force_scatter(gvec, csr, pos.shape[0])
     return Ei, F, X, Ez, virial, Ei_pair
 

@@ -290,6 +290,42 @@ int ab2_nl_fill(int pos_dtype, int64_t n_centres, const void* pos, const double*
                 const int32_t* cell_start, const int32_t* order, const int32_t* row_ptr, int32_t* nbr,
                 void* shift, void* stream);
 
+/* ---- batches of frames: many small frames concatenated into one graph ------------------------ */
+
+/* All-pairs search for a batch of frames (nequip's batched data: `batch`, `num_atoms`, one cell per frame), for any
+ * cell the all-pairs search of the reference data pipeline accepts: triclinic, narrower than r_max (several images per
+ * axis, n_a = ceil(r_max / h_a) with h_a the cell height along axis a), mixed per-axis periodicity, or no periodic axis
+ * at all (a molecule: no wrap, one image).  Each centre checks every atom of its own frame over the frame's image
+ * range, so the work of frame b is O(N_b^2 * images): meant for small frames (the Python wrapper caps them).
+ * Geometry, all device buffers: frame_ptr[n_frames+1] int32 (atoms of frame b are [frame_ptr[b], frame_ptr[b+1]),
+ * frame_ptr[0] = 0, frame_ptr[n_frames] = n), cell / inv_cell [n_frames][3][3] (rows = lattice vectors; inv_cell its
+ * inverse, any finite values for a frame with no periodic axis), pbc [n_frames][3] int32.  pos: [n][3] fp64 or fp32
+ * raw (unwrapped) coordinates; cell, inv_cell and shift in the same dtype.  Positions are wrapped along the periodic
+ * axes in fractional coordinates (frac = pos @ inv_cell, image = floor(frac)) and the raw images folded back, so
+ *   r = pos[nbr] + shift - pos[centre]  holds for the raw positions; shift = (integer image) @ cell.
+ * Rows are ordered by neighbour index, then by image (x, y, z) lexicographically.  Every atom is a centre.
+ * Call order: ab2_nl_frames_count -> (host: row_ptr = prefix sum of counts) -> ab2_nl_frames_fill. */
+int ab2_nl_frames_count(int pos_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* pos,
+                        const void* cell, const void* inv_cell, const int32_t* pbc, double r_max, int32_t* counts,
+                        void* stream);
+int ab2_nl_frames_fill(int pos_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* pos,
+                       const void* cell, const void* inv_cell, const int32_t* pbc, double r_max, const int32_t* row_ptr,
+                       int32_t* nbr, void* shift, void* stream);
+
+/* Per-frame reductions (nequip's per-graph sums of a batch):
+ *   ab2_frame_sum     out[b] = sum_{a in [frame_ptr[b], frame_ptr[b+1])} x[a]                 x [n], out [n_frames]
+ *   ab2_frame_virial  W[b] = sum_{z in frame b} vec[z] (x) gvec[z]                 vec, gvec [E][3], W [n_frames][3][3]
+ *                     frame b's edges are [row_ptr[frame_ptr[b]], row_ptr[frame_ptr[b+1]])   (centre-sorted CSR)
+ * in the accumulate dtype (acc_dtype fp64 or fp32; summed in fp64 and rounded once).  Every frame is cut into fixed
+ * chunks counted from its own start and the chunk sums are added in chunk order: deterministic, no atomics, independent
+ * of the launch and of the other frames in the batch; an empty frame gives exactly 0.  scratch: fp64 device buffer of
+ * at least ab2_frame_scratch_elems(n or E, n_frames) * width elements (width 1 for the sum, 9 for the virial). */
+int64_t ab2_frame_scratch_elems(int64_t total, int64_t n_frames);
+int ab2_frame_sum(int acc_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* x, double* scratch,
+                  int64_t scratch_elems, void* out, void* stream);
+int ab2_frame_virial(int acc_dtype, int64_t E, int64_t n_frames, const int32_t* frame_ptr, const int32_t* row_ptr,
+                     const void* vec, const void* gvec, double* scratch, int64_t scratch_elems, void* W, void* stream);
+
 /* Radial embedding with per-type-pair matrices: out[z][c] = sum_n B_n(x_z) PQ[t_c * T + t_n][n][c], B_n as above
  * (num_bessels must be 8, S <= 128).  PQ: [T*T][8][S] in the accumulate dtype.  The product embedding above is
  * PQ = typeemb(t_c,t_n)[c] * Wb[n][c]; because everything up to the first nonlinearity is linear
