@@ -506,6 +506,13 @@ class _CoreFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, vec, x_emb, core: AllegroCore, csr: EdgeCSR, stash: Dict):
+        if csr.num_edges == 0:
+            # no edge at all: zero energies and empty per-edge outputs, as energy_forces gives (the kernels take no
+            # empty inputs)
+            ctx.core, ctx.sv, ctx.empty = core, None, (vec.shape, vec.dtype, x_emb.shape, x_emb.dtype, vec.device)
+            stash["edge_features"] = torch.empty(0, core.S * (core.L + 1), dtype=core.dtype, device=vec.device)
+            stash["edge_energy"] = torch.empty(0, 1, dtype=core.dtype, device=vec.device)
+            return torch.zeros(csr.num_atoms, dtype=core.acc, device=vec.device)
         Ei, X, Ez, sv = core.forward(csr, vec.detach(), x_emb.detach())
         ctx.core, ctx.sv = core, sv
         stash["edge_features"], stash["edge_energy"] = X, Ez
@@ -513,6 +520,9 @@ class _CoreFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gEi):
+        if ctx.sv is None:  # no edge: zero gradients of the empty vec and x_emb
+            vs, vd, xs, xd, dev = ctx.empty
+            return torch.zeros(vs, dtype=vd, device=dev), torch.zeros(xs, dtype=xd, device=dev), None, None, None
         gvec, gx = ctx.core.backward(ctx.sv, gEi.to(ctx.core.acc))
         ctx.sv = None
         return gvec, gx, None, None, None

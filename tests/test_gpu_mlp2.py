@@ -18,6 +18,19 @@ C2_SHAPES = [
     ("bwd.L1", True, [64], 64, [128, 32], [True, False]),
     ("bwd.L0", True, [64, 96], 64, [64, 32], [True, True]),
 ]
+# the other shapes fp32 models hand to ab2_mlp2 (tests/test_gpu_fp32_grid.py): every stage of the S = H = 32 model
+# (U = 32, L = 2; the fused readout declines H = 32, so the last latent MLP and the readout run here), and the first
+# inner latent MLP of a U = 64 model (N = 64 + 3 x 64 = 256: four 64-column chunks, the most the kernel holds)
+MODEL_SHAPES = C2_SHAPES + [
+    ("H32.fwd.L0", False, [32, 32], 32, [32, 96], [False, False]),
+    ("H32.fwd.L1", False, [64, 32], 32, [32], [False]),
+    ("H32.fwd.readout", False, [96], 32, [1], [False]),
+    ("H32.bwd.readout", True, [1], 32, [96], [False]),
+    ("H32.bwd.L1", True, [32], 32, [64, 32], [True, False]),
+    ("H32.bwd.L0", True, [32, 96], 32, [32, 32], [True, True]),
+    ("U64.fwd.L0", False, [64, 64], 64, [64, 192], [False, False]),
+    ("U64.bwd.L0", True, [64, 192], 64, [64, 64], [True, True]),
+]
 
 
 def _dsilu(x):
@@ -117,14 +130,16 @@ def _check(M, backward, a_w, H, o_w, accum, seed=0):
         assert torch.equal(pre_f, pre)  # read only
 
 
-@pytest.mark.parametrize("shape", C2_SHAPES, ids=[s[0] for s in C2_SHAPES])
+@pytest.mark.parametrize("shape", MODEL_SHAPES, ids=[s[0] for s in MODEL_SHAPES])
 def test_mlp2_c2_shapes(shape):
     _, backward, a_w, H, o_w, accum = shape
     _check(C2_M, backward, a_w, H, o_w, accum)
 
 
-@pytest.mark.parametrize("M", [77, 129, 40000])
-@pytest.mark.parametrize("shape", C2_SHAPES, ids=[s[0] for s in C2_SHAPES])
+# one row, a partial and an exact 128-row tile, and one tile less / more than the 132 SMs hold (with M = 132 x 128 + 1
+# a persistent CTA runs a second, one-row tile)
+@pytest.mark.parametrize("M", [1, 77, 128, 129, 132 * 128 - 1, 132 * 128 + 1, 40000])
+@pytest.mark.parametrize("shape", MODEL_SHAPES, ids=[s[0] for s in MODEL_SHAPES])
 def test_mlp2_partial_tiles(shape, M):
     _, backward, a_w, H, o_w, accum = shape
     _check(M, backward, a_w, H, o_w, accum, seed=M)

@@ -16,10 +16,16 @@ from test_host_mlp2 import _dsilu, _mlp2_spec, _rel
 MODELS = {r["name"]: r for r in load_models()}
 
 
-def _mlp2_readout_spec(calls, core_of):
+def _mlp2_readout_spec(calls, core_of, decline=(), declined=None):
+    """``decline``: the directions ("fwd", "bwd") in which the stand-in declines as the library does for a plan that
+    does not fit, before writing anything; those calls go to ``declined``, the taken ones to ``calls``."""
+
     def mlp2_readout(backward, x, s, xl, pre_l, pre_r, ez, w2_ro, W_packed, S):
         if x.dtype != torch.float32:
             return False  # the kernel takes fp32 storage only
+        if ("bwd" if backward else "fwd") in decline:
+            declined.append(backward)
+            return False
         calls.append(backward)
         core = core_of()
         lat, ro = core.layers[-1]["mlp"], core.readout
@@ -44,17 +50,22 @@ def _mlp2_readout_spec(calls, core_of):
     return mlp2_readout
 
 
-@pytest.fixture()
-def spec_kernels_fused(monkeypatch):
+def _install_spec(monkeypatch, decline=(), mlp2_declines=False):
+    """The kernels replaced by their restatements on the CPU -> (taken mlp2_readout calls, declined mlp2_readout calls,
+    mlp2 calls).  ``mlp2_declines``: ab2_mlp2 declines every call (the callers then run two linear layers)."""
     from allegro_b200 import _lib
     from allegro_b200.model.allegro_models import FusedAllegroEnergy
 
     for name in kernel_spec.ALL:
         monkeypatch.setattr(_lib, name, getattr(kernel_spec, name))
-    monkeypatch.setattr(_lib, "mlp2", _mlp2_spec([]))
+    mlp2_calls = []
+    if mlp2_declines:
+        monkeypatch.setattr(_lib, "mlp2", lambda *a, **k: mlp2_calls.append(k.get("backward", False)) and False)
+    else:
+        monkeypatch.setattr(_lib, "mlp2", _mlp2_spec(mlp2_calls))
     cores = []
-    calls = []
-    monkeypatch.setattr(_lib, "mlp2_readout", _mlp2_readout_spec(calls, lambda: cores[-1]))
+    calls, declined = [], []
+    monkeypatch.setattr(_lib, "mlp2_readout", _mlp2_readout_spec(calls, lambda: cores[-1], decline, declined))
 
     def core(self):
         c = self._core_for(torch.device("cpu"))
@@ -62,7 +73,12 @@ def spec_kernels_fused(monkeypatch):
         return c
 
     monkeypatch.setattr(FusedAllegroEnergy, "core", core)
-    return calls
+    return calls, declined, mlp2_calls
+
+
+@pytest.fixture()
+def spec_kernels_fused(monkeypatch):
+    return _install_spec(monkeypatch)[0]
 
 
 @pytest.mark.parametrize("name", model_case_ids())
@@ -85,6 +101,54 @@ def test_host_pipeline_with_fused_readout(name, spec_kernels_fused):
         assert False in spec_kernels_fused and True in spec_kernels_fused, spec_kernels_fused
     else:
         assert not spec_kernels_fused
+
+
+def _fused_offered(rec):
+    kw = rec["kwargs"]
+    two_layer = kw.get("allegro_mlp_hidden_layers_depth", 1) == 1 and kw.get("readout_mlp_hidden_layers_depth", 1) == 1
+    same_width = kw["allegro_mlp_hidden_layers_width"] == kw["readout_mlp_hidden_layers_width"]
+    return kw["model_dtype"] == "float32" and two_layer and same_width and rec["data"]["edge_index"].shape[1] > 0
+
+
+@pytest.mark.parametrize("mlp2", ["mlp2_takes", "mlp2_declines"])
+@pytest.mark.parametrize("decline", ["fwd", "bwd", "both"])
+@pytest.mark.parametrize("name", model_case_ids())
+def test_host_pipeline_readout_declines(name, decline, mlp2, monkeypatch):
+    """ab2_mlp2_readout declining the forward only, the backward only, or both (as for a plan that does not fit the
+    shared memory), with ab2_mlp2 taking or declining the separate MLPs.  The reference cases as they are must give the
+    reference's results.  None of them is an fp32 model with equal latent and readout hidden widths, so each also runs
+    as one (its other settings kept, new weights): AllegroCore's mixed paths -- the backward of a fused forward through
+    the two separate MLPs, the fused backward of a forward that ran them separately -- must give what the fully fused
+    path gives, at the bar of the fused-against-separate comparison below."""
+    from allegro_b200.model import AllegroModel
+
+    rec = MODELS[name]
+    dirs = ("fwd", "bwd") if decline == "both" else (decline,)
+    calls, declined, _ = _install_spec(monkeypatch, dirs, mlp2 == "mlp2_declines")
+    model = AllegroModel(**rec["kwargs"])
+    model.load_state_dict(unpack_state_dict(rec["state_dict"]), strict=True)
+    out = model.model._energy_and_forces(dict(rec["data"]), True)
+    tol = 5e-5 if rec["kwargs"]["model_dtype"] == "float32" else 1e-10
+    for key in ("atomic_energy", "forces", "edge_energy", "edge_features", "total_energy"):
+        if key in rec:
+            assert _rel(out[key], rec[key]) < tol, (key, _rel(out[key], rec[key]))
+    assert _fused_offered(rec) or not (calls or declined)
+
+    kw = dict(rec["kwargs"], model_dtype="float32", readout_mlp_hidden_layers_width=rec["kwargs"]["allegro_mlp_hidden_layers_width"])
+    if not _fused_offered({"kwargs": kw, "data": rec["data"]}):
+        return  # MLP depths the fused kernels are not built for, or no atoms
+    torch.manual_seed(0)
+    model = AllegroModel(**kw)
+    _install_spec(monkeypatch)
+    fused = model.model._energy_and_forces(dict(rec["data"]), True)
+    calls, declined, mlp2_calls = _install_spec(monkeypatch, dirs, mlp2 == "mlp2_declines")
+    mixed = model.model._energy_and_forces(dict(rec["data"]), True)
+    # each direction asked once: the declined ones declined, the others taken; the separate MLPs then asked ab2_mlp2
+    assert sorted(declined) == sorted(d == "bwd" for d in dirs), declined
+    assert sorted(calls) == sorted(d == "bwd" for d in ("fwd", "bwd") if d not in dirs), calls
+    assert mlp2_calls
+    for key in ("atomic_energy", "forces", "edge_energy", "edge_features", "total_energy"):
+        assert _rel(mixed[key], fused[key]) < 5e-5, (key, _rel(mixed[key], fused[key]))
 
 
 def test_host_pipeline_unequal_hidden_widths(spec_kernels_fused):
