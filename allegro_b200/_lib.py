@@ -16,6 +16,8 @@ from . import build as _build
 AB2_F64, AB2_F32, AB2_BF16 = 0, 1, 2
 ACT_NONE, ACT_SILU, ACT_MUL_DSILU = 0, 1, 2
 EPI_NONE, EPI_MUL_DSILU = 0, 1
+# MLP nonlinearity of the *_nl entries; ACT_SILU / ACT_MUL_DSILU / EPI_MUL_DSILU then mean phi / phi' of that nonlinearity
+NL_SILU, NL_MISH, NL_GELU = 1, 2, 3
 NOT_ELIGIBLE = -1
 MAX_SEG = 4
 
@@ -38,10 +40,14 @@ _SIGNATURES = {
     "ab2_sh_fwd": ([_i32, _i32, _i64, _vp, _vp, _vp], C.c_int),
     "ab2_sh_bwd": ([_i32, _i32, _i64, _vp, _vp, _vp, _i32, _vp], C.c_int),
     "ab2_linear": ([_i32, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _i64, _vp], C.c_int),
+    "ab2_linear_nl": ([_i32, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _i64, _vp, _i32], C.c_int),
     "ab2_linear_packed_bytes": ([_i32, _i32, _i32], C.c_int64),
     "ab2_linear_pack": ([_i32, _i32, _i32, _vp, _vp, _vp], C.c_int),
     "ab2_mlp2_readout": ([_i32, _i32, _i64, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _vp], C.c_int),
     "ab2_mlp2": ([_i32, _i32, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_mlp2_nl": ([_i32, _i32, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _i32], C.c_int),
+    "ab2_mlp2_readout_nl": ([_i32, _i32, _i64, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _i32],
+                            C.c_int),
     "ab2_env_sum": ([_i32, _i32, _i64, _i32, _vp, _vp, _vp, _i64, _dbl, _vp, _vp], C.c_int),
     "ab2_env_bwd": ([_i32, _i32, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _i64, _vp, _dbl, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_tp_fwd": ([_i32, _i32, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp], C.c_int),
@@ -56,6 +62,7 @@ _SIGNATURES = {
     "ab2_radial_fwd": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_radial_pq_fwd": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_radial_pq_bwd": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_radial_pq_bwd_nl": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32], C.c_int),
     "ab2_zbl": ([_i32, _i64, _i32, _dbl, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_p2p_mailbox_bytes": ([_i32, _i32], C.c_int64),
     "ab2_p2p_alloc": ([_i64, C.POINTER(C.c_void_p)], C.c_int),
@@ -239,9 +246,11 @@ def linear(
     aux: Optional[torch.Tensor] = None,
     W_packed: Optional[torch.Tensor] = None,
     a_aux: Optional[Sequence[Optional[torch.Tensor]]] = None,
+    nonlin: int = NL_SILU,
 ):
     """Out (+)= epi(act(cat(a_segs, -1)) @ W); a_segs / o_segs are 2-D row-strided views.
-    ``W_packed`` (from ``linear_pack``) enables the wgmma tensor-core path."""
+    ``W_packed`` (from ``linear_pack``) enables the wgmma tensor-core path.  ``nonlin`` (NL_*): the nonlinearity that
+    ``act`` / ``epi`` apply (ab2_linear_nl); SiLU calls ab2_linear."""
     M = a_segs[0].shape[0]
     K, N = W.shape
     dt = W.dtype
@@ -281,13 +290,10 @@ def linear(
     if aux is not None:
         aux, aux_ld = _row_strided(aux, "aux")
         assert aux.dtype == dt
+    args = (DTYPE_ENUM[dt], M, K, N, na, a_ptr, a_ld, a_w, x_ptr, x_ld, act, _ptr(_contig(W, "W")), _ptr(W_packed), no, o_ptr, o_ld, o_w, o_acc,
+            epi, _ptr(aux), aux_ld, _stream())
     with _timed("linear", 1):
-        _check(
-            load().ab2_linear(
-                DTYPE_ENUM[dt], M, K, N, na, a_ptr, a_ld, a_w, x_ptr, x_ld, act, _ptr(_contig(W, "W")), _ptr(W_packed), no, o_ptr, o_ld, o_w, o_acc, epi,
-                _ptr(aux), aux_ld, _stream(),
-            )
-        )
+        _check(load().ab2_linear(*args) if nonlin == NL_SILU else load().ab2_linear_nl(*args, nonlin))
 
 
 def mlp2(
@@ -300,10 +306,11 @@ def mlp2(
     backward: bool = False,
     W1_packed: Optional[torch.Tensor] = None,
     W2_packed: Optional[torch.Tensor] = None,
+    nonlin: int = NL_SILU,
 ) -> bool:
-    """Two-layer SiLU MLP in one kernel (ab2_mlp2), A = cat(a_segs, -1):
-    forward   pre = A @ W1 (written),  Out (+)= silu(pre) @ W2;
-    backward  Out (+)= ((A @ W1) * silu'(pre)) @ W2   (A = Gout, W1 = W2_fwd^T, W2 = W1_fwd^T).
+    """Two-layer MLP with nonlinearity phi (``nonlin``, NL_*) in one kernel (ab2_mlp2 / ab2_mlp2_nl), A = cat(a_segs, -1):
+    forward   pre = A @ W1 (written),  Out (+)= phi(pre) @ W2;
+    backward  Out (+)= ((A @ W1) * phi'(pre)) @ W2   (A = Gout, W1 = W2_fwd^T, W2 = W1_fwd^T).
     A one-column backward (K = 1) takes W1 as it is (rank-1 first stage, no packed image).
     Returns False, with nothing computed, when the kernel does not take this case: the caller then runs two ``linear``
     calls."""
@@ -336,11 +343,10 @@ def mlp2(
     pre, pre_ld = _row_strided(pre, "pre")
     assert pre.dtype == dt and tuple(pre.shape) == (M, H)
     timer = _timed("mlp2", 1)
+    args = (DTYPE_ENUM[dt], int(backward), M, K, H, N, na, a_ptr, a_ld, a_w, _ptr(W1_packed), _ptr(W2_packed),
+            _ptr(_contig(W1, "W1")) if rank1 else None, _ptr(pre), pre_ld, no, o_ptr, o_ld, o_w, o_acc, _stream())
     with timer:
-        rc = load().ab2_mlp2(
-            DTYPE_ENUM[dt], int(backward), M, K, H, N, na, a_ptr, a_ld, a_w, _ptr(W1_packed), _ptr(W2_packed),
-            _ptr(_contig(W1, "W1")) if rank1 else None, _ptr(pre), pre_ld, no, o_ptr, o_ld, o_w, o_acc, _stream(),
-        )
+        rc = load().ab2_mlp2(*args) if nonlin == NL_SILU else load().ab2_mlp2_nl(*args, nonlin)
     if rc == NOT_ELIGIBLE:
         timer.cancel()
         return False
@@ -359,9 +365,10 @@ def mlp2_readout(
     w2_ro: torch.Tensor,
     W_packed: Sequence[Optional[torch.Tensor]],
     S: int,
+    nonlin: int = NL_SILU,
 ) -> bool:
-    """Last latent MLP + readout MLP in one kernel (ab2_mlp2_readout), P = x.shape[1], U = s.shape[1], S the width of
-    x_L, H the hidden width of both MLPs:
+    """Last latent MLP + readout MLP in one kernel (ab2_mlp2_readout / ab2_mlp2_readout_nl with the one nonlinearity
+    ``nonlin`` of both MLPs), P = x.shape[1], U = s.shape[1], S the width of x_L, H the hidden width of both MLPs:
     forward   reads x = X[:, :P] and s; writes pre_l, xl = X[:, P:P+S], pre_r and ez = Ez;
               W_packed = packed (W1_lat [P+U][H], W2_lat [H][S], W1_ro[:P] [P][H], W1_ro[P:] [S][H]);
     backward  reads ez = gEz, pre_l and pre_r; writes x = gX[:, :P] and s = gs (xl is None);
@@ -397,11 +404,10 @@ def mlp2_readout(
     for w in W_packed:
         _ptr(w)
     timer = _timed("mlp2_readout", 1)
+    args = (DTYPE_ENUM[dt], int(backward), M, P, S, U, H, *views["x"], *views["s"], *views["xl"], *views["pre_l"], *views["pre_r"],
+            *views["ez"], wp, _ptr(_contig(w2_ro, "w2_ro")), _stream())
     with timer:
-        rc = load().ab2_mlp2_readout(
-            DTYPE_ENUM[dt], int(backward), M, P, S, U, H, *views["x"], *views["s"], *views["xl"], *views["pre_l"], *views["pre_r"],
-            *views["ez"], wp, _ptr(_contig(w2_ro, "w2_ro")), _stream(),
-        )
+        rc = load().ab2_mlp2_readout(*args) if nonlin == NL_SILU else load().ab2_mlp2_readout_nl(*args, nonlin)
     if rc == NOT_ELIGIBLE:
         timer.cancel()
         return False
@@ -700,12 +706,14 @@ def radial_pq_fwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table,
     return out
 
 
-def radial_pq_bwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table, bessel_w, PQ, g_out, aux, gvec):
+def radial_pq_bwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table, bessel_w, PQ, g_out, aux, gvec, nonlin: int = NL_SILU):
+    """gvec += (d out / d vec)^T (g_out * phi'(aux)) (aux None: plain g_out); phi the nonlinearity ``nonlin`` (NL_*)."""
     E = ctr.shape[0]
+    args = (DTYPE_ENUM[dtype], E, S, bessel_w.numel(), float(p_cut), _ptr(vec), _ptr(ctr), _ptr(nbr), _ptr(types), _ptr(rmax_table),
+            rmax_table.shape[0], _ptr(bessel_w), _ptr(_contig(PQ, "PQ")), _ptr(_contig(g_out, "g_out")),
+            _ptr(_contig(aux, "aux")) if aux is not None else None, _ptr(gvec), _stream())
     with _timed("radial_bwd"):
-        _check(load().ab2_radial_pq_bwd(DTYPE_ENUM[dtype], E, S, bessel_w.numel(), float(p_cut), _ptr(vec), _ptr(ctr), _ptr(nbr), _ptr(types),
-                                        _ptr(rmax_table), rmax_table.shape[0], _ptr(bessel_w), _ptr(_contig(PQ, "PQ")), _ptr(_contig(g_out, "g_out")),
-                                        _ptr(_contig(aux, "aux")) if aux is not None else None, _ptr(gvec), _stream()))
+        _check(load().ab2_radial_pq_bwd(*args) if nonlin == NL_SILU else load().ab2_radial_pq_bwd_nl(*args, nonlin))
 
 
 # --------------------------------------------------------------------------- #

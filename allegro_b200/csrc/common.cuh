@@ -119,6 +119,58 @@ __device__ __forceinline__ T dsilu_f(T x) {
     return s * (T(1) + x * (T(1) - s));
 }
 
+__device__ __forceinline__ float ab2_erfc(float x) { return erfcf(x); }
+__device__ __forceinline__ double ab2_erfc(double x) { return erfc(x); }
+
+// mish(x) = x tanh(softplus(x)).  With n = e^min(x, 20): tanh(softplus(x)) = n (n + 2) / (n (n + 2) + 2), and 1 - tanh =
+// 2 / (n (n + 2) + 2) without cancellation; past x = 20 the clamp changes tanh by less than 1e-17.
+template <typename T>
+__device__ __forceinline__ T mish_f(T x) {
+    const T n = ab2_exp(x < T(20) ? x : T(20)), nn = n * (n + T(2));
+    return x * (nn / (nn + T(2)));
+}
+// mish'(x) = t + x (1 - t^2) sigma(x), t = tanh(softplus(x)), sigma(x) = n / (1 + n).  The second term takes the clamped
+// x as well: past 20 it is below 4e-16 (true and clamped), where the unclamped x times the clamped 1 - t^2 would grow with x.
+template <typename T>
+__device__ __forceinline__ T dmish_f(T x) {
+    const T xc = x < T(20) ? x : T(20);
+    const T n = ab2_exp(xc), nn = n * (n + T(2)), d = nn + T(2);
+    const T t = nn / d, omt = T(2) / d;
+    return t + xc * (omt * (T(1) + t)) * (n / (T(1) + n));
+}
+// gelu(x) = x Phi(x) = x erfc(-x / sqrt2) / 2, the exact (erf) form; erfc instead of 1 + erf, which cancels for x < -3
+template <typename T>
+__device__ __forceinline__ T gelu_f(T x) { return T(0.5) * x * ab2_erfc(-x * T(0.70710678118654752440)); }
+template <typename T>
+__device__ __forceinline__ T dgelu_f(T x) {
+    return T(0.5) * ab2_erfc(-x * T(0.70710678118654752440)) + x * ab2_exp(T(-0.5) * x * x) * T(0.39894228040143267794);
+}
+
+// the MLP nonlinearity NL (AB2_NL_*) and its derivative, in T = float / double
+template <int NL, typename T>
+__device__ __forceinline__ T act_f(T x) {
+    if constexpr (NL == AB2_NL_MISH) return mish_f(x);
+    else if constexpr (NL == AB2_NL_GELU) return gelu_f(x);
+    else return silu_f(x);
+}
+template <int NL, typename T>
+__device__ __forceinline__ T dact_f(T x) {
+    if constexpr (NL == AB2_NL_MISH) return dmish_f(x);
+    else if constexpr (NL == AB2_NL_GELU) return dgelu_f(x);
+    else return dsilu_f(x);
+}
+
+// nonlinearity dispatch: NL = the constexpr AB2_NL_* code
+#define AB2_DISPATCH_NL(nonlin, ...)                                                   \
+    switch (nonlin) {                                                                  \
+        case AB2_NL_SILU: { constexpr int NL = AB2_NL_SILU; __VA_ARGS__; } break;      \
+        case AB2_NL_MISH: { constexpr int NL = AB2_NL_MISH; __VA_ARGS__; } break;      \
+        case AB2_NL_GELU: { constexpr int NL = AB2_NL_GELU; __VA_ARGS__; } break;      \
+        default:                                                                       \
+            ab2_set_error("unknown nonlinearity %d", (int)(nonlin));                   \
+            return 1;                                                                  \
+    }
+
 // irrep (l) of SH component j: floor(sqrt(j)) for j < 25
 __host__ __device__ __forceinline__ int sh_l_of(int j) { return (j >= 16) ? 4 : (j >= 9) ? 3 : (j >= 4) ? 2 : (j >= 1) ? 1 : 0; }
 

@@ -7,8 +7,8 @@
 //   column segments (pointer, leading dimension, width);
 // * the output is split into up to 4 column segments (latent -> [new scalars | env weights],
 //   _allegro.py:284-294), each either stored or accumulated (gradient fan-in);
-// * act = silu on load (second MLP layer reads the stored pre-activation);
-// * epi = multiply by silu'(aux) (MLP backward, appendix B step 6).
+// * act = the MLP nonlinearity phi (NL: silu, mish or gelu) on load (second MLP layer reads the stored pre-activation);
+// * epi = multiply by phi'(aux) (MLP backward, appendix B step 6).
 //
 // This file is the precision-generic CUDA-core path (fp64 / fp32 / bf16-storage with fp32
 // accumulate): 64x64 block tile, 16-deep K slices, 4x4 register micro-tile per thread.
@@ -37,7 +37,7 @@ struct LinParams {
     int64_t aux_ld;
 };
 
-template <typename TAct, typename TAcc>
+template <typename TAct, typename TAcc, int NL>
 __device__ __forceinline__ TAcc lin_load_a(const LinParams& p, int64_t m, int k) {
     // locate the segment holding concat column k
 #pragma unroll
@@ -46,7 +46,7 @@ __device__ __forceinline__ TAcc lin_load_a(const LinParams& p, int64_t m, int k)
             if (k < p.a[s].width) {
                 TAcc v = to_acc<TAcc>(((const TAct*)p.a[s].ptr)[m * p.a[s].ld + k]);
                 if (p.act == AB2_ACT_MUL_DSILU && p.a[s].aux)
-                    v *= dsilu_f(to_acc<TAcc>(((const TAct*)p.a[s].aux)[m * p.a[s].aux_ld + k]));
+                    v *= dact_f<NL>(to_acc<TAcc>(((const TAct*)p.a[s].aux)[m * p.a[s].aux_ld + k]));
                 return v;
             }
             k -= p.a[s].width;
@@ -55,7 +55,7 @@ __device__ __forceinline__ TAcc lin_load_a(const LinParams& p, int64_t m, int k)
     return TAcc(0);
 }
 
-template <typename TAct, typename TAcc>
+template <typename TAct, typename TAcc, int NL>
 __global__ void __launch_bounds__(256) linear_kernel(const LinParams p) {
     constexpr int BM = 64, BN = 64, BK = 16;
     __shared__ TAcc As[BK][BM + 4];
@@ -80,8 +80,8 @@ __global__ void __launch_bounds__(256) linear_kernel(const LinParams p) {
             const int64_t m = m0 + r;
             TAcc v = TAcc(0);
             if (m < p.M && k0 + kk < p.K) {
-                v = lin_load_a<TAct, TAcc>(p, m, k0 + kk);
-                if (p.act == AB2_ACT_SILU) v = silu_f(v);
+                v = lin_load_a<TAct, TAcc, NL>(p, m, k0 + kk);
+                if (p.act == AB2_ACT_SILU) v = act_f<NL>(v);
             }
             As[kk][r] = v;
         }
@@ -119,7 +119,7 @@ __global__ void __launch_bounds__(256) linear_kernel(const LinParams p) {
             int n = n0 + tx * 4 + j;
             if (n >= p.N) continue;
             TAcc v = acc[i][j];
-            if (p.epi == AB2_EPI_MUL_DSILU) v *= dsilu_f(to_acc<TAcc>(((const TAct*)p.aux)[m * p.aux_ld + n]));
+            if (p.epi == AB2_EPI_MUL_DSILU) v *= dact_f<NL>(to_acc<TAcc>(((const TAct*)p.aux)[m * p.aux_ld + n]));
 #pragma unroll
             for (int s = 0; s < AB2_MAX_SEG; ++s) {
                 if (s < p.n_o) {
@@ -138,13 +138,14 @@ __global__ void __launch_bounds__(256) linear_kernel(const LinParams p) {
 
 int ab2_linear_tc_try(int dtype, int64_t M, int K, int N, int n_a, const void* const* a_ptr, const int64_t* a_ld,
                       const int32_t* a_width, const void* const* a_aux, const int64_t* a_aux_ld, int act, const void* Wpacked, int n_o, void* const* o_ptr, const int64_t* o_ld,
-                      const int32_t* o_width, const int32_t* o_accum, int epi, const void* aux, int64_t aux_ld, cudaStream_t st);
+                      const int32_t* o_width, const int32_t* o_accum, int epi, const void* aux, int64_t aux_ld, cudaStream_t st, int nonlin);
 
-extern "C" int ab2_linear(int dtype, int64_t M, int K, int N, int n_a, const void* const* a_ptr, const int64_t* a_ld,
+extern "C" int ab2_linear_nl(int dtype, int64_t M, int K, int N, int n_a, const void* const* a_ptr, const int64_t* a_ld,
                           const int32_t* a_width, const void* const* a_aux, const int64_t* a_aux_ld, int act, const void* W,
                           const void* Wpacked, int n_o, void* const* o_ptr,
                           const int64_t* o_ld, const int32_t* o_width, const int32_t* o_accum, int epi, const void* aux,
-                          int64_t aux_ld, void* stream) {
+                          int64_t aux_ld, void* stream, int nonlin) {
+    AB2_CHECK_ARG(nonlin == AB2_NL_SILU || nonlin == AB2_NL_MISH || nonlin == AB2_NL_GELU, "nonlinearity");
     if (M == 0) return 0;
     AB2_CHECK_ARG(n_a >= 1 && n_a <= AB2_MAX_SEG && n_o >= 1 && n_o <= AB2_MAX_SEG, "segment count");
     AB2_CHECK_ARG(K > 0 && N > 0 && W, "shape");
@@ -168,7 +169,7 @@ extern "C" int ab2_linear(int dtype, int64_t M, int K, int N, int n_a, const voi
     AB2_CHECK_ARG(ns == N, "output segment widths must sum to N");
     cudaStream_t st = (cudaStream_t)stream;
     const int tc = Wpacked ? ab2_linear_tc_try(dtype, M, K, N, n_a, a_ptr, a_ld, a_width, a_aux, a_aux_ld, act, Wpacked, n_o, o_ptr, o_ld, o_width,
-                                               o_accum, epi, aux, aux_ld, st)
+                                               o_accum, epi, aux, aux_ld, st, nonlin)
                            : -1;
     if (tc == 0) {
         AB2_CUDA_LAUNCH_CHECK();
@@ -179,7 +180,16 @@ extern "C" int ab2_linear(int dtype, int64_t M, int K, int N, int n_a, const voi
         return 2;
     }
     dim3 grid(ab2_blocks(M, 64), (unsigned)((N + 63) / 64));
-    AB2_DISPATCH_DTYPE(dtype, linear_kernel<TAct, TAcc><<<grid, 256, 0, st>>>(p));
+    AB2_DISPATCH_NL(nonlin, AB2_DISPATCH_DTYPE(dtype, linear_kernel<TAct, TAcc, NL><<<grid, 256, 0, st>>>(p)));
     AB2_CUDA_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int ab2_linear(int dtype, int64_t M, int K, int N, int n_a, const void* const* a_ptr, const int64_t* a_ld,
+                          const int32_t* a_width, const void* const* a_aux, const int64_t* a_aux_ld, int act, const void* W,
+                          const void* Wpacked, int n_o, void* const* o_ptr,
+                          const int64_t* o_ld, const int32_t* o_width, const int32_t* o_accum, int epi, const void* aux,
+                          int64_t aux_ld, void* stream) {
+    return ab2_linear_nl(dtype, M, K, N, n_a, a_ptr, a_ld, a_width, a_aux, a_aux_ld, act, W, Wpacked, n_o, o_ptr, o_ld, o_width, o_accum, epi, aux,
+                         aux_ld, stream, AB2_NL_SILU);
 }

@@ -24,6 +24,8 @@
 // (ab2_linear_pack) and stays resident in shared memory.
 #include <cuda.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 extern int g_ab2_opt_linear_tc;
@@ -228,6 +230,36 @@ __device__ __forceinline__ float dsilu_fast(float x) {
     const float sg = sigmoid_fast(x);
     return sg * (1.f + x * (1.f - sg));
 }
+// mish and mish' in the same style (the forms of mish_f / dmish_f in common.cuh): n = e^min(x, 20) keeps every
+// denominator below 2^60, far inside the range where __fdividef is exact to ~2 ulp.  Finite for every finite x.
+__device__ __forceinline__ float mish_fast(float x) {
+    const float n = __expf(fminf(x, 20.f)), nn = n * (n + 2.f);
+    return x * __fdividef(nn, nn + 2.f);
+}
+__device__ __forceinline__ float dmish_fast(float x) {
+    const float xc = fminf(x, 20.f), n = __expf(xc), nn = n * (n + 2.f), r = __fdividef(1.f, nn + 2.f);
+    const float t = nn * r;
+    return t + xc * (2.f * r * (1.f + t)) * __fdividef(n, 1.f + n);
+}
+// gelu and gelu' (exact erf form): erfcf(-x / sqrt2) does not cancel for x < -3 as 1 + erff(x / sqrt2) does; the Gaussian
+// factor underflows to 0 (not NaN) for |x| beyond ~13
+__device__ __forceinline__ float gelu_fast(float x) { return 0.5f * x * erfcf(-x * 0.70710678118654752f); }
+__device__ __forceinline__ float dgelu_fast(float x) {
+    return 0.5f * erfcf(-x * 0.70710678118654752f) + x * __expf(-0.5f * x * x) * 0.39894228040143268f;
+}
+// the MLP nonlinearity NL (AB2_NL_*) and its derivative; AB2_NL_SILU is silu_fast / dsilu_fast exactly
+template <int NL>
+__device__ __forceinline__ float act_fast(float x) {
+    if constexpr (NL == AB2_NL_MISH) return mish_fast(x);
+    else if constexpr (NL == AB2_NL_GELU) return gelu_fast(x);
+    else return silu_fast(x);
+}
+template <int NL>
+__device__ __forceinline__ float dact_fast(float x) {
+    if constexpr (NL == AB2_NL_MISH) return dmish_fast(x);
+    else if constexpr (NL == AB2_NL_GELU) return dgelu_fast(x);
+    else return dsilu_fast(x);
+}
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
     __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
@@ -381,9 +413,9 @@ __device__ __forceinline__ void tc_mma_resident(float (&acc)[16 * NCH], uint32_t
 
 // Epilogue of one 64-row half tile from the accumulator registers: this warp's 16 rows, one 32-column chunk at a time,
 // into the output segments of p (chunk table `chunks`, one entry per 32 columns of p).  DSILU = false compiles out the
-// silu' epilogue (p.epi must then be AB2_EPI_NONE).  GENERIC = false compiles out the per-element path: every chunk must
-// then be on the coalesced path (ChunkInfo::ok, checked by the caller's host code).
-template <typename TSrc, int NCH, bool DSILU = true, bool GENERIC = true>
+// phi' epilogue (p.epi must then be AB2_EPI_NONE).  GENERIC = false compiles out the per-element path: every chunk must
+// then be on the coalesced path (ChunkInfo::ok, checked by the caller's host code).  NL: the nonlinearity phi (AB2_NL_*).
+template <typename TSrc, int NCH, bool DSILU = true, bool GENERIC = true, int NL = AB2_NL_SILU>
 __device__ __forceinline__ void tc_epilogue(const TcParams& p, const ChunkInfo* chunks, float* stg, const float (&acc)[16 * NCH], int64_t tile,
                                             int wg, int w4, int lane) {
     {
@@ -405,12 +437,12 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, const ChunkInfo* 
 #pragma unroll
                     for (int t = 0; t < 4; ++t) {
                         const float4 x = __ldg(a4 + t);
-                        v[4 * t] *= dsilu_f(x.x); v[4 * t + 1] *= dsilu_f(x.y); v[4 * t + 2] *= dsilu_f(x.z); v[4 * t + 3] *= dsilu_f(x.w);
+                        v[4 * t] *= dact_f<NL>(x.x); v[4 * t + 1] *= dact_f<NL>(x.y); v[4 * t + 2] *= dact_f<NL>(x.z); v[4 * t + 3] *= dact_f<NL>(x.w);
                     }
                 } else {
 #pragma unroll
                     for (int j = 0; j < 16; ++j)
-                        if (c0 + j < p.N) v[j] *= dsilu_f(to_acc<float>(ax[j]));
+                        if (c0 + j < p.N) v[j] *= dact_f<NL>(to_acc<float>(ax[j]));
                 }
             }
             // scatter the 16 columns into the output segments
@@ -483,8 +515,8 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, const ChunkInfo* 
                     for (int itr = 0; itr < 4; ++itr) ax[itr] = ldg128_nc(ab + (uint32_t)row_of(itr) * al);
 #pragma unroll
                     for (int itr = 0; itr < 4; ++itr) {
-                        x[itr].x *= dsilu_fast(ax[itr].x); x[itr].y *= dsilu_fast(ax[itr].y);
-                        x[itr].z *= dsilu_fast(ax[itr].z); x[itr].w *= dsilu_fast(ax[itr].w);
+                        x[itr].x *= dact_fast<NL>(ax[itr].x); x[itr].y *= dact_fast<NL>(ax[itr].y);
+                        x[itr].z *= dact_fast<NL>(ax[itr].z); x[itr].w *= dact_fast<NL>(ax[itr].w);
                     }
                 }
                 if (ci.accum) {
@@ -517,7 +549,7 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, const ChunkInfo* 
     }
 }
 
-template <typename TSrc, bool SPLIT, int NCH>
+template <typename TSrc, bool SPLIT, int NCH, int NL>
 __device__ __forceinline__ void tc_consumer_role(const TcParams& p, const TcCtx& c, int cw, int lane) {
     const int wg = cw >> 2, w4 = cw & 3;
     float* stg = c.sEpi + cw * 16 * EPI_LD;
@@ -526,11 +558,11 @@ __device__ __forceinline__ void tc_consumer_role(const TcParams& p, const TcCtx&
     float acc[16 * NCH];
     for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         tc_mma_ring<SPLIT, NCH>(acc, p, c, wg, lane, stage, phase);
-        tc_epilogue<TSrc, NCH>(p, c.sChunk, stg, acc, tile, wg, w4, lane);
+        tc_epilogue<TSrc, NCH, true, true, NL>(p, c.sChunk, stg, acc, tile, wg, w4, lane);
     }
 }
 
-template <typename TSrc, bool SPLIT, int NCH>
+template <typename TSrc, bool SPLIT, int NCH, int NL>
 __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const TcParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;  // warp-uniform role index
@@ -687,7 +719,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const TcParams p
                     rd8(4 + i * CH, w);
                     if (has) {
 #pragma unroll
-                        for (int t = 0; t < 8; ++t) v[i][t] *= dsilu_fast(w[t]);
+                        for (int t = 0; t < 8; ++t) v[i][t] *= dact_fast<NL>(w[t]);
                     }
                 }
             }
@@ -701,7 +733,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const TcParams p
             for (int i = 0; i < GPW; ++i) {
                 if (p.act == AB2_ACT_SILU) {
 #pragma unroll
-                    for (int t = 0; t < 8; ++t) v[i][t] = silu_fast(v[i][t]);
+                    for (int t = 0; t < 8; ++t) v[i][t] = act_fast<NL>(v[i][t]);
                 }
                 const int g = warp * GPW + i;
                 const uint32_t off = g * (KC / 8) * 128 + kc * 128 + r8 * 16;
@@ -738,7 +770,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tc_kernel(const TcParams p
         }
         cp_async_wait<0>();
     } else {
-        tc_consumer_role<TSrc, SPLIT, NCH>(p, ctx, warp - NPROD, lane);
+        tc_consumer_role<TSrc, SPLIT, NCH, NL>(p, ctx, warp - NPROD, lane);
     }
 }
 
@@ -822,7 +854,7 @@ __device__ __forceinline__ void stage_w(uint8_t* dst, const void* hi, const void
 // (NR % G == 0 and nstage % G == 0, checked on the host): a group then never waits more than one mbarrier phase ahead
 // of its own slot.  (With slots shared between groups a group's first wait can be for the SECOND fill of a slot whose
 // first fill has not completed yet -- the parity wait returns immediately and the pipeline falls apart.)
-template <int G>
+template <int G, int NL>
 __device__ __forceinline__ void tma_converter_role(const TcParams& p, const TmaMaps& maps, int NR, const TcCtx& ctx, uint8_t* sRaw,
                                                    const int4* sKseg, uint32_t rbar0, int64_t total, int warp, int lane) {
     constexpr int WPG = NPROD / G;      // warps per converter group
@@ -883,8 +915,8 @@ __device__ __forceinline__ void tma_converter_role(const TcParams& p, const TmaM
                     const uint8_t* rp = raw + TMA_BOX_BYTES + row * 128;
                     const float4 x = *reinterpret_cast<const float4*>(rp + (((2 * kc) ^ r8) << 4));
                     const float4 y = *reinterpret_cast<const float4*>(rp + (((2 * kc + 1) ^ r8) << 4));
-                    v[i][0] *= dsilu_fast(x.x); v[i][1] *= dsilu_fast(x.y); v[i][2] *= dsilu_fast(x.z); v[i][3] *= dsilu_fast(x.w);
-                    v[i][4] *= dsilu_fast(y.x); v[i][5] *= dsilu_fast(y.y); v[i][6] *= dsilu_fast(y.z); v[i][7] *= dsilu_fast(y.w);
+                    v[i][0] *= dact_fast<NL>(x.x); v[i][1] *= dact_fast<NL>(x.y); v[i][2] *= dact_fast<NL>(x.z); v[i][3] *= dact_fast<NL>(x.w);
+                    v[i][4] *= dact_fast<NL>(y.x); v[i][5] *= dact_fast<NL>(y.y); v[i][6] *= dact_fast<NL>(y.z); v[i][7] *= dact_fast<NL>(y.w);
                 }
             }
             // raw slot drained by every warp of the group (values are in registers): refill it
@@ -896,7 +928,7 @@ __device__ __forceinline__ void tma_converter_role(const TcParams& p, const TmaM
             for (int i = 0; i < RGW; ++i) {
                 if (p.act == AB2_ACT_SILU) {
 #pragma unroll
-                    for (int t = 0; t < 8; ++t) v[i][t] = silu_fast(v[i][t]);
+                    for (int t = 0; t < 8; ++t) v[i][t] = act_fast<NL>(v[i][t]);
                 }
                 const int g = sub * RGW + i;
                 const uint32_t off = g * (KC / 8) * 128 + kc * 128 + r8 * 16;
@@ -925,7 +957,7 @@ __device__ __forceinline__ void tma_converter_role(const TcParams& p, const TmaM
     }
 }
 
-template <int G, int NCH>
+template <int G, int NCH, int NL>
 __global__ void __launch_bounds__(NTHREADS, 1) linear_tma_kernel(const TcParams p, const __grid_constant__ TmaMaps maps, int NR) {
     constexpr int WPG = NPROD / G;      // warps per converter group
     using TSrc = float;
@@ -966,9 +998,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tma_kernel(const TcParams 
     const int64_t total = my_tiles * nkb;
 
     if (warp >= NPROD) {
-        tc_consumer_role<TSrc, SPLIT, NCH>(p, ctx, warp - NPROD, lane);
+        tc_consumer_role<TSrc, SPLIT, NCH, NL>(p, ctx, warp - NPROD, lane);
     } else {
-        tma_converter_role<G>(p, maps, NR, ctx, sRaw, sKseg, rbar0, total, warp, lane);
+        tma_converter_role<G, NL>(p, maps, NR, ctx, sRaw, sKseg, rbar0, total, warp, lane);
     }
 }
 
@@ -1016,7 +1048,7 @@ __device__ __forceinline__ void mlp2_stage2(const TcParams& p2, const ChunkInfo*
     tc_epilogue<float, NCH, false>(p2, chunks, stg, acc, tile, wg, w4, lane);
 }
 
-template <int NCH1>
+template <int NCH1, int NL>
 __global__ void __launch_bounds__(NTHREADS, 1) mlp2_kernel(const __grid_constant__ Mlp2Params q, const __grid_constant__ TmaMaps maps, int NR) {
     constexpr int G = 2, WPG = NPROD / G;
     constexpr int H = 32 * NCH1;
@@ -1065,7 +1097,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp2_kernel(const __grid_constant
     if (warp < NPROD) {
         if (!rank1) {
             const int64_t my_tiles = (p.num_tiles > blockIdx.x) ? (p.num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-            tma_converter_role<G>(p, maps, NR, ctx, sRaw, sKseg, rbar0, my_tiles * nkb, warp, lane);
+            // stage 1 loads A as it is (p.act == AB2_ACT_NONE): the converters take no nonlinearity
+            tma_converter_role<G, AB2_NL_SILU>(p, maps, NR, ctx, sRaw, sKseg, rbar0, my_tiles * nkb, warp, lane);
         }
         return;
     }
@@ -1122,17 +1155,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp2_kernel(const __grid_constant
             cp_async_wait<0>();  // this thread's own copies: visible to it once complete
             store_hidden([&](int i) {
                 const float w = __ldg(q.w1row + 8 * (i >> 2) + cq + (i & 1));
-                return ((i & 2) ? gb : ga) * w * dsilu_fast(pre_at(i));
+                return ((i & 2) ? gb : ga) * w * dact_fast<NL>(pre_at(i));
             });
         } else {
             float acc[16 * NCH1];
             tc_mma_ring<true, NCH1>(acc, p, ctx, wg, lane, stage, phase);
             if (!q.backward) {
                 tc_epilogue<float, NCH1, false>(p, sChunk, stg, acc, tile, wg, w4, lane);  // pre
-                store_hidden([&](int i) { return silu_fast(acc[i]); });
+                store_hidden([&](int i) { return act_fast<NL>(acc[i]); });
             } else {
                 cp_async_wait<0>();
-                store_hidden([&](int i) { return acc[i] * dsilu_fast(pre_at(i)); });
+                store_hidden([&](int i) { return acc[i] * dact_fast<NL>(pre_at(i)); });
             }
         }
         fence_proxy_async();  // generic-proxy writes, read by wgmma through the async proxy
@@ -1256,6 +1289,7 @@ struct RoFwdPlan {
     }
 };
 
+template <int NL>
 __global__ void __launch_bounds__(NTHREADS, 1) mlp2_readout_fwd_kernel(const __grid_constant__ Mlp2RoParams q, const __grid_constant__ TmaMaps maps,
                                                                         int NR) {
     constexpr int G = 2, WPG = NPROD / G;
@@ -1281,7 +1315,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp2_readout_fwd_kernel(const __g
         __syncthreads();
         if (warp < NPROD) {
             const int64_t my_tiles = (p.num_tiles > blockIdx.x) ? (p.num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-            tma_converter_role<G>(p, maps, NR, sp.ctx(q), sp.raw, sp.kseg, smem_u32(sp.rbars), my_tiles * (p.K / KC), warp, threadIdx.x & 31);
+            // the ring carries A as it is (p.act == AB2_ACT_NONE): the converters take no nonlinearity
+            tma_converter_role<G, AB2_NL_SILU>(p, maps, NR, sp.ctx(q), sp.raw, sp.kseg, smem_u32(sp.rbars), my_tiles * (p.K / KC), warp,
+                                               threadIdx.x & 31);
             return;
         }
     }
@@ -1319,7 +1355,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp2_readout_fwd_kernel(const __g
             }
         });
         tc_epilogue<float, 2, false, false>(p, sp.chunk, stg, acc, tile, wg, w4, lane);  // pre_L
-        ro_store_tile(tl, off_a, off_b, [&](int i) { return silu_fast(acc[i]); });
+        ro_store_tile(tl, off_a, off_b, [&](int i) { return act_fast<NL>(acc[i]); });
         fence_proxy_async();  // generic-proxy writes, read by wgmma through the async proxy
         wg_sync();
         {
@@ -1338,10 +1374,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp2_readout_fwd_kernel(const __g
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const float2 w = *reinterpret_cast<const float2*>(sp.w2ro + 8 * j + cq);
-            ea = fmaf(silu_fast(acc_r[4 * j]), w.x, ea);
-            ea = fmaf(silu_fast(acc_r[4 * j + 1]), w.y, ea);
-            eb = fmaf(silu_fast(acc_r[4 * j + 2]), w.x, eb);
-            eb = fmaf(silu_fast(acc_r[4 * j + 3]), w.y, eb);
+            ea = fmaf(act_fast<NL>(acc_r[4 * j]), w.x, ea);
+            ea = fmaf(act_fast<NL>(acc_r[4 * j + 1]), w.y, ea);
+            eb = fmaf(act_fast<NL>(acc_r[4 * j + 2]), w.x, eb);
+            eb = fmaf(act_fast<NL>(acc_r[4 * j + 3]), w.y, eb);
         }
         ea += __shfl_xor_sync(0xffffffffu, ea, 1);
         eb += __shfl_xor_sync(0xffffffffu, eb, 1);
@@ -1372,6 +1408,7 @@ __device__ __forceinline__ void ro_bwd_chunk(const TcParams& pc, const ChunkInfo
     }
 }
 
+template <int NL>
 __global__ void __launch_bounds__(NTHREADS, 1) mlp2_readout_bwd_kernel(const __grid_constant__ Mlp2RoParams q) {
     const TcParams& p = q.s1;
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -1415,7 +1452,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp2_readout_bwd_kernel(const __g
         cp_async_wait<1>();  // pre_r (this thread's own copies: visible to it once complete)
         ro_store_tile(t_r, off_a, off_b, [&](int i) {
             const float w = __ldg(q.w2ro + 8 * (i >> 2) + cq + (i & 1));
-            return ((i & 2) ? gb : ga) * w * dsilu_fast(ro_pre_at(t_r, off_a, off_b, i));
+            return ((i & 2) ? gb : ga) * w * dact_fast<NL>(ro_pre_at(t_r, off_a, off_b, i));
         });
         fence_proxy_async();
         wg_sync();
@@ -1430,7 +1467,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp2_readout_bwd_kernel(const __g
             float gh[32];  // g_h = (g_x @ W2_lat^T) silu'(pre_L)
             tc_mma_resident<2>(gh, tx_u, RO_TILE, RO_H, smem_u32(sWi[1]), q.w_half[1]);
             cp_async_wait<0>();
-            ro_store_tile(t_h, off_a, off_b, [&](int i) { return gh[i] * dsilu_fast(ro_pre_at(t_h, off_a, off_b, i)); });
+            ro_store_tile(t_h, off_a, off_b, [&](int i) { return gh[i] * dact_fast<NL>(ro_pre_at(t_h, off_a, off_b, i)); });
         }
         fence_proxy_async();
         wg_sync();
@@ -1528,7 +1565,17 @@ static bool tc_make_map(CUtensorMap* map, const void* ptr, int64_t ld, int width
               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-static int tc_launch_tma(TcParams& p, int w_bytes, int stage_bytes, int max_smem, unsigned grid, cudaStream_t st, bool dry) {
+// runs f(std::integral_constant<int, NL>) for the AB2_NL_* code nonlin (validated by the caller)
+template <typename F>
+static int tc_with_nl(int nonlin, F&& f) {
+    switch (nonlin) {
+        case AB2_NL_MISH: return f(std::integral_constant<int, AB2_NL_MISH>{});
+        case AB2_NL_GELU: return f(std::integral_constant<int, AB2_NL_GELU>{});
+        default: return f(std::integral_constant<int, AB2_NL_SILU>{});
+    }
+}
+
+static int tc_launch_tma(TcParams& p, int w_bytes, int stage_bytes, int max_smem, unsigned grid, cudaStream_t st, bool dry, int nonlin) {
     TmaMaps maps;
     memset(&maps, 0, sizeof(maps));
     if (!tc_encode_fn()) return -1;
@@ -1558,17 +1605,20 @@ static int tc_launch_tma(TcParams& p, int w_bytes, int stage_bytes, int max_smem
         kern<<<grid, NTHREADS, smem, st>>>(p, maps, NR);
         return 0;
     };
-    switch ((G == 4 ? 4 : 0) + p.Npad / 32) {
-        case 1: return go(linear_tma_kernel<2, 1>);
-        case 2: return go(linear_tma_kernel<2, 2>);
-        case 3: return go(linear_tma_kernel<2, 3>);
-        case 4: return go(linear_tma_kernel<2, 4>);
-        case 5: return go(linear_tma_kernel<4, 1>);
-        case 6: return go(linear_tma_kernel<4, 2>);
-        case 7: return go(linear_tma_kernel<4, 3>);
-        case 8: return go(linear_tma_kernel<4, 4>);
-    }
-    return -1;
+    return tc_with_nl(nonlin, [&](auto nl) -> int {
+        constexpr int NL = decltype(nl)::value;
+        switch ((G == 4 ? 4 : 0) + p.Npad / 32) {
+            case 1: return go(linear_tma_kernel<2, 1, NL>);
+            case 2: return go(linear_tma_kernel<2, 2, NL>);
+            case 3: return go(linear_tma_kernel<2, 3, NL>);
+            case 4: return go(linear_tma_kernel<2, 4, NL>);
+            case 5: return go(linear_tma_kernel<4, 1, NL>);
+            case 6: return go(linear_tma_kernel<4, 2, NL>);
+            case 7: return go(linear_tma_kernel<4, 3, NL>);
+            case 8: return go(linear_tma_kernel<4, 4, NL>);
+        }
+        return -1;
+    });
 }
 
 // SM count and opt-in shared memory per block of the current device (queried once)
@@ -1588,7 +1638,7 @@ static void tc_device_limits(int& num_sms, int& max_smem) {
 static int tc_launch_slice(int dtype, int64_t M, int K, int N, int n_a, const void* const* a_ptr, const int64_t* a_ld,
                            const int32_t* a_width, const void* const* a_aux, const int64_t* a_aux_ld, int act, const void* Whi, const void* Wlo,
                            int n_o, void* const* o_ptr, const int64_t* o_ld, const int32_t* o_width, const int32_t* o_accum, int epi,
-                           const void* aux, int64_t aux_ld, cudaStream_t st, bool dry = false) {
+                           const void* aux, int64_t aux_ld, cudaStream_t st, int nonlin, bool dry = false) {
     const int has_aux = (act == AB2_ACT_MUL_DSILU && a_aux) ? 1 : 0;
     if (tc_npad(N) > MAX_N) return -1;
     int num_sms = 0, max_smem = 0;
@@ -1626,7 +1676,7 @@ static int tc_launch_slice(int dtype, int64_t M, int K, int N, int n_a, const vo
     bool tma_ok = g_ab2_opt_linear_tma && split && K % KC == 0 && M < ((int64_t)1 << 31);
     for (int s = 0; s < n_a && tma_ok; ++s) tma_ok = a_width[s] % KC == 0;
     if (tma_ok) {
-        const int rc = tc_launch_tma(p, w_bytes, stage_bytes, max_smem, grid, st, dry);
+        const int rc = tc_launch_tma(p, w_bytes, stage_bytes, max_smem, grid, st, dry, nonlin);
         if (rc == 0) return 0;
     }
     auto go = [&](auto kern) -> int {
@@ -1637,17 +1687,20 @@ static int tc_launch_slice(int dtype, int64_t M, int K, int N, int n_a, const vo
         kern<<<grid, NTHREADS, smem, st>>>(p);
         return 0;
     };
-    switch ((split ? 4 : 0) + p.Npad / 32) {
-        case 1: return go(linear_tc_kernel<bf16, false, 1>);
-        case 2: return go(linear_tc_kernel<bf16, false, 2>);
-        case 3: return go(linear_tc_kernel<bf16, false, 3>);
-        case 4: return go(linear_tc_kernel<bf16, false, 4>);
-        case 5: return go(linear_tc_kernel<float, true, 1>);
-        case 6: return go(linear_tc_kernel<float, true, 2>);
-        case 7: return go(linear_tc_kernel<float, true, 3>);
-        case 8: return go(linear_tc_kernel<float, true, 4>);
-    }
-    return -1;
+    return tc_with_nl(nonlin, [&](auto nl) -> int {
+        constexpr int NL = decltype(nl)::value;
+        switch ((split ? 4 : 0) + p.Npad / 32) {
+            case 1: return go(linear_tc_kernel<bf16, false, 1, NL>);
+            case 2: return go(linear_tc_kernel<bf16, false, 2, NL>);
+            case 3: return go(linear_tc_kernel<bf16, false, 3, NL>);
+            case 4: return go(linear_tc_kernel<bf16, false, 4, NL>);
+            case 5: return go(linear_tc_kernel<float, true, 1, NL>);
+            case 6: return go(linear_tc_kernel<float, true, 2, NL>);
+            case 7: return go(linear_tc_kernel<float, true, 3, NL>);
+            case 8: return go(linear_tc_kernel<float, true, 4, NL>);
+        }
+        return -1;
+    });
 }
 
 // returns 0 if launched, -1 if this call is not eligible (caller falls back to linear.cu).
@@ -1655,7 +1708,7 @@ static int tc_launch_slice(int dtype, int64_t M, int K, int N, int n_a, const vo
 // per slice, each with its W slice resident; the A rows are re-read per slice).
 int ab2_linear_tc_try(int dtype, int64_t M, int K, int N, int n_a, const void* const* a_ptr, const int64_t* a_ld,
                       const int32_t* a_width, const void* const* a_aux, const int64_t* a_aux_ld, int act, const void* Wpacked, int n_o, void* const* o_ptr, const int64_t* o_ld,
-                      const int32_t* o_width, const int32_t* o_accum, int epi, const void* aux, int64_t aux_ld, cudaStream_t st) {
+                      const int32_t* o_width, const int32_t* o_accum, int epi, const void* aux, int64_t aux_ld, cudaStream_t st, int nonlin) {
     if (!g_ab2_opt_linear_tc || !Wpacked || dtype == AB2_F64) return -1;
     if (ab2_linear_packed_bytes(dtype, K, N) == 0) return -1;
     const int esz = (dtype == AB2_F32) ? 4 : 2;
@@ -1677,7 +1730,7 @@ int ab2_linear_tc_try(int dtype, int64_t M, int K, int N, int n_a, const void* c
     while (true) {
         const int probe = width < N ? width : N;
         if (tc_launch_slice(dtype, M, K, probe, n_a, a_ptr, a_ld, a_width, a_aux, a_aux_ld, act, Wpacked, Wpacked, 1, o_ptr, o_ld, &probe, &any_accum, epi,
-                            aux, aux_ld, st, /*dry=*/true) == 0)
+                            aux, aux_ld, st, nonlin, /*dry=*/true) == 0)
             break;
         if (width <= 32) return -1;
         width = (width / 2 + 31) / 32 * 32;
@@ -1705,17 +1758,19 @@ int ab2_linear_tc_try(int dtype, int64_t M, int K, int N, int n_a, const void* c
         }
         const void* aux_s = aux ? reinterpret_cast<const uint8_t*>(aux) + (size_t)n0 * esz : nullptr;
         const int rc = tc_launch_slice(dtype, M, K, ns, n_a, a_ptr, a_ld, a_width, a_aux, a_aux_ld, act, hi + (size_t)n0 * K * 2,
-                                       lo + (size_t)n0 * K * 2, cnt, so_ptr, so_ld, so_w, so_acc, epi, aux_s, aux_ld, st);
+                                       lo + (size_t)n0 * K * 2, cnt, so_ptr, so_ld, so_w, so_acc, epi, aux_s, aux_ld, st, nonlin);
         if (rc != 0) return n0 == 0 ? -1 : 1;  // a later slice failing would leave a half-written output: report an error
     }
     return 0;
 }
 
-// Fused two-layer SiLU MLP (mlp2_kernel); contract in include/allegro_b200.h.  Returns AB2_NOT_ELIGIBLE, with nothing
-// enqueued and no error set, for a case the kernel does not take: the caller then runs two ab2_linear launches.
-extern "C" int ab2_mlp2(int dtype, int backward, int64_t M, int K, int H, int N, int n_a, const void* const* a_ptr, const int64_t* a_ld,
-                        const int32_t* a_width, const void* W1_packed, const void* W2_packed, const void* w1_row, void* pre, int64_t pre_ld, int n_o,
-                        void* const* o_ptr, const int64_t* o_ld, const int32_t* o_width, const int32_t* o_accum, void* stream) {
+// Fused two-layer MLP (mlp2_kernel); contract in include/allegro_b200.h.  Returns AB2_NOT_ELIGIBLE, with nothing
+// enqueued and no error set, for a case the kernel does not take: the caller then runs two ab2_linear_nl launches.
+extern "C" int ab2_mlp2_nl(int dtype, int backward, int64_t M, int K, int H, int N, int n_a, const void* const* a_ptr, const int64_t* a_ld,
+                           const int32_t* a_width, const void* W1_packed, const void* W2_packed, const void* w1_row, void* pre, int64_t pre_ld,
+                           int n_o, void* const* o_ptr, const int64_t* o_ld, const int32_t* o_width, const int32_t* o_accum, void* stream,
+                           int nonlin) {
+    AB2_CHECK_ARG(nonlin == AB2_NL_SILU || nonlin == AB2_NL_MISH || nonlin == AB2_NL_GELU, "nonlinearity");
     AB2_CHECK_ARG(n_a >= 1 && n_a <= AB2_MAX_SEG && n_o >= 1 && n_o <= AB2_MAX_SEG, "segment count");
     AB2_CHECK_ARG(K > 0 && H > 0 && N > 0 && pre && pre_ld >= H, "shape");
     int ks = 0, ns = 0;
@@ -1825,19 +1880,30 @@ extern "C" int ab2_mlp2(int dtype, int backward, int64_t M, int K, int H, int N,
         AB2_CUDA_LAUNCH_CHECK();
         return 0;
     };
-    switch (H / 32) {
-        case 1: return go(mlp2_kernel<1>);
-        case 2: return go(mlp2_kernel<2>);
-    }
-    return AB2_NOT_ELIGIBLE;
+    return tc_with_nl(nonlin, [&](auto nl) -> int {
+        constexpr int NL = decltype(nl)::value;
+        switch (H / 32) {
+            case 1: return go(mlp2_kernel<1, NL>);
+            case 2: return go(mlp2_kernel<2, NL>);
+        }
+        return AB2_NOT_ELIGIBLE;
+    });
+}
+
+extern "C" int ab2_mlp2(int dtype, int backward, int64_t M, int K, int H, int N, int n_a, const void* const* a_ptr, const int64_t* a_ld,
+                        const int32_t* a_width, const void* W1_packed, const void* W2_packed, const void* w1_row, void* pre, int64_t pre_ld, int n_o,
+                        void* const* o_ptr, const int64_t* o_ld, const int32_t* o_width, const int32_t* o_accum, void* stream) {
+    return ab2_mlp2_nl(dtype, backward, M, K, H, N, n_a, a_ptr, a_ld, a_width, W1_packed, W2_packed, w1_row, pre, pre_ld, n_o, o_ptr, o_ld, o_width,
+                       o_accum, stream, AB2_NL_SILU);
 }
 
 // Last latent MLP + readout MLP (mlp2_readout_fwd_kernel / mlp2_readout_bwd_kernel); contract in include/allegro_b200.h.
 // Returns AB2_NOT_ELIGIBLE, with nothing enqueued and no error set, for a case the kernels do not take: the caller then
-// runs the two MLPs as two ab2_mlp2 (or ab2_linear) calls.
-extern "C" int ab2_mlp2_readout(int dtype, int backward, int64_t M, int P, int S, int U, int H, void* x, int64_t x_ld, void* s, int64_t s_ld,
-                                void* xl, int64_t xl_ld, void* pre_l, int64_t pre_l_ld, void* pre_r, int64_t pre_r_ld, void* ez, int64_t ez_ld,
-                                const void* const* w_packed, const void* w2_ro, void* stream) {
+// runs the two MLPs as two ab2_mlp2_nl (or ab2_linear_nl) calls.
+extern "C" int ab2_mlp2_readout_nl(int dtype, int backward, int64_t M, int P, int S, int U, int H, void* x, int64_t x_ld, void* s, int64_t s_ld,
+                                   void* xl, int64_t xl_ld, void* pre_l, int64_t pre_l_ld, void* pre_r, int64_t pre_r_ld, void* ez, int64_t ez_ld,
+                                   const void* const* w_packed, const void* w2_ro, void* stream, int nonlin) {
+    AB2_CHECK_ARG(nonlin == AB2_NL_SILU || nonlin == AB2_NL_MISH || nonlin == AB2_NL_GELU, "nonlinearity");
     AB2_CHECK_ARG(P > 0 && S > 0 && U > 0 && H > 0 && M >= 0, "shape");
     AB2_CHECK_ARG(x && s && pre_l && pre_r && ez && w2_ro && w_packed && (backward || xl), "null pointer");
     AB2_CHECK_ARG(x_ld >= P && s_ld >= U && (backward || xl_ld >= S) && pre_l_ld >= H && pre_r_ld >= H && ez_ld >= 1, "leading dimension");
@@ -1900,7 +1966,7 @@ extern "C" int ab2_mlp2_readout(int dtype, int backward, int64_t M, int P, int S
         q.pre_r = reinterpret_cast<const float*>(pre_r); q.pre_r_ld = pre_r_ld;
         const size_t smem = (size_t)2 * (q.w_half[0] + q.w_half[1] + q.w_half[2]) + (size_t)12 * RO_TILE + EPI_BYTES + RO_TAIL;
         if (smem > (size_t)max_smem) return AB2_NOT_ELIGIBLE;
-        return go(mlp2_readout_bwd_kernel, smem);
+        return tc_with_nl(nonlin, [&](auto nl) { return go(mlp2_readout_bwd_kernel<decltype(nl)::value>, smem); });
     }
 
     p.K = P + U; p.N = H; p.Npad = H; p.n_a = 2; p.act = AB2_ACT_NONE; p.epi = AB2_EPI_NONE;
@@ -1928,5 +1994,12 @@ extern "C" int ab2_mlp2_readout(int dtype, int backward, int64_t M, int P, int S
     TmaMaps maps;
     memset(&maps, 0, sizeof(maps));
     if (!tc_make_map(&maps.a[0], x, x_ld, P, M) || !tc_make_map(&maps.a[1], s, s_ld, U, M)) return AB2_NOT_ELIGIBLE;
-    return go(mlp2_readout_fwd_kernel, smem, maps, NR);
+    return tc_with_nl(nonlin, [&](auto nl) { return go(mlp2_readout_fwd_kernel<decltype(nl)::value>, smem, maps, NR); });
+}
+
+extern "C" int ab2_mlp2_readout(int dtype, int backward, int64_t M, int P, int S, int U, int H, void* x, int64_t x_ld, void* s, int64_t s_ld,
+                                void* xl, int64_t xl_ld, void* pre_l, int64_t pre_l_ld, void* pre_r, int64_t pre_r_ld, void* ez, int64_t ez_ld,
+                                const void* const* w_packed, const void* w2_ro, void* stream) {
+    return ab2_mlp2_readout_nl(dtype, backward, M, P, S, U, H, x, x_ld, s, s_ld, xl, xl_ld, pre_l, pre_l_ld, pre_r, pre_r_ld, ez, ez_ld, w_packed, w2_ro,
+                               stream, AB2_NL_SILU);
 }

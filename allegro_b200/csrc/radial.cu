@@ -295,12 +295,12 @@ __global__ void __launch_bounds__(256) radial_pq_fwd_kernel(int64_t E, int S, TA
     }
 }
 
-// adjoint: gvec[z] += d out / d vec ^T (g_out[z] (* silu'(aux[z]) if aux)).
+// adjoint: gvec[z] += d out / d vec ^T (g_out[z] (* phi'(aux[z]) if aux)), phi the nonlinearity NL (AB2_NL_*).
 // ONE THREAD PER EDGE end to end: gx = sum_c g[c] * sum_n dB_n * PQ[pair][n][c] needs no cross-lane reduction when the
 // thread walks its own row (S contiguous values, 16-byte loads, all independent -> deep memory-level parallelism),
 // and the PQ entries are warp-uniform broadcasts (same type pair for most lanes; L1-resident 2-4 KB per pair).
 // The first version (warp per edge, lane = column) serialised 32 edges per warp behind a load -> shuffle-reduce chain.
-template <typename TAct, typename TAcc, int NB, int CPL>
+template <typename TAct, typename TAcc, int NB, int CPL, int NL>
 __global__ void __launch_bounds__(128) radial_pq_bwd_kernel(int64_t E, int S, TAcc p, const TAcc* __restrict__ vec,
                                                             const int32_t* __restrict__ ctr, const int32_t* __restrict__ nbr,
                                                             const int32_t* __restrict__ types, const TAcc* __restrict__ rmax_table,
@@ -328,7 +328,7 @@ __global__ void __launch_bounds__(128) radial_pq_bwd_kernel(int64_t E, int S, TA
 #pragma unroll
             for (int k = 0; k < V; ++k) {
                 TAcc gc = to_acc<TAcc>(gv[k]);
-                if (a) gc *= dsilu_f(to_acc<TAcc>(av[k]));
+                if (a) gc *= dact_f<NL>(to_acc<TAcc>(av[k]));
                 TAcc sN = TAcc(0);
 #pragma unroll
                 for (int n = 0; n < NB; ++n) sN += dB[n] * __ldg(m + n * S + c0 + k);
@@ -338,7 +338,7 @@ __global__ void __launch_bounds__(128) radial_pq_bwd_kernel(int64_t E, int S, TA
     } else {
         for (int c = 0; c < S; ++c) {
             TAcc gc = to_acc<TAcc>(g[c]);
-            if (a) gc *= dsilu_f(to_acc<TAcc>(a[c]));
+            if (a) gc *= dact_f<NL>(to_acc<TAcc>(a[c]));
             TAcc sN = TAcc(0);
 #pragma unroll
             for (int n = 0; n < NB; ++n) sN += dB[n] * __ldg(m + n * S + c);
@@ -376,16 +376,24 @@ extern "C" int ab2_radial_pq_fwd(int dtype, int64_t E, int S, int num_bessels, d
     return 0;
 }
 
-extern "C" int ab2_radial_pq_bwd(int dtype, int64_t E, int S, int num_bessels, double p_cut, const void* vec, const int32_t* ctr,
-                                 const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types, const void* bessel_w,
-                                 const void* PQ, const void* g_out, const void* aux, void* gvec, void* stream) {
+extern "C" int ab2_radial_pq_bwd_nl(int dtype, int64_t E, int S, int num_bessels, double p_cut, const void* vec, const int32_t* ctr,
+                                    const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types, const void* bessel_w,
+                                    const void* PQ, const void* g_out, const void* aux, void* gvec, void* stream, int nonlin) {
+    AB2_CHECK_ARG(nonlin == AB2_NL_SILU || nonlin == AB2_NL_MISH || nonlin == AB2_NL_GELU, "nonlinearity");
     if (E == 0) return 0;
     AB2_CHECK_ARG(vec && ctr && nbr && types && rmax_table && bessel_w && PQ && g_out && gvec, "null pointer");
     AB2_CHECK_ARG(num_bessels == 8 && S > 0 && S <= 128, "radial_pq: 8 Bessel functions, at most 128 output columns");
     cudaStream_t st = (cudaStream_t)stream;
-    AB2_DISPATCH_DTYPE(dtype, radial_pq_bwd_kernel<TAct, TAcc, 8, 1><<<ab2_blocks(E, 128), 128, 0, st>>>(
+    AB2_DISPATCH_NL(nonlin, AB2_DISPATCH_DTYPE(dtype, radial_pq_bwd_kernel<TAct, TAcc, 8, 1, NL><<<ab2_blocks(E, 128), 128, 0, st>>>(
                                   E, S, (TAcc)p_cut, (const TAcc*)vec, ctr, nbr, types, (const TAcc*)rmax_table, num_types, (const TAcc*)bessel_w,
-                                  (const TAcc*)PQ, (const TAct*)g_out, (const TAct*)aux, (TAcc*)gvec));
+                                  (const TAcc*)PQ, (const TAct*)g_out, (const TAct*)aux, (TAcc*)gvec)));
     AB2_CUDA_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int ab2_radial_pq_bwd(int dtype, int64_t E, int S, int num_bessels, double p_cut, const void* vec, const int32_t* ctr,
+                                 const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types, const void* bessel_w,
+                                 const void* PQ, const void* g_out, const void* aux, void* gvec, void* stream) {
+    return ab2_radial_pq_bwd_nl(dtype, E, S, num_bessels, p_cut, vec, ctr, nbr, types, rmax_table, num_types, bessel_w, PQ, g_out, aux, gvec, stream,
+                                AB2_NL_SILU);
 }

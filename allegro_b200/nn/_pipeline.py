@@ -109,21 +109,26 @@ class AllegroCore:
         # the last latent MLP and the readout in one kernel per direction (ab2_mlp2_readout); the readout's first layer
         # is packed once more split by rows into the x_0..x_{L-1} block and the x_L block
         last = self.layers[-1]["mlp"]
-        self.ro_fused = last.is_two_layer_silu and self.readout.is_two_layer_silu and last.dims[1] == self.readout.dims[1]
+        # (the kernel applies one nonlinearity to both MLPs, whose kwargs are independent in the reference: on a mismatch the
+        # two MLPs run as two mlp2 calls)
+        self.ro_fused = (last.is_two_layer_nonlinear and self.readout.is_two_layer_nonlinear and last.dims[1] == self.readout.dims[1]
+                         and last.nonlinearity == self.readout.nonlinearity)
         if self.ro_fused:
             P = S * self.L
             W1r = self.readout.W[0]
             self.ro_fwd_p = [last.Wp[0], last.Wp[1], _lib.linear_pack(W1r[:P].contiguous()), _lib.linear_pack(W1r[P:].contiguous())]
             self.ro_bwd_p = [self.readout.WTp[0], last.WTp[1], last.WTp[0]]
-        # "plain GEMM" backward plan (all latent/readout MLPs are 2-layer SiLU): the gradient of the
+        # "plain GEMM" backward plan (all latent/readout MLPs are 2-layer with one nonlinearity): the gradient of the
         # densenet block x_b is ONE GEMM over all its consumers (readout, latents m >= b), concatenated
-        # along K, each consumer's g_h scaled by silu'(pre) in the GEMM prologue -- no accumulation.
+        # along K, each consumer's g_h scaled by phi'(pre) in the GEMM prologue -- no accumulation.  That GEMM applies one
+        # phi' to all its segments, so every latent MLP must share the readout's nonlinearity.
         import os as _os
 
         # the epilogue/accumulate plan is the default, this one is opt-in (ALLEGRO_B200_PLAIN_BWD=1); both are covered
         # by the GPU tests.
-        self.plain_ok = (_os.environ.get("ALLEGRO_B200_PLAIN_BWD", "0") == "1" and self.readout.is_two_layer_silu
-                         and all(ly["mlp"].is_two_layer_silu for ly in self.layers))
+        self.plain_ok = (_os.environ.get("ALLEGRO_B200_PLAIN_BWD", "0") == "1" and self.readout.is_two_layer_nonlinear
+                         and all(ly["mlp"].is_two_layer_nonlinear and ly["mlp"].nonlinearity == self.readout.nonlinearity
+                                 for ly in self.layers))
         if self.plain_ok:
             L = self.L
             self.gxW, self.gxWp, self.gsW, self.gsWp = [], [], [], []
@@ -198,7 +203,7 @@ class AllegroCore:
                 P = S * L
                 pre_l = torch.empty(E, ly["mlp"].dims[1], dtype=dt, device=dev)
                 pre_r = torch.empty(E, self.readout.dims[1], dtype=dt, device=dev)
-                if _lib.mlp2_readout(False, X[:, :P], s, X[:, P:], pre_l, pre_r, Ez, self.readout.W[1], self.ro_fwd_p, S):
+                if _lib.mlp2_readout(False, X[:, :P], s, X[:, P:], pre_l, pre_r, Ez, self.readout.W[1], self.ro_fwd_p, S, **self.readout.nl_kw):
                     pre_lat.append([pre_l])
                     pre_read = [pre_r]
             if pre_read is None:
@@ -239,7 +244,7 @@ class AllegroCore:
             cons = ["r"] + [mm for mm in range(L - 1, b - 1, -1) if mm >= b]
             out = torch.empty(E, S, dtype=dt, device=dev)
             _lib.linear([g_h[c] for c in cons], self.gxW[b], [out], act=_lib.ACT_MUL_DSILU, a_aux=[pre[c] for c in cons],
-                        W_packed=self.gxWp[b])
+                        W_packed=self.gxWp[b], **self.readout.nl_kw)
             return out
 
         for l in range(L - 1, -1, -1):
@@ -257,7 +262,8 @@ class AllegroCore:
             else:
                 gs_acc = True
             gs = gV_next.view(E, ly["d_out"] * U)[:, :U]
-            _lib.linear([g_h[l]], self.gsW[l], [gs], o_accum=[gs_acc], act=_lib.ACT_MUL_DSILU, a_aux=[pre[l]], W_packed=self.gsWp[l])
+            _lib.linear([g_h[l]], self.gsW[l], [gs], o_accum=[gs_acc], act=_lib.ACT_MUL_DSILU, a_aux=[pre[l]], W_packed=self.gsWp[l],
+                        **self.readout.nl_kw)
             ggamma = torch.empty(N, D, U, dtype=self.acc, device=dev)
             if l == 0:
                 gw0 = torch.empty(E, self.nw, dtype=dt, device=dev)
@@ -281,7 +287,7 @@ class AllegroCore:
         return gvec, gx_emb
 
     def _backward_legacy(self, sv: _Saved, gEi: torch.Tensor):
-        """General MLP depth / nonlinearity: SiLU' in the GEMM epilogue, gradient accumulation."""
+        """General MLP depth / nonlinearity: phi' in the GEMM epilogue, gradient accumulation."""
         csr = sv.csr
         E, N, U, S, L, D = csr.num_edges, csr.num_atoms, self.U, self.S, self.L, self.D
         dt, dev = self.dtype, self.device
@@ -294,7 +300,7 @@ class AllegroCore:
             gV_last.zero_()
         # readout and last latent MLP in one kernel: gX[:, :S L] and gs of the last layer (gX[:, S L:] is not formed)
         fused = self.ro_fused and _lib.mlp2_readout(True, gX[:, : S * L], gV_last.view(E, -1)[:, :U], None, sv.pre_lat[-1][0],
-                                                     sv.pre_read[0], gEz, self.readout.W[1], self.ro_bwd_p, S)
+                                                     sv.pre_read[0], gEz, self.readout.W[1], self.ro_bwd_p, S, **self.readout.nl_kw)
         if not fused:
             self.readout.backward([gEz], sv.pre_read, [gX], [False])
         gY = torch.zeros(E, D, dtype=self.acc, device=dev)
@@ -399,7 +405,7 @@ class UpstreamPack:
             T = ce.shape[0]
             temb = torch.cat([ce.unsqueeze(1).expand(T, T, -1), ne.unsqueeze(0).expand(T, T, -1)], dim=-1)  # [tc, tn, S_rc]
             PQ0 = temb.reshape(T * T, 1, -1) * Wb64.unsqueeze(0)                          # [T*T, nb, S_rc]
-            if self.mlp.is_two_layer_silu and self.mlp.dims[1] <= 128 and _os.environ.get("ALLEGRO_B200_FOLD_RADIAL", "1") == "1":
+            if self.mlp.is_two_layer_nonlinear and self.mlp.dims[1] <= 128 and _os.environ.get("ALLEGRO_B200_FOLD_RADIAL", "1") == "1":
                 self.fold_radial = True
                 PQ0 = PQ0 @ self.mlp.W64[0]                                                # [T*T, nb, width]
             if PQ0.shape[-1] <= 128:
@@ -422,7 +428,7 @@ class UpstreamPack:
             return ("spline", sp_saved, self.mlp.forward([e0], outs))
         if self.fold_radial:
             h = _lib.radial_pq_fwd(dt, self.S_pq, self.p, vec, csr.ctr, csr.nbr, types_i32, self.rmax_table, self.bessel_w, self.PQ)
-            _lib.linear([h], self.mlp.W[1], outs, act=_lib.ACT_SILU, W_packed=self.mlp.Wp[1])
+            _lib.linear([h], self.mlp.W[1], outs, act=_lib.ACT_SILU, W_packed=self.mlp.Wp[1], **self.mlp.nl_kw)
             return ("pq_fold", None, [h])
         if self.PQ is not None:
             e0 = _lib.radial_pq_fwd(dt, self.S_pq, self.p, vec, csr.ctr, csr.nbr, types_i32, self.rmax_table, self.bessel_w, self.PQ)
@@ -436,11 +442,12 @@ class UpstreamPack:
         dt = self.dtype
         E = vec.shape[0]
         if kind == "pq_fold":
-            g_h = self.mlp.hidden_grad(gouts)  # gradient w.r.t. silu(h); silu'(h) is applied by the radial adjoint (aux = h)
-            _lib.radial_pq_bwd(dt, self.S_pq, self.p, vec, csr.ctr, csr.nbr, types_i32, self.rmax_table, self.bessel_w, self.PQ, g_h, pre[0], gvec)
+            g_h = self.mlp.hidden_grad(gouts)  # gradient w.r.t. phi(h); phi'(h) is applied by the radial adjoint (aux = h)
+            _lib.radial_pq_bwd(dt, self.S_pq, self.p, vec, csr.ctr, csr.nbr, types_i32, self.rmax_table, self.bessel_w, self.PQ, g_h, pre[0], gvec,
+                               **self.mlp.nl_kw)
             return
         g_e0 = torch.empty(E, self.S_rc, dtype=dt, device=vec.device)
-        if self.mlp.is_two_layer_silu:
+        if self.mlp.is_two_layer_nonlinear:
             self.mlp.backward_plain(gouts, pre, [g_e0])
         else:
             self.mlp.backward(gouts, pre, [g_e0], [False])

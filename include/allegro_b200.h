@@ -30,6 +30,13 @@ extern "C" {
 enum { AB2_F64 = 0, AB2_F32 = 1, AB2_BF16 = 2 };
 enum { AB2_ACT_NONE = 0, AB2_ACT_SILU = 1, AB2_ACT_MUL_DSILU = 2 };
 enum { AB2_EPI_NONE = 0, AB2_EPI_MUL_DSILU = 1 };
+/* MLP nonlinearity of the _nl entry points (nequip ScalarMLPFunction `nonlinearity`).  With it the act / epi codes above
+ * keep their meaning: AB2_ACT_SILU applies the nonlinearity phi, AB2_ACT_MUL_DSILU and AB2_EPI_MUL_DSILU multiply by phi'.
+ *   AB2_NL_SILU  phi(x) = x sigma(x)
+ *   AB2_NL_MISH  phi(x) = x tanh(softplus(x))
+ *   AB2_NL_GELU  phi(x) = x Phi(x) = x erfc(-x / sqrt2) / 2   (the exact erf form, not the tanh approximation)
+ * Every entry without the _nl suffix is its _nl twin with AB2_NL_SILU. */
+enum { AB2_NL_SILU = 1, AB2_NL_MISH = 2, AB2_NL_GELU = 3 };
 
 #define AB2_MAX_SEG 4
 #define AB2_MAX_LMAX 4
@@ -114,6 +121,16 @@ int ab2_linear(int dtype, int64_t M, int K, int N, int n_a, const void* const* a
                int n_o, void* const* o_ptr_host, const int64_t* o_ld_host,
                const int32_t* o_width_host, const int32_t* o_accum_host, int epi, const void* aux,
                int64_t aux_ld, void* stream);
+/* ab2_linear with the MLP nonlinearity `nonlin` (AB2_NL_*) in place of SiLU: act applies phi or multiplies by phi'(a_aux),
+ * epi multiplies by phi'(aux).  fp32 / bf16 storage evaluate phi and phi' with fast fp32 intrinsics (gelu: erfcf), fp64
+ * with the IEEE functions.  Returns 1 (and sets ab2_last_error) for an unknown nonlin. */
+int ab2_linear_nl(int dtype, int64_t M, int K, int N, int n_a, const void* const* a_ptr_host,
+                  const int64_t* a_ld_host, const int32_t* a_width_host,
+                  const void* const* a_aux_ptr_host /* nullable */, const int64_t* a_aux_ld_host,
+                  int act, const void* W, const void* W_packed /* nullable */,
+                  int n_o, void* const* o_ptr_host, const int64_t* o_ld_host,
+                  const int32_t* o_width_host, const int32_t* o_accum_host, int epi, const void* aux,
+                  int64_t aux_ld, void* stream, int nonlin);
 
 /* Tensor-core (wgmma) path of ab2_linear.  ab2_linear_packed_bytes returns the size of the
  * packed weight image (bf16 hi + lo parts in the GMMA canonical K-major core-matrix layout) or 0
@@ -146,6 +163,14 @@ int ab2_mlp2(int dtype, int backward, int64_t M, int K, int H, int N, int n_a, c
              const void* w1_row /* nullable: rank-1 backward */, void* pre, int64_t pre_ld, int n_o,
              void* const* o_ptr_host, const int64_t* o_ld_host, const int32_t* o_width_host,
              const int32_t* o_accum_host, void* stream);
+/* ab2_mlp2 with the nonlinearity `nonlin` (AB2_NL_*) in place of SiLU: forward Out (+)= phi(pre) @ W2, backward
+ * Out (+)= ((A @ W1) * phi'(pre)) @ W2.  The results are bitwise those of the two ab2_linear_nl launches it replaces (with
+ * the rank-1 exception above).  Returns 1 (and sets ab2_last_error) for an unknown nonlin. */
+int ab2_mlp2_nl(int dtype, int backward, int64_t M, int K, int H, int N, int n_a, const void* const* a_ptr_host,
+                const int64_t* a_ld_host, const int32_t* a_width_host, const void* W1_packed, const void* W2_packed,
+                const void* w1_row /* nullable: rank-1 backward */, void* pre, int64_t pre_ld, int n_o,
+                void* const* o_ptr_host, const int64_t* o_ld_host, const int32_t* o_width_host,
+                const int32_t* o_accum_host, void* stream, int nonlin);
 
 /* Last latent MLP + readout MLP in one tensor-core kernel per direction (two-layer SiLU MLPs, hidden width H).  The
  * readout reads X[:, :P + S] and the last latent MLP reads [X[:, :P] | s] and writes x_L = X[:, P:P+S], with P = S L;
@@ -167,6 +192,12 @@ int ab2_mlp2(int dtype, int backward, int64_t M, int K, int H, int N, int n_a, c
 int ab2_mlp2_readout(int dtype, int backward, int64_t M, int P, int S, int U, int H, void* x, int64_t x_ld, void* s, int64_t s_ld,
                      void* xl, int64_t xl_ld, void* pre_l, int64_t pre_l_ld, void* pre_r, int64_t pre_r_ld, void* ez, int64_t ez_ld,
                      const void* const* w_packed_host, const void* w2_ro, void* stream);
+/* ab2_mlp2_readout with one nonlinearity `nonlin` (AB2_NL_*) for both MLPs in place of SiLU (silu / silu' above become
+ * phi / phi').  The same numerics contract holds against two ab2_mlp2_nl calls.  Returns 1 (and sets ab2_last_error) for
+ * an unknown nonlin; AB2_NOT_ELIGIBLE as above. */
+int ab2_mlp2_readout_nl(int dtype, int backward, int64_t M, int P, int S, int U, int H, void* x, int64_t x_ld, void* s, int64_t s_ld,
+                        void* xl, int64_t xl_ld, void* pre_l, int64_t pre_l_ld, void* pre_r, int64_t pre_r_ld, void* ez, int64_t ez_ld,
+                        const void* const* w_packed_host, const void* w2_ro, void* stream, int nonlin);
 
 /* _channels.py:44-57 + _contract.py:195-204 fused: gamma[c][j][u] =
  *   sf * sum_{z in row c} Y[z][j] * w[z][irrep(j)][u]      (a4, a7; deterministic, no atomics) */
@@ -339,6 +370,12 @@ int ab2_radial_pq_bwd(int dtype, int64_t E, int S, int num_bessels, double p_cut
                       const int32_t* ctr, const int32_t* nbr, const int32_t* types, const void* rmax_table,
                       int num_types, const void* bessel_w, const void* PQ, const void* g_out, const void* aux,
                       void* gvec, void* stream);
+/* ab2_radial_pq_bwd with phi'(aux[z]) of the nonlinearity `nonlin` (AB2_NL_*) in place of silu'(aux[z]).  Returns 1 (and
+ * sets ab2_last_error) for an unknown nonlin. */
+int ab2_radial_pq_bwd_nl(int dtype, int64_t E, int S, int num_bessels, double p_cut, const void* vec,
+                         const int32_t* ctr, const int32_t* nbr, const int32_t* types, const void* rmax_table,
+                         int num_types, const void* bessel_w, const void* PQ, const void* g_out, const void* aux,
+                         void* gvec, void* stream, int nonlin);
 
 /* ZBL pair term (reference call site allegro/model/allegro_models.py:270-288; the module is nequip's
  * nequip.nn.pair_potential.ZBL = LAMMPS pair_style zbl, constants of pair_zbl_const.h):
