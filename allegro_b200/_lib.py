@@ -57,6 +57,7 @@ _SIGNATURES = {
     "ab2_edge_sum": ([_i32, _i64, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_edge_sum_bwd": ([_i32, _i64, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_force_scatter": ([_i32, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_force_virial_scatter": ([_i32, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_transpose_ui": ([_i32, _i64, _i32, _i32, _vp, _vp, _i32, _vp], C.c_int),
     "ab2_edge_vec": ([_i32, _i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_radial_fwd": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
@@ -84,6 +85,7 @@ _SIGNATURES = {
     "ab2_frame_scratch_elems": ([_i64, _i64], C.c_int64),
     "ab2_frame_sum": ([_i32, _i64, _i64, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_frame_virial": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
+    "ab2_frame_heat_current": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
 }
 
 
@@ -574,6 +576,21 @@ def force_scatter(gvec: torch.Tensor, csr, num_atoms_total: int) -> torch.Tensor
     return F
 
 
+def force_virial_scatter(vec: torch.Tensor, gvec: torch.Tensor, csr, num_atoms_total: int):
+    """``force_scatter`` plus the centroid per-atom virial  W[a] = - sum over the edges whose neighbour is a of vec (x) gvec
+    -> (F [n_total,3], W [n_total,3,3]) in gvec's dtype (ab2_force_virial_scatter; F bitwise force_scatter's)."""
+    N = csr.row_ptr.shape[0] - 1
+    E = csr.nbr.shape[0]
+    assert vec.dtype == gvec.dtype and vec.shape == gvec.shape
+    col_ptr, col_perm = csr.transposed(num_atoms_total)
+    F = torch.empty(num_atoms_total, 3, dtype=gvec.dtype, device=gvec.device)
+    W = torch.empty(num_atoms_total, 3, 3, dtype=gvec.dtype, device=gvec.device)
+    with _timed("force_virial_scatter"):
+        _check(load().ab2_force_virial_scatter(DTYPE_ENUM[gvec.dtype], N, num_atoms_total, E, _ptr(csr.row_ptr), _ptr(col_ptr), _ptr(col_perm),
+                                               _ptr(_contig(vec, "vec")), _ptr(_contig(gvec, "gvec")), _ptr(F), _ptr(W), _stream()))
+    return F, W
+
+
 def transpose_ui(x: torch.Tensor, to_internal: bool) -> torch.Tensor:
     """[E,U,d] (reference strided layout) <-> [E,d,U] (internal)."""
     E, a, b = x.shape
@@ -771,3 +788,19 @@ def frame_virial(vec: torch.Tensor, gvec: torch.Tensor, frame_ptr: torch.Tensor,
         _check(load().ab2_frame_virial(DTYPE_ENUM[vec.dtype], E, B, _ptr(_contig(frame_ptr, "frame_ptr")), _ptr(_contig(row_ptr, "row_ptr")),
                                        _ptr(_contig(vec, "vec")), _ptr(_contig(gvec, "gvec")), _ptr(scratch), m, _ptr(W), _stream()))
     return W
+
+
+def frame_heat_current(e_atom: torch.Tensor, vel: torch.Tensor, W: torch.Tensor, frame_ptr: torch.Tensor) -> torch.Tensor:
+    """J[b] = sum over the atoms [frame_ptr[b], frame_ptr[b+1]) of e_atom[a] vel[a] + W[a] @ vel[a] -> [B,3] in W's dtype
+    (ab2_frame_heat_current; fixed order, no atomics).  ``vel`` is cast to W's dtype."""
+    B = frame_ptr.shape[0] - 1
+    n = W.shape[0]
+    assert e_atom.numel() == n and vel.shape == (n, 3) and W.shape == (n, 3, 3)
+    e_atom = e_atom.reshape(n).to(W.dtype).contiguous()
+    vel = vel.to(W.dtype).contiguous()
+    J = torch.empty(B, 3, dtype=W.dtype, device=W.device)
+    scratch, m = _frame_scratch(n, B, 3, W.device)
+    with _timed("frame_heat_current", 2):
+        _check(load().ab2_frame_heat_current(DTYPE_ENUM[W.dtype], n, B, _ptr(_contig(frame_ptr, "frame_ptr")), _ptr(e_atom), _ptr(vel),
+                                             _ptr(_contig(W, "W")), _ptr(scratch), m, _ptr(J), _stream()))
+    return J

@@ -17,9 +17,10 @@ import torch
 
 from . import data as D
 
-_PER_ATOM = (D.POSITIONS_KEY, D.ATOM_TYPE_KEY, D.PER_ATOM_ENERGY_KEY, D.FORCE_KEY)
+_PER_ATOM = (D.POSITIONS_KEY, D.ATOM_TYPE_KEY, D.PER_ATOM_ENERGY_KEY, D.FORCE_KEY, D.VELOCITY_KEY, D.ATOMIC_VIRIAL_KEY)
 _PER_EDGE = (D.EDGE_CELL_SHIFT_KEY, D.EDGE_ENERGY_KEY, D.EDGE_FEATURES_KEY)
-_PER_FRAME = (D.TOTAL_ENERGY_KEY, D.STRESS_KEY, D.VIRIAL_KEY, D.CELL_KEY, D.PBC_KEY)
+_PER_FRAME = (D.TOTAL_ENERGY_KEY, D.STRESS_KEY, D.VIRIAL_KEY, D.CELL_KEY, D.PBC_KEY, D.HEAT_CURRENT_KEY)
+_PER_FRAME_ROWS = (D.TOTAL_ENERGY_KEY, D.STRESS_KEY, D.VIRIAL_KEY, D.HEAT_CURRENT_KEY)  # kept as [1, ...] per frame
 
 
 def _pbc_of(frame: D.Type) -> torch.Tensor:
@@ -32,7 +33,7 @@ def _pbc_of(frame: D.Type) -> torch.Tensor:
 
 def collate(frames: Sequence[D.Type], r_max: Optional[float] = None) -> D.Type:
     """Single-frame dicts (``pos``, ``atom_types``, optional ``cell`` / ``pbc``, optional ``edge_index`` /
-    ``edge_cell_shift``) -> one batched dict.  When every frame has ``edge_index`` the lists are offset and concatenated;
+    ``edge_cell_shift``, optional ``velocities``, on every frame or none) -> one batched dict.  When every frame has ``edge_index`` the lists are offset and concatenated;
     when none has, the list is built on the device with ``data.neighbor_csr_frames`` (needs ``r_max``; frames of at most
     ``data.FRAMES_MAX_ATOMS`` atoms).  A mix of the two is rejected.  A frame without a cell gets a zero cell and no
     periodic axis."""
@@ -51,6 +52,11 @@ def collate(frames: Sequence[D.Type], r_max: Optional[float] = None) -> D.Type:
         D.BATCH_KEY: torch.repeat_interleave(torch.arange(B, device=dev), torch.tensor(sizes, device=dev)),
         D.NUM_NODES_KEY: torch.tensor(sizes, dtype=torch.long, device=dev),
     }
+    has_vel = [D.VELOCITY_KEY in f for f in frames]
+    if any(has_vel) and not all(has_vel):
+        raise ValueError("collate: some frames carry velocities and others do not")
+    if all(has_vel):
+        out[D.VELOCITY_KEY] = torch.cat([f[D.VELOCITY_KEY].reshape(-1, 3) for f in frames], 0)
     with_cell = any(D.CELL_KEY in f for f in frames)
     pbc = torch.stack([_pbc_of(f) for f in frames]).to(dev)
     if with_cell:
@@ -101,7 +107,7 @@ def split(out: D.Type) -> List[D.Type]:
                 frames[b][k] = out[k][a0:a1]
         for k in _PER_FRAME:
             if k in out:
-                frames[b][k] = out[k][b : b + 1] if k in (D.TOTAL_ENERGY_KEY, D.STRESS_KEY, D.VIRIAL_KEY) else out[k][b]
+                frames[b][k] = out[k][b : b + 1] if k in _PER_FRAME_ROWS else out[k][b]
     if D.CSR_KEY in out:
         csr = out[D.CSR_KEY]
         rp = csr.row_ptr.cpu()

@@ -26,12 +26,18 @@ from . import data as D
 
 class AllegroCalculator:
     def __init__(self, model, r_max: float, skin: float = 0.5, pbc=(True, True, True), use_graph: bool = True,
-                 compute_stress: bool = False, check_every: int = 1):
+                 compute_stress: bool = False, check_every: int = 1, compute_atomic_virial: bool = False,
+                 compute_heat_current: bool = False):
         assert skin >= 0.0 and check_every >= 1
         self.model, self.r_max, self.skin = model, float(r_max), float(skin)
         self.pbc = tuple(bool(p) for p in (pbc if not isinstance(pbc, bool) else (pbc,) * 3))
         self.compute_stress = bool(compute_stress)
+        # per-atom virial / heat current: skin edges have zero gradient, so they add nothing to either
+        self.compute_heat_current = bool(compute_heat_current)
+        self.compute_atomic_virial = bool(compute_atomic_virial) or self.compute_heat_current
         inner = getattr(model, "model", model)
+        if self.compute_atomic_virial and not hasattr(inner, "energy_and_forces"):
+            raise NotImplementedError("atomic_virial / heat_current need the fused energy_and_forces path")
         self.use_graph = bool(use_graph) and hasattr(inner, "energy_and_forces")
         self.check_every = int(check_every)
         self.n_rebuilds = 0
@@ -84,28 +90,44 @@ class AllegroCalculator:
         if self.use_graph:
             from .graph import GraphedEnergyForces
 
-            self._graphed = GraphedEnergyForces(self.model, data, stress=self.compute_stress)
+            self._graphed = GraphedEnergyForces(self.model, data, stress=self.compute_stress, **self._extra_kw())
+
+    def _extra_kw(self):
+        if not self.compute_atomic_virial:
+            return {}
+        return dict(atomic_virial=True, heat_current=self.compute_heat_current)
 
     # ---- evaluation ----------------------------------------------------------------------------
-    def compute(self, pos: torch.Tensor, cell: Optional[torch.Tensor] = None, atom_types: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
-        """-> {"energy" [1,1], "forces" [N,3], "atomic_energy" [N,1]} (+ "stress", "virial" [1,3,3] if asked for).
-        The returned tensors are the model's output buffers: with graph replay they are overwritten by the next call."""
+    def compute(self, pos: torch.Tensor, cell: Optional[torch.Tensor] = None, atom_types: Optional[torch.Tensor] = None,
+                velocities: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
+        """-> {"energy" [1,1], "forces" [N,3], "atomic_energy" [N,1]} (+ "stress", "virial" [1,3,3] if asked for;
+        "atomic_virial" [N,3,3] with compute_atomic_virial; "heat_current" [1,3] with compute_heat_current, which needs
+        ``velocities`` [N,3]).  The returned tensors are the model's output buffers: with graph replay they are
+        overwritten by the next call."""
+        if self.compute_heat_current and (velocities is None or tuple(velocities.shape) != (pos.shape[0], 3)):
+            raise ValueError(f"compute_heat_current needs velocities [{pos.shape[0]},3]")
         if self._needs_rebuild(pos, cell, atom_types):
             self._rebuild(pos, cell, atom_types)
         if self._graphed is not None:
-            out = self._graphed(pos)
+            out = self._graphed(pos, velocities if self.compute_heat_current else None)
         else:
             d = dict(self._data)
             d[D.POSITIONS_KEY] = pos
+            if self.compute_heat_current:
+                d[D.VELOCITY_KEY] = velocities
             inner = getattr(self.model, "model", self.model)
             if hasattr(inner, "energy_and_forces"):
-                out = inner.energy_and_forces(d, stress=self.compute_stress)
+                out = inner.energy_and_forces(d, stress=self.compute_stress, **self._extra_kw())
             else:
                 out = self.model(d)
         self.n_evaluations += 1
         res = {"energy": out[D.TOTAL_ENERGY_KEY], "forces": out[D.FORCE_KEY], "atomic_energy": out[D.PER_ATOM_ENERGY_KEY]}
         if self.compute_stress and D.STRESS_KEY in out:
             res["stress"], res["virial"] = out[D.STRESS_KEY], out[D.VIRIAL_KEY]
+        if self.compute_atomic_virial:
+            res["atomic_virial"] = out[D.ATOMIC_VIRIAL_KEY]
+        if self.compute_heat_current:
+            res["heat_current"] = out[D.HEAT_CURRENT_KEY]
         return res
 
     @property

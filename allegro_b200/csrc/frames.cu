@@ -1,4 +1,5 @@
-// Per-frame reductions of a batch of frames concatenated into one graph: the total energy of every frame and its virial.
+// Per-frame reductions of a batch of frames concatenated into one graph: the total energy of every frame, its virial and
+// its potential heat current.
 //
 // A batch may hold one frame of several million edges next to thousands of frames of ten edges, and the result of a frame
 // may depend neither on the launch nor on the other frames.  So every frame is cut into fixed chunks of FR_CHUNK
@@ -27,11 +28,13 @@ __device__ __forceinline__ int64_t fr_vid(const int32_t* frame_ptr, const int32_
     return fr_start(frame_ptr, row_ptr, b) / FR_CHUNK + b;
 }
 
-// W values per element: W = 1, out += x[e];  W = 9, out[a][c] += vec[e][a] * gvec[e][c]
+// W values per element: W = 1, out += x[e];  W = 9, out[a][c] += vec[e][a] * gvec[e][c] (x = vec, y = gvec);
+// W = 3, out[a] += e[e] v[e][a] + sum_c m[e][a][c] v[e][c]  (x = e_atom, y = vel, m = per-atom virial)
 template <typename T, int W>
 __global__ void __launch_bounds__(FR_THREADS) fr_partial_kernel(int64_t B, const int32_t* __restrict__ frame_ptr,
                                                                 const int32_t* __restrict__ row_ptr, const T* __restrict__ x,
-                                                                const T* __restrict__ y, double* __restrict__ part) {
+                                                                const T* __restrict__ y, const T* __restrict__ m,
+                                                                double* __restrict__ part) {
     const int64_t v = blockIdx.x;
     int64_t lo = 0, hi = B - 1;
     while (lo < hi) {
@@ -50,6 +53,16 @@ __global__ void __launch_bounds__(FR_THREADS) fr_partial_kernel(int64_t B, const
     for (int64_t e = e0 + threadIdx.x; e < e1; e += FR_THREADS) {
         if (W == 1) {
             acc[0] += (double)x[e];
+        } else if (W == 3) {
+            const double ea = (double)x[e];
+            const double v[3] = {(double)y[e * 3 + 0], (double)y[e * 3 + 1], (double)y[e * 3 + 2]};
+#pragma unroll
+            for (int p = 0; p < 3; ++p) {
+                double s = ea * v[p];
+#pragma unroll
+                for (int q = 0; q < 3; ++q) s += (double)m[e * 9 + p * 3 + q] * v[q];
+                acc[p] += s;
+            }
         } else {
             const double a[3] = {(double)x[e * 3 + 0], (double)x[e * 3 + 1], (double)x[e * 3 + 2]};
             const double g[3] = {(double)y[e * 3 + 0], (double)y[e * 3 + 1], (double)y[e * 3 + 2]};
@@ -94,20 +107,25 @@ __global__ void __launch_bounds__(256) fr_combine_kernel(int64_t B, const int32_
 
 template <int W>
 int fr_run(int acc_dtype, int64_t total, int64_t B, const int32_t* frame_ptr, const int32_t* row_ptr, const void* x, const void* y,
-           double* scratch, int64_t scratch_elems, void* out, void* stream) {
+           const void* m, double* scratch, int64_t scratch_elems, void* out, void* stream) {
     if (B == 0) return 0;
     AB2_CHECK_ARG(acc_dtype == AB2_F64 || acc_dtype == AB2_F32, "values must be fp64 or fp32");
-    AB2_CHECK_ARG(frame_ptr && out && (total == 0 || (x && scratch)) && (W == 1 || total == 0 || y), "null pointer");
+    AB2_CHECK_ARG(frame_ptr && out && (total == 0 || (x && scratch)) && (W == 1 || total == 0 || y) && (W != 3 || total == 0 || m),
+                  "null pointer");
     AB2_CHECK_ARG(total >= 0 && B > 0, "sizes");
     const int64_t nv = total / FR_CHUNK + B;
     AB2_CHECK_ARG(total == 0 || scratch_elems >= nv * W, "scratch smaller than ab2_frame_scratch_elems(total, n_frames) * width");
     AB2_CHECK_ARG(nv <= 0x7fffffffLL, "too many chunks for one launch");
     cudaStream_t st = (cudaStream_t)stream;
     if (acc_dtype == AB2_F64) {
-        if (total > 0) fr_partial_kernel<double, W><<<(unsigned)nv, FR_THREADS, 0, st>>>(B, frame_ptr, row_ptr, (const double*)x, (const double*)y, scratch);
+        if (total > 0)
+            fr_partial_kernel<double, W><<<(unsigned)nv, FR_THREADS, 0, st>>>(B, frame_ptr, row_ptr, (const double*)x, (const double*)y,
+                                                                             (const double*)m, scratch);
         fr_combine_kernel<double, W><<<ab2_blocks(B * W, 256), 256, 0, st>>>(B, frame_ptr, row_ptr, scratch, (double*)out);
     } else {
-        if (total > 0) fr_partial_kernel<float, W><<<(unsigned)nv, FR_THREADS, 0, st>>>(B, frame_ptr, row_ptr, (const float*)x, (const float*)y, scratch);
+        if (total > 0)
+            fr_partial_kernel<float, W><<<(unsigned)nv, FR_THREADS, 0, st>>>(B, frame_ptr, row_ptr, (const float*)x, (const float*)y,
+                                                                            (const float*)m, scratch);
         fr_combine_kernel<float, W><<<ab2_blocks(B * W, 256), 256, 0, st>>>(B, frame_ptr, row_ptr, scratch, (float*)out);
     }
     AB2_CUDA_LAUNCH_CHECK();
@@ -120,11 +138,16 @@ extern "C" int64_t ab2_frame_scratch_elems(int64_t total, int64_t n_frames) { re
 
 extern "C" int ab2_frame_sum(int acc_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* x, double* scratch,
                              int64_t scratch_elems, void* out, void* stream) {
-    return fr_run<1>(acc_dtype, n, n_frames, frame_ptr, nullptr, x, nullptr, scratch, scratch_elems, out, stream);
+    return fr_run<1>(acc_dtype, n, n_frames, frame_ptr, nullptr, x, nullptr, nullptr, scratch, scratch_elems, out, stream);
 }
 
 extern "C" int ab2_frame_virial(int acc_dtype, int64_t E, int64_t n_frames, const int32_t* frame_ptr, const int32_t* row_ptr,
                                 const void* vec, const void* gvec, double* scratch, int64_t scratch_elems, void* W, void* stream) {
     AB2_CHECK_ARG(row_ptr != nullptr, "null row_ptr");
-    return fr_run<9>(acc_dtype, E, n_frames, frame_ptr, row_ptr, vec, gvec, scratch, scratch_elems, W, stream);
+    return fr_run<9>(acc_dtype, E, n_frames, frame_ptr, row_ptr, vec, gvec, nullptr, scratch, scratch_elems, W, stream);
+}
+
+extern "C" int ab2_frame_heat_current(int acc_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* e_atom,
+                                      const void* vel, const void* W, double* scratch, int64_t scratch_elems, void* J, void* stream) {
+    return fr_run<3>(acc_dtype, n, n_frames, frame_ptr, nullptr, e_atom, vel, W, scratch, scratch_elems, J, stream);
 }

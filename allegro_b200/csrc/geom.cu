@@ -185,12 +185,18 @@ extern "C" int ab2_edge_sum_bwd(int acc_dtype, int64_t E, const int32_t* ctr, co
 // (edges grouped by neighbour: col_ptr[n_total+1], col_perm[E] = edge ids sorted by neighbour,
 // built once per neighbour list).  One warp per atom, fixed summation order, no atomics: forces
 // are bitwise reproducible from run to run, and F needs no zero-fill.
+//
+// WITH_W: the same walk also forms the centroid per-atom virial
+//   W[a][p][q] = - sum_{z : nbr[z] = a} vec[z][p] gvec[z][q]
+// from the column loop (vec gathered through col_perm like gvec).  F's arithmetic is untouched
+// by it, so F is bitwise that of the instantiation without W.  The 9 lane sums are reduced in
+// the fixed order p-major, q-minor.
 // ---------------------------------------------------------------------------------------
-template <typename TAcc>
+template <typename TAcc, bool WITH_W>
 __global__ void __launch_bounds__(256) force_scatter_kernel(int64_t N, int64_t n_total, const int32_t* __restrict__ row_ptr,
                                                             const int32_t* __restrict__ col_ptr,
-                                                            const int32_t* __restrict__ col_perm, const TAcc* __restrict__ gvec,
-                                                            TAcc* __restrict__ F) {
+                                                            const int32_t* __restrict__ col_perm, const TAcc* __restrict__ vec,
+                                                            const TAcc* __restrict__ gvec, TAcc* __restrict__ F, TAcc* __restrict__ W) {
     const int64_t a = ((int64_t)blockIdx.x * 256 + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (a >= n_total) return;
@@ -203,18 +209,41 @@ __global__ void __launch_bounds__(256) force_scatter_kernel(int64_t N, int64_t n
             sz += gvec[(int64_t)z * 3 + 2];
         }
     }
+    TAcc w[WITH_W ? 9 : 1];
+    if (WITH_W) {
+#pragma unroll
+        for (int k = 0; k < 9; ++k) w[k] = 0;
+    }
     const int cb = col_ptr[a], ce = col_ptr[a + 1];
     for (int t = cb + lane; t < ce; t += 32) {
         const int64_t z = col_perm[t];
-        sx -= gvec[z * 3 + 0];
-        sy -= gvec[z * 3 + 1];
-        sz -= gvec[z * 3 + 2];
+        const TAcc gx = gvec[z * 3 + 0], gy = gvec[z * 3 + 1], gz = gvec[z * 3 + 2];
+        sx -= gx;
+        sy -= gy;
+        sz -= gz;
+        if (WITH_W) {
+            const TAcc v[3] = {vec[z * 3 + 0], vec[z * 3 + 1], vec[z * 3 + 2]};
+#pragma unroll
+            for (int p = 0; p < 3; ++p) {
+                w[p * 3 + 0] += v[p] * gx;
+                w[p * 3 + 1] += v[p] * gy;
+                w[p * 3 + 2] += v[p] * gz;
+            }
+        }
     }
     sx = warp_sum(sx); sy = warp_sum(sy); sz = warp_sum(sz);
+    if (WITH_W) {
+#pragma unroll
+        for (int k = 0; k < 9; ++k) w[k] = warp_sum(w[k]);
+    }
     if (lane == 0) {
         F[a * 3 + 0] = sx;
         F[a * 3 + 1] = sy;
         F[a * 3 + 2] = sz;
+        if (WITH_W) {
+#pragma unroll
+            for (int k = 0; k < 9; ++k) W[a * 9 + k] = -w[k];
+        }
     }
 }
 
@@ -224,8 +253,21 @@ extern "C" int ab2_force_scatter(int acc_dtype, int64_t N, int64_t n_total, int6
     AB2_CHECK_ARG(row_ptr && col_ptr && gvec && F && (E == 0 || col_perm), "null pointer");
     AB2_CHECK_ARG(N <= n_total, "more centres than atoms");
     cudaStream_t st = (cudaStream_t)stream;
-    AB2_DISPATCH_ACC(acc_dtype, force_scatter_kernel<TAcc><<<ab2_blocks(n_total * 32, 256), 256, 0, st>>>(
-                                    N, n_total, row_ptr, col_ptr, col_perm, (const TAcc*)gvec, (TAcc*)F));
+    AB2_DISPATCH_ACC(acc_dtype, force_scatter_kernel<TAcc, false><<<ab2_blocks(n_total * 32, 256), 256, 0, st>>>(
+                                    N, n_total, row_ptr, col_ptr, col_perm, nullptr, (const TAcc*)gvec, (TAcc*)F, nullptr));
+    AB2_CUDA_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int ab2_force_virial_scatter(int acc_dtype, int64_t N, int64_t n_total, int64_t E, const int32_t* row_ptr,
+                                        const int32_t* col_ptr, const int32_t* col_perm, const void* vec, const void* gvec, void* F,
+                                        void* W, void* stream) {
+    if (n_total == 0) return 0;
+    AB2_CHECK_ARG(row_ptr && col_ptr && F && W && (E == 0 || (col_perm && vec && gvec)), "null pointer");
+    AB2_CHECK_ARG(N <= n_total, "more centres than atoms");
+    cudaStream_t st = (cudaStream_t)stream;
+    AB2_DISPATCH_ACC(acc_dtype, force_scatter_kernel<TAcc, true><<<ab2_blocks(n_total * 32, 256), 256, 0, st>>>(
+                                    N, n_total, row_ptr, col_ptr, col_perm, (const TAcc*)vec, (const TAcc*)gvec, (TAcc*)F, (TAcc*)W));
     AB2_CUDA_LAUNCH_CHECK();
     return 0;
 }

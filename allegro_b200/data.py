@@ -42,6 +42,12 @@ VIRIAL_KEY = "virial"
 # so the int64 COO list never has to exist (neighbor_csr below; 5x10^7 edges at the 1M-atom scale).
 CSR_KEY = "edge_csr"
 EDGE_SHIFT_VEC_KEY = "edge_shift_vec"
+# per-atom virial and heat current (this package): velocities [N,3] in; the centroid per-atom virial [n_rows,3,3]
+# (W[a] = -sum over the edges whose neighbour is a of r_z (x) dE/dr_z, not symmetric) and the potential heat current
+# J = sum_a E_a v_a + W[a] v_a ([1,3] for one frame, [B,3] for a batch) out
+VELOCITY_KEY = "velocities"
+ATOMIC_VIRIAL_KEY = "atomic_virial"
+HEAT_CURRENT_KEY = "heat_current"
 
 Type = Dict[str, torch.Tensor]
 

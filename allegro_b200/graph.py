@@ -17,7 +17,8 @@ from . import data as D
 
 
 class GraphedEnergyForces:
-    def __init__(self, model: torch.nn.Module, data: D.Type, warmup: int = 3, stress: bool = False):
+    def __init__(self, model: torch.nn.Module, data: D.Type, warmup: int = 3, stress: bool = False, atomic_virial: bool = False,
+                 heat_current: bool = False):
         inner = getattr(model, "model", model)  # ForceStressOutput(FusedAllegroEnergy) or the energy model itself
         if not hasattr(inner, "energy_and_forces"):
             raise TypeError("model has no fused energy_and_forces path")
@@ -25,7 +26,16 @@ class GraphedEnergyForces:
         self.data = dict(data)
         self.static_pos = data[D.POSITIONS_KEY].detach().clone()
         self.data[D.POSITIONS_KEY] = self.static_pos
+        # with the heat current the velocities are an input of the graph as well: a static buffer, like the positions
+        self.static_vel = None
+        if heat_current:
+            v = data.get(D.VELOCITY_KEY)
+            self.static_vel = (v.detach().clone() if v is not None
+                               else torch.zeros(self.static_pos.shape[0], 3, dtype=self.static_pos.dtype, device=self.static_pos.device))
+            self.data[D.VELOCITY_KEY] = self.static_vel
         kw = {"stress": True} if stress else {}  # stress / virial captured into the graph only on request
+        if atomic_virial or heat_current:
+            kw.update(atomic_virial=bool(atomic_virial), heat_current=bool(heat_current))
         prof = _lib.PROF.enabled
         _lib.PROF.enabled = False
         s = torch.cuda.Stream()
@@ -42,10 +52,15 @@ class GraphedEnergyForces:
         self.launches_per_replay = _lib.PROF.launches - n0
         _lib.PROF.enabled = prof
 
-    def __call__(self, pos: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
-        """Replay with new positions (device or pinned-host tensor); returns the static outputs."""
+    def __call__(self, pos: Optional[torch.Tensor] = None, vel: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
+        """Replay with new positions (and, with the heat current, velocities; device or pinned-host tensors); returns the
+        static outputs."""
         if pos is not None:
             self.static_pos.copy_(pos, non_blocking=True)
+        if vel is not None:
+            if self.static_vel is None:
+                raise ValueError("velocities are only an input of a graph captured with heat_current=True")
+            self.static_vel.copy_(vel, non_blocking=True)
         self.graph.replay()
         _lib.PROF.launches += self.launches_per_replay
         return self.out

@@ -159,15 +159,21 @@ class FusedAllegroEnergy(torch.nn.Module):
             self._core_key = key
         return self._core
 
-    def energy_and_forces(self, data: D.Type, stress: bool = False) -> D.Type:
+    def energy_and_forces(self, data: D.Type, stress: bool = False, atomic_virial: bool = False, heat_current: bool = False) -> D.Type:
         """Energies AND forces in one pass of hand-written kernels (no torch autograd anywhere):
         what ForceStressOutput(AllegroEnergyModel) computes (allegro_models.py:101-103).  With
         ``stress=True`` and a cell in ``data`` also nequip's ``stress`` = sym(sum_z r_z (x) dE/dr_z)/V and
-        ``virial`` = -sym(...) ([1,3,3] each), from the same per-edge gradients."""
+        ``virial`` = -sym(...) ([1,3,3] each), from the same per-edge gradients.
+
+        ``atomic_virial=True`` adds ``atomic_virial`` [n,3,3], the centroid per-atom virial
+        W[a] = -sum_{z: nbr[z] = a} r_z (x) dE/dr_z (9 components, not symmetric; sym(sum_a W[a]) = ``virial``), one row per
+        atom, ghosts included: a ghost row holds what its owner must receive, like a ghost force.  ``heat_current=True``
+        (implies ``atomic_virial``) adds ``heat_current`` [1,3] = sum_a E_a v_a + W[a] v_a over every row, from ``velocities``
+        [n,3] and the final ``atomic_energy`` (scale/shift and pair term included); the kinetic term is the caller's."""
         pos = data[D.POSITIONS_KEY]
         if not pos.is_cuda:
             raise RuntimeError("allegro_b200: inputs must be CUDA tensors (no CPU fallback on the hot path)")
-        return self._energy_and_forces(data, stress)
+        return self._energy_and_forces(data, stress, atomic_virial, heat_current)
 
     def _cached(self, slot: str, srcs, extra, build):
         """Derived per-neighbour-list data (CSR, int32 types, shift vectors) keyed on the IDENTITY of the
@@ -197,11 +203,36 @@ class FusedAllegroEnergy(torch.nn.Module):
             raise NotImplementedError("allegro_b200: more than one cell in `data` (batched frames) is not supported by the "
                                       "single-frame entry points; use energy_and_forces_frames")
 
-    def _energy_and_forces(self, data: D.Type, stress: bool) -> D.Type:
+    @staticmethod
+    def _velocities(data: D.Type, n: int, heat_current: bool) -> Optional[torch.Tensor]:
+        """``velocities`` [n,3] when the heat current is asked for (checked before any kernel runs), else None."""
+        if not heat_current:
+            return None
+        v = data.get(D.VELOCITY_KEY)
+        if v is None:
+            raise ValueError(f"heat_current=True needs `{D.VELOCITY_KEY}` [{n},3]")
+        if tuple(v.shape) != (n, 3):
+            raise ValueError(f"`{D.VELOCITY_KEY}` has shape {tuple(v.shape)}, expected ({n}, 3): one row per atom")
+        return v
+
+    def _heat_current_ptr(self, n: int, device):
+        return self._cached("heat_ptr", (), (n, str(device)), lambda: torch.tensor([0, n], dtype=torch.int32, device=device))
+
+    @staticmethod
+    def _pad_rows(e_atom: torch.Tensor, n: int) -> torch.Tensor:
+        """Per-atom energies on every row: atoms without a centre row (ghosts of a prepared CSR) have none."""
+        e = e_atom.reshape(-1)
+        if e.shape[0] == n:
+            return e
+        return torch.cat([e, torch.zeros(n - e.shape[0], dtype=e.dtype, device=e.device)])
+
+    def _energy_and_forces(self, data: D.Type, stress: bool, atomic_virial: bool = False, heat_current: bool = False) -> D.Type:
         self._single_frame(data)
         pos = data[D.POSITIONS_KEY]
         core = self.core()
         n = pos.shape[0]
+        vel = self._velocities(data, n, heat_current)
+        atomic_virial = bool(atomic_virial) or bool(heat_current)
         prepared = D.CSR_KEY in data  # prebuilt CSR (+ shift vectors in CSR order): data.neighbor_csr
         csr = data[D.CSR_KEY] if prepared else self._csr(data[D.EDGE_INDEX_KEY], n)
         shift_vec = None
@@ -231,12 +262,17 @@ class FusedAllegroEnergy(torch.nn.Module):
         pair = None
         if self.pair_potential is not None:
             pair = (self.pair_potential, self.edge_norm.rmax_table.to(device=pos.device, dtype=core.acc))
-        Ei, F, X, Ez, virial, Ei_pair = energy_forces(core, self._upstream, csr, pos.detach().contiguous(), types_i32, shift_vec,
-                                                      gscale, want_virial, pair=pair)
+        Ei, F, X, Ez, virial, Ei_pair, W = energy_forces(core, self._upstream, csr, pos.detach().contiguous(), types_i32, shift_vec,
+                                                         gscale, want_virial, pair=pair, want_atomic_virial=atomic_virial)
         e_atom = ss(Ei.unsqueeze(-1), types_c)
         if Ei_pair is not None:
             e_atom = e_atom + Ei_pair.unsqueeze(-1).to(e_atom.dtype)
         out = dict(data)
+        if atomic_virial:
+            out[D.ATOMIC_VIRIAL_KEY] = W.to(pos.dtype)
+        if heat_current:
+            J = _lib.frame_heat_current(self._pad_rows(e_atom, n), vel, W, self._heat_current_ptr(n, pos.device))
+            out[D.HEAT_CURRENT_KEY] = J.to(pos.dtype)
         if csr.perm is not None:
             inv = torch.empty_like(csr.perm)
             inv[csr.perm] = torch.arange(csr.perm.shape[0], device=csr.perm.device)
@@ -256,7 +292,7 @@ class FusedAllegroEnergy(torch.nn.Module):
     # ------------------------------------------------------------------------------------
     # many frames per call
     # ------------------------------------------------------------------------------------
-    def energy_and_forces_frames(self, data: D.Type, stress: bool = False) -> D.Type:
+    def energy_and_forces_frames(self, data: D.Type, stress: bool = False, atomic_virial: bool = False, heat_current: bool = False) -> D.Type:
         """Energies and forces of a BATCH of frames in one pass: the frames are one larger graph to the kernels (every
         reduction on the path is per centre or per atom), and the per-frame sums are fixed-order segmented reductions
         (ab2_frame_sum / ab2_frame_virial), so a frame's results do not depend on the rest of the batch.
@@ -266,11 +302,12 @@ class FusedAllegroEnergy(torch.nn.Module):
         ``edge_csr`` + ``edge_shift_vec`` of ``data.neighbor_csr_frames`` (``batch.collate`` builds either).  Writes
         ``atomic_energy`` [N,1], ``forces`` [N,3], ``edge_energy`` / ``edge_features`` (input edge order) and
         ``total_energy`` [B,1]; with ``stress=True`` also ``stress`` / ``virial`` [B,3,3], which need a non-singular cell
-        on every frame."""
+        on every frame.  ``atomic_virial`` / ``heat_current`` as in ``energy_and_forces``: ``atomic_virial`` [N,3,3] and
+        ``heat_current`` [B,3], one row per frame (ab2_frame_heat_current)."""
         pos = data[D.POSITIONS_KEY]
         if not pos.is_cuda:
             raise RuntimeError("allegro_b200: inputs must be CUDA tensors (no CPU fallback on the hot path)")
-        return self._energy_and_forces_frames(data, stress)
+        return self._energy_and_forces_frames(data, stress, atomic_virial, heat_current)
 
     @staticmethod
     def _frame_layout(batch: torch.Tensor, num: Optional[torch.Tensor], csr: D.EdgeCSR, n: int):
@@ -305,10 +342,12 @@ class FusedAllegroEnergy(torch.nn.Module):
         frame_ptr[1:] = torch.cumsum(counts, 0).to(device=frame_ptr.device, dtype=torch.int32)
         return frame_ptr, B
 
-    def _energy_and_forces_frames(self, data: D.Type, stress: bool) -> D.Type:
+    def _energy_and_forces_frames(self, data: D.Type, stress: bool, atomic_virial: bool = False, heat_current: bool = False) -> D.Type:
         pos = data[D.POSITIONS_KEY]
         core = self.core()
         n = pos.shape[0]
+        vel = self._velocities(data, n, heat_current)
+        atomic_virial = bool(atomic_virial) or bool(heat_current)
         if D.BATCH_KEY not in data:
             raise ValueError("energy_and_forces_frames needs `batch` (and `num_atoms`): see allegro_b200.batch.collate")
         batch, num = data[D.BATCH_KEY], data.get(D.NUM_NODES_KEY)
@@ -362,12 +401,16 @@ class FusedAllegroEnergy(torch.nn.Module):
         pair = None
         if self.pair_potential is not None:
             pair = (self.pair_potential, self.edge_norm.rmax_table.to(device=pos.device, dtype=core.acc))
-        Ei, F, X, Ez, virial, Ei_pair = energy_forces(core, self._upstream, csr, pos.detach().contiguous(), types_i32, shift_vec,
-                                                      gscale, bool(stress), pair=pair, frame_ptr=frame_ptr)
+        Ei, F, X, Ez, virial, Ei_pair, W = energy_forces(core, self._upstream, csr, pos.detach().contiguous(), types_i32, shift_vec,
+                                                         gscale, bool(stress), pair=pair, frame_ptr=frame_ptr, want_atomic_virial=atomic_virial)
         e_atom = ss(Ei.unsqueeze(-1), types)
         if Ei_pair is not None:
             e_atom = e_atom + Ei_pair.unsqueeze(-1).to(e_atom.dtype)
         out = dict(data)
+        if atomic_virial:
+            out[D.ATOMIC_VIRIAL_KEY] = W.to(pos.dtype)
+        if heat_current:
+            out[D.HEAT_CURRENT_KEY] = _lib.frame_heat_current(e_atom.reshape(-1), vel, W, frame_ptr).to(pos.dtype)
         if csr.perm is not None:
             inv = torch.empty_like(csr.perm)
             inv[csr.perm] = torch.arange(csr.perm.shape[0], device=csr.perm.device)
@@ -434,11 +477,18 @@ class ForceStressOutput(torch.nn.Module):
     def __init__(self, model: torch.nn.Module):
         super().__init__()
         self.model = model
+        # per-atom virial / heat current (``atomic_virial`` / ``heat_current`` outputs of energy_and_forces): off by default
+        self.compute_atomic_virial = False
+        self.compute_heat_current = False
 
     def forward(self, data: D.Type) -> D.Type:
+        av, hc = bool(getattr(self, "compute_atomic_virial", False)), bool(getattr(self, "compute_heat_current", False))
         if hasattr(self.model, "energy_and_forces") and not getattr(self, "use_autograd", False):
             # like nequip's ForceStressOutput, stress/virial come with the forces whenever a cell is given
-            return self.model.energy_and_forces(data, stress=getattr(self, "compute_stress", True))
+            kw = dict(atomic_virial=av, heat_current=hc) if (av or hc) else {}
+            return self.model.energy_and_forces(data, stress=getattr(self, "compute_stress", True), **kw)
+        if av or hc:
+            raise NotImplementedError("atomic_virial / heat_current come from the fused energy_and_forces path only, not from autograd")
         data = dict(data)
         pos = data[D.POSITIONS_KEY].detach().clone().requires_grad_(True)
         data[D.POSITIONS_KEY] = pos
@@ -449,9 +499,9 @@ class ForceStressOutput(torch.nn.Module):
         out[D.POSITIONS_KEY] = pos.detach()
         return {k: (v.detach() if isinstance(v, torch.Tensor) else v) for k, v in out.items()}
 
-    def energy_and_forces_frames(self, data: D.Type, stress: bool = False) -> D.Type:
+    def energy_and_forces_frames(self, data: D.Type, stress: bool = False, atomic_virial: bool = False, heat_current: bool = False) -> D.Type:
         """A batch of frames in one call: ``FusedAllegroEnergy.energy_and_forces_frames``."""
-        return self.model.energy_and_forces_frames(data, stress)
+        return self.model.energy_and_forces_frames(data, stress, atomic_virial, heat_current)
 
 
 def _builder_common(kwargs: Dict):

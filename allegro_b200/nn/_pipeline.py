@@ -463,14 +463,16 @@ class UpstreamPack:
 
 def energy_forces(core: "AllegroCore", up: UpstreamPack, csr: EdgeCSR, pos: torch.Tensor, types_i32: torch.Tensor,
                   shift_vec: Optional[torch.Tensor], gEi_scale: Optional[torch.Tensor], want_virial: bool = False, pair=None,
-                  frame_ptr: Optional[torch.Tensor] = None):
-    """Whole path with no torch autograd: positions -> (Ei [N], forces [n_atoms,3], X, Ez, virial).
+                  frame_ptr: Optional[torch.Tensor] = None, want_atomic_virial: bool = False):
+    """Whole path with no torch autograd: positions -> (Ei [N], forces [n_atoms,3], X, Ez, virial, Ei_pair, W).
     ``gEi_scale`` = d E_total / d Ei (per-type scales), None = ones.  ``virial`` (only if asked for) is
     sum_z r_z (x) dE/dr_z [3,3] = dE/d(strain) before symmetrisation, from the per-edge gradients the
     force scatter consumes anyway.  ``pair`` = (ZBL module, r_max table) adds the pair potential's gradient to the
     per-edge gradients and returns its per-atom energies as a sixth value (added AFTER the per-type scale/shift,
     allegro_models.py:270-288).  ``frame_ptr`` [B+1] int32 (a batch of frames concatenated into one graph): the virial is
-    then per frame, [B,3,3] (ab2_frame_virial)."""
+    then per frame, [B,3,3] (ab2_frame_virial).  ``want_atomic_virial``: W (the seventh value, else None) is the centroid
+    per-atom virial [n_atoms,3,3], W[a] = -sum_{z: nbr[z] = a} r_z (x) dE/dr_z, formed by the force scatter itself
+    (ab2_force_virial_scatter)."""
     dt, acc = core.dtype, core.acc
     vshape = (3, 3) if frame_ptr is None else (frame_ptr.shape[0] - 1, 3, 3)
     E = csr.num_edges
@@ -481,7 +483,8 @@ def energy_forces(core: "AllegroCore", up: UpstreamPack, csr: EdgeCSR, pos: torc
         return (torch.zeros(csr.num_atoms, dtype=acc, device=dev), torch.zeros(pos.shape[0], 3, dtype=acc, device=dev),
                 torch.empty(0, core.S * (core.L + 1), dtype=dt, device=dev), torch.empty(0, 1, dtype=dt, device=dev),
                 torch.zeros(vshape, dtype=acc, device=dev) if want_virial else None,
-                torch.zeros(csr.num_atoms, dtype=acc, device=dev) if pair is not None else None)
+                torch.zeros(csr.num_atoms, dtype=acc, device=dev) if pair is not None else None,
+                torch.zeros(pos.shape[0], 3, 3, dtype=acc, device=dev) if want_atomic_virial else None)
     _lib.set_tag("fwd.radial")
     vec = _lib.edge_vec(pos, csr.ctr, csr.nbr, shift_vec, acc)
     if up.fold:
@@ -503,8 +506,12 @@ def energy_forces(core: "AllegroCore", up: UpstreamPack, csr: EdgeCSR, pos: torc
     virial = None
     if want_virial:
         virial = (vec.T @ gvec.to(vec.dtype)) if frame_ptr is None else _lib.frame_virial(vec, gvec.to(vec.dtype), frame_ptr, csr.row_ptr)
-    F = _lib.force_scatter(gvec, csr, pos.shape[0])
-    return Ei, F, X, Ez, virial, Ei_pair
+    W = None
+    if want_atomic_virial:
+        F, W = _lib.force_virial_scatter(vec, gvec, csr, pos.shape[0])
+    else:
+        F = _lib.force_scatter(gvec, csr, pos.shape[0])
+    return Ei, F, X, Ez, virial, Ei_pair, W
 
 
 class _CoreFn(torch.autograd.Function):

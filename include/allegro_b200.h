@@ -275,6 +275,19 @@ int ab2_edge_sum_bwd(int acc_dtype, int64_t E, const int32_t* ctr, const void* g
 int ab2_force_scatter(int acc_dtype, int64_t N, int64_t n_total, int64_t E, const int32_t* row_ptr,
                       const int32_t* col_ptr, const int32_t* col_perm, const void* gvec, void* F,
                       void* stream);
+/* ab2_force_scatter plus the centroid per-atom virial (Fan et al., PRB 92, 094301 (2015)) in the same walk:
+ *   W[a][p][q] = - sum_{z : nbr[z] = a} vec[z][p] gvec[z][q]          W: [n_total][3][3], acc dtype
+ * vec[z] = pos[nbr[z]] - pos[ctr[z]] (+ shift) and gvec[z] = dE/dvec[z].  In Allegro vec[z] reaches only the energy of
+ * its centre, so gvec[z] = dE_ctr(z)/dvec[z] and W is exact.  W has 9 components and is NOT symmetric.
+ * Sign: sum_a W[a] = -vec^T gvec = -dE/d(strain) before symmetrisation, the sign LAMMPS uses for its virial (sym of the
+ * sum is the `virial` output of the Python layer).  Ghost rows (a >= N) carry the contributions their owners must
+ * receive, like ghost forces.  F is bitwise ab2_force_scatter's for the same gvec; W is reduced in a fixed order (no
+ * atomics, no zero-fill needed).  A pair style maps W[a] to LAMMPS' 9-component cvatom order
+ *   cvatom[a] = { W[a][0][0], W[a][1][1], W[a][2][2], W[a][0][1], W[a][0][2], W[a][1][2], W[a][1][0], W[a][2][0], W[a][2][1] }
+ * (xx, yy, zz, xy, xz, yz, yx, zx, zy).  vec may be null when E == 0. */
+int ab2_force_virial_scatter(int acc_dtype, int64_t N, int64_t n_total, int64_t E, const int32_t* row_ptr,
+                             const int32_t* col_ptr, const int32_t* col_perm, const void* vec, const void* gvec,
+                             void* F, void* W, void* stream);
 
 /* ---- upstream two-body scalar track + geometry (SURVEY section 8 row f1) ------------------ */
 
@@ -356,6 +369,15 @@ int ab2_frame_sum(int acc_dtype, int64_t n, int64_t n_frames, const int32_t* fra
                   int64_t scratch_elems, void* out, void* stream);
 int ab2_frame_virial(int acc_dtype, int64_t E, int64_t n_frames, const int32_t* frame_ptr, const int32_t* row_ptr,
                      const void* vec, const void* gvec, double* scratch, int64_t scratch_elems, void* W, void* stream);
+/* Potential part of the heat current of every frame, from per-atom energies and the centroid per-atom virial:
+ *   J[b][p] = sum_{a in frame b} ( e_atom[a] vel[a][p] + sum_q W[a][p][q] vel[a][q] )
+ * e_atom [n], vel [n][3], W [n][3][3] (ab2_force_virial_scatter), J [n_frames][3], all in the accumulate dtype; summed
+ * in fp64 and rounded once, with the chunking of the reductions above (a frame's J does not depend on the launch or on
+ * the other frames; an empty frame gives 0).  One frame: n_frames = 1, frame_ptr = {0, n}.  scratch: at least
+ * ab2_frame_scratch_elems(n, n_frames) * 3 elements.  The kinetic term sum_a m_a |v_a|^2 v_a / 2 needs masses and is
+ * the caller's. */
+int ab2_frame_heat_current(int acc_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* e_atom,
+                           const void* vel, const void* W, double* scratch, int64_t scratch_elems, void* J, void* stream);
 
 /* Radial embedding with per-type-pair matrices: out[z][c] = sum_n B_n(x_z) PQ[t_c * T + t_n][n][c], B_n as above
  * (num_bessels must be 8, S <= 128).  PQ: [T*T][8][S] in the accumulate dtype.  The product embedding above is
