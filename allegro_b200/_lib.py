@@ -679,14 +679,15 @@ def radial_bwd(dtype, S_rc: int, p_cut: float, vec, ctr, nbr, types, rmax_table,
                                      _ptr(_contig(g_e0, "g_e0")), _ptr(gvec), _stream()))
 
 
-def neighbor_csr(pos: torch.Tensor, r_max: float, box, pbc=(True, True, True), origin=None, n_centres: Optional[int] = None):
+def neighbor_csr(pos: torch.Tensor, r_max: float, box, ncell, pbc=(True, True, True), origin=None, n_centres: Optional[int] = None):
     """Cell-list neighbour search on the device -> (row_ptr [n_centres+1] int32, nbr [E] int32, shift_vec [E,3] pos dtype).
-    Orthorhombic ``box`` (3 lengths); centres are atoms [0, n_centres) (owned atoms first)."""
+    Orthorhombic ``box`` (3 lengths) cut into ``ncell`` (3 counts, from ``data.cell_grid``); centres are atoms
+    [0, n_centres) (owned atoms first)."""
     n = pos.shape[0]
     n_centres = n if n_centres is None else int(n_centres)
     box = [float(b) for b in box]
     origin = [0.0, 0.0, 0.0] if origin is None else [float(o) for o in origin]
-    ncell = [max(1, int(b // float(r_max))) for b in box]
+    ncell = [int(c) for c in ncell]
     g_box, g_org = (C.c_double * 3)(*box), (C.c_double * 3)(*origin)
     g_pbc, g_nc = (C.c_int32 * 3)(*[int(bool(p)) for p in pbc]), (C.c_int32 * 3)(*ncell)
     dt = DTYPE_ENUM[pos.dtype]

@@ -108,6 +108,9 @@ int nl_geom(NlGeom& g, const double* box, const double* origin, const int32_t* p
         if (pbc[a] && ncell[a] < 3) return 2;                 // a periodic axis would visit the same cell twice
         if (box[a] / ncell[a] < r_max * (1 - 1e-12)) return 3;  // cells must be at least r_max wide
     }
+    // cell ids and cell_start offsets are int32 (a far-flung atom on an open axis asks for billions of cells: the host
+    // coarsens such grids, data.cell_grid)
+    if ((int64_t)ncell[0] * ncell[1] * ncell[2] >= (int64_t)0x7fffffff) return 4;
     g.rmax2 = r_max * r_max;
     return 0;
 }
@@ -120,7 +123,7 @@ extern "C" int ab2_nl_bin(int pos_dtype, int64_t n, const void* pos, const doubl
     AB2_CHECK_ARG(pos && cell_id && box_host && origin_host && pbc_host && ncell_host, "null pointer");
     AB2_CHECK_ARG(pos_dtype == AB2_F64 || pos_dtype == AB2_F32, "positions must be fp64 or fp32");
     NlGeom g;
-    AB2_CHECK_ARG(nl_geom(g, box_host, origin_host, pbc_host, ncell_host, r_max) == 0, "box / cell grid (need cells >= r_max, >= 3 cells per periodic axis)");
+    AB2_CHECK_ARG(nl_geom(g, box_host, origin_host, pbc_host, ncell_host, r_max) == 0, "box / cell grid (need cells >= r_max, >= 3 cells per periodic axis, < 2^31 cells)");
     cudaStream_t st = (cudaStream_t)stream;
     if (pos_dtype == AB2_F64) nl_bin_kernel<double><<<ab2_blocks(n, 256), 256, 0, st>>>(g, n, (const double*)pos, cell_id);
     else nl_bin_kernel<float><<<ab2_blocks(n, 256), 256, 0, st>>>(g, n, (const float*)pos, cell_id);

@@ -97,15 +97,74 @@ def _brute_force(pos, cell, pbc, r_max):
     return torch.cat(ei, dim=1), torch.cat(sh, dim=0)
 
 
-def _cell_list(pos, box, r_max, pbc=(True, True, True), origin=None):
+# Narrowest cell the device search takes, as a fraction of r_max: the same bound as nl_geom in csrc/nlist.cu, so that a
+# box of exactly 3 r_max (rounded either way) is one grid on both sides
+CELL_WIDTH_TOL = 1 - 1e-12
+
+
+def _cells_along(length: float, r_max: float) -> int:
+    """Most cells of width >= r_max (to CELL_WIDTH_TOL) that fit in ``length``, at least 1.  Decided on the quotient the
+    device check computes (length / n in double): ``length // r_max`` alone can be one short, (3 r) // r == 2 for many r."""
+    w = r_max * CELL_WIDTH_TOL
+    n = max(1, int(length // r_max))
+    while length / (n + 1) >= w:
+        n += 1
+    while n > 1 and length / n < w:
+        n -= 1
+    return n
+
+
+def cell_grid(pos: torch.Tensor, r_max: float, box, pbc=(True, True, True)):
+    """Grid of the cell-list search (``neighbor_csr`` and ``neighbor_list(method="cell")``) for an orthorhombic box of
+    lengths ``box`` -> (box [3], origin [3], ncell [3]) as Python numbers, or None when a periodic axis is shorter
+    than 3 r_max.
+
+    * Periodic axes span [0, L) with the most cells of width >= r_max; at least 3, so the 27-cell walk never visits a
+      cell twice.
+    * Open axes span the occupied extent [lo, hi], widened to r_max when thinner (a sheet, a wire, a molecule, one
+      atom): one cell of width >= r_max is a valid grid.
+    * The cell count stays at most max(27, 4 N): an atom far out on an open axis would otherwise ask for billions of
+      mostly empty cells (and overflow the int32 cell id).  Open axes are coarsened first, periodic axes never below 3
+      cells; wider cells are always correct, only slower.
+    Every grid returned has cells >= r_max wide (to CELL_WIDTH_TOL) and passes the device check (``nl_geom`` in
+    csrc/nlist.cu)."""
+    r = float(r_max)
+    pbc = [bool(p) for p in pbc]
+    box = [float(b) for b in box]
+    origin = [0.0, 0.0, 0.0]
+    n = int(pos.shape[0])
+    open_axes = [a for a in range(3) if not pbc[a]]
+    if open_axes:
+        lo, hi = (pos.amin(0).tolist(), pos.amax(0).tolist()) if n > 0 else ([0.0] * 3, [0.0] * 3)
+        for a in open_axes:
+            origin[a] = float(lo[a])
+            box[a] = max((float(hi[a]) - float(lo[a])) * (1 + 1e-9) + 1e-6, r)
+    if any(p and not box[a] > 0 for a, p in enumerate(pbc)):
+        return None
+    ncell = [_cells_along(b, r) for b in box]
+    if any(p and ncell[a] < 3 for a, p in enumerate(pbc)):
+        return None
+    limit = max(27, 4 * n)
+    while ncell[0] * ncell[1] * ncell[2] > limit:
+        cand = [a for a in open_axes if ncell[a] > 1] or [a for a in range(3) if pbc[a] and ncell[a] > 3]
+        a = max(cand, key=lambda x: ncell[x])
+        ncell[a] = max(3 if pbc[a] else 1, ncell[a] // 2)
+    return box, origin, ncell
+
+
+def _cell_list(pos, box, r_max, pbc=(True, True, True), origin=None, ncell=None):
     """Orthorhombic box, per-axis periodicity.  Periodic axes need >= 3 cells; on a
-    non-periodic axis the grid spans [origin, origin+box) and nothing wraps."""
+    non-periodic axis the grid spans [origin, origin+box) and nothing wraps.  ``ncell``: the grid of ``cell_grid``
+    (default: cells of edge >= r_max)."""
     dev = pos.device
     n = pos.shape[0]
     pbc_t = torch.tensor([bool(p) for p in pbc], device=dev)
     if origin is None:
         origin = torch.zeros(3, dtype=pos.dtype, device=dev)
-    ncell = torch.floor(box / r_max).to(torch.long).clamp(min=1)
+    if ncell is None:
+        ncell = torch.floor(box / r_max).to(torch.long).clamp(min=1)
+    else:
+        ncell = torch.tensor([int(c) for c in ncell], dtype=torch.long, device=dev)
     assert int(ncell[pbc_t].min() if bool(pbc_t.any()) else 3) >= 3, "cell list needs box >= 3 r_max on every periodic axis"
     rel = pos - origin
     img0 = torch.where(pbc_t, torch.floor(rel / box), torch.zeros_like(rel)).to(torch.long)  # image index of the raw position
@@ -145,6 +204,8 @@ def _cell_list(pos, box, r_max, pbc=(True, True, True), origin=None):
                 s = img_rep[keep] - img0[j_k] + img0[i_k]
                 ei.append(torch.stack([i_k, j_k]))
                 sh.append(s)
+    if not ei:
+        return torch.zeros(2, 0, dtype=torch.long, device=dev), torch.zeros(0, 3, dtype=torch.long, device=dev)
     return torch.cat(ei, dim=1), torch.cat(sh, dim=0)
 
 
@@ -159,21 +220,18 @@ def neighbor_list(
     Returns edge_index [2,E] int64 (row 0 = centre) and edge_cell_shift [E,3] (pos dtype)."""
     pbc = tuple(bool(p) for p in (pbc if not isinstance(pbc, bool) else (pbc,) * 3))
     ortho = cell is not None and bool((cell.view(3, 3) - torch.diag(torch.diagonal(cell.view(3, 3)))).abs().max() == 0)
+    grid = None
+    if ortho and (method == "cell" or (method == "auto" and pos.shape[0] > 3000)):
+        grid = cell_grid(pos, r_max, torch.diagonal(cell.view(3, 3)).tolist(), pbc)
     if method == "auto":
-        big = pos.shape[0] > 3000
-        can = cell is not None and ortho and all(
-            (not p) or float(cell.view(3, 3)[a, a]) >= 3 * r_max for a, p in enumerate(pbc)
-        )
-        method = "cell" if (big and can) else "brute"
+        method = "cell" if grid is not None else "brute"
     if method == "cell":
-        box = torch.diagonal(cell.view(3, 3)).to(pos.dtype).clone()
-        origin = torch.zeros(3, dtype=pos.dtype, device=pos.device)
-        for a, p in enumerate(pbc):
-            if not p:  # non-periodic axis: grid over the occupied extent
-                lo, hi = pos[:, a].min(), pos[:, a].max()
-                origin[a] = lo
-                box[a] = (hi - lo) * (1 + 1e-9) + 1e-6
-        ei, sh = _cell_list(pos, box, float(r_max), pbc, origin)
+        if grid is None:
+            raise ValueError("the cell list needs an orthorhombic box with >= 3 r_max on every periodic axis")
+        box_l, origin_l, ncell = grid  # open axes: grid over the occupied extent
+        box = torch.tensor(box_l, dtype=pos.dtype, device=pos.device)
+        origin = torch.tensor(origin_l, dtype=pos.dtype, device=pos.device)
+        ei, sh = _cell_list(pos, box, float(r_max), pbc, origin, ncell)
     else:
         ei, sh = _brute_force(pos, cell, pbc, float(r_max))
     n = pos.shape[0]
@@ -268,14 +326,19 @@ def to_ghost_format(data: Type) -> Type:
 
 
 def csr_supported(pos: torch.Tensor, r_max: float, cell: Optional[torch.Tensor], pbc=(True, True, True)) -> bool:
-    """Can ``neighbor_csr`` (CUDA cell list) take this frame?  CUDA positions, orthorhombic box, >= 3 cells of
-    edge r_max on every periodic axis."""
+    """Can ``neighbor_csr`` (CUDA cell list) take this frame?  CUDA positions and an orthorhombic box with >= 3 cells of
+    edge r_max on every periodic axis (``cell_grid`` decides, with the device's tolerance).  Open axes take any extent:
+    a sheet, a wire or a molecule thinner than r_max gets one cell on that axis, and far-flung atoms coarsen the grid."""
+    return _csr_grid(pos, r_max, cell, pbc) is not None
+
+
+def _csr_grid(pos, r_max, cell, pbc):
     if not pos.is_cuda or cell is None:
-        return False
+        return None
     c = cell.view(3, 3)
     if bool((c - torch.diag(torch.diagonal(c))).abs().max() != 0):
-        return False
-    return all((not p) or float(c[a, a]) >= 3 * r_max for a, p in enumerate(pbc))
+        return None
+    return cell_grid(pos, r_max, torch.diagonal(c).tolist(), pbc)
 
 
 def neighbor_csr(pos: torch.Tensor, r_max: float, cell: torch.Tensor, pbc=(True, True, True), n_centres: Optional[int] = None):
@@ -284,18 +347,13 @@ def neighbor_csr(pos: torch.Tensor, r_max: float, cell: torch.Tensor, pbc=(True,
     from . import _lib
 
     pbc = tuple(bool(p) for p in (pbc if not isinstance(pbc, bool) else (pbc,) * 3))
-    if not csr_supported(pos, r_max, cell, pbc):
+    grid = _csr_grid(pos, r_max, cell, pbc)
+    if grid is None:
         raise ValueError("neighbor_csr needs CUDA positions and an orthorhombic box with >= 3 r_max per periodic axis")
-    box = [float(v) for v in torch.diagonal(cell.view(3, 3))]
-    origin = [0.0, 0.0, 0.0]
-    for a, p in enumerate(pbc):
-        if not p:  # open axis: grid over the occupied extent
-            lo, hi = float(pos[:, a].min()), float(pos[:, a].max())
-            origin[a] = lo
-            box[a] = (hi - lo) * (1 + 1e-9) + 1e-6
+    box, origin, ncell = grid
     n = pos.shape[0]
     nc = n if n_centres is None else int(n_centres)
-    row_ptr, nbr, shift = _lib.neighbor_csr(pos, r_max, box, pbc, origin, nc)
+    row_ptr, nbr, shift = _lib.neighbor_csr(pos, r_max, box, ncell, pbc, origin, nc)
     counts = (row_ptr[1:] - row_ptr[:-1])
     ctr = torch.repeat_interleave(torch.arange(nc, device=pos.device, dtype=torch.int32), counts.long())
     maxdeg = int(counts.max()) if nc > 0 else 0

@@ -318,8 +318,9 @@ int ab2_radial_bwd(int dtype, int64_t E, int S_rc, int num_bessels, double p_cut
 /* Cell-list search on an orthorhombic box with per-axis periodicity.  The reference receives edge_index [2,E] int64
  * from nequip's data pipeline / LAMMPS (allegro/nn/_allegro.py:238, allegro/_compile.py:41-61); these three kernels
  * produce the centre-sorted CSR (row_ptr / nbr int32) and the per-edge shift VECTORS the path consumes, without the
- * int64 COO list.  Host-side geometry: box[3], origin[3] (doubles), pbc[3], ncell[3] with box/ncell >= r_max and
- * >= 3 cells on every periodic axis.  pos: [n][3] fp64 or fp32, raw (unwrapped) coordinates;
+ * int64 COO list.  Host-side geometry: box[3], origin[3] (doubles), pbc[3], ncell[3] with box/ncell >= r_max,
+ * >= 3 cells on every periodic axis and fewer than 2^31 - 1 cells in all.  An open axis spans [origin, origin + box):
+ * every position must lie inside it; one cell wider than r_max is valid for a layer thinner than the cutoff.  pos: [n][3] fp64 or fp32, raw (unwrapped) coordinates;
  *   r = pos[nbr] + shift - pos[centre]  holds for the raw positions.
  * Call order: ab2_nl_bin -> (host: order = stable argsort(cell_id), cell_start = prefix sum of the cell histogram)
  *             -> ab2_nl_count -> (host: row_ptr = prefix sum) -> ab2_nl_fill.
