@@ -79,6 +79,9 @@ _SIGNATURES = {
     "ab2_nl_bin": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_nl_count": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_nl_fill": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_nl_lattice_bin": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
+    "ab2_nl_lattice_count": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_nl_lattice_fill": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_radial_bwd": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_nl_frames_count": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_nl_frames_fill": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp], C.c_int),
@@ -683,34 +686,50 @@ def neighbor_csr(pos: torch.Tensor, r_max: float, box, ncell, pbc=(True, True, T
     """Cell-list neighbour search on the device -> (row_ptr [n_centres+1] int32, nbr [E] int32, shift_vec [E,3] pos dtype).
     Orthorhombic ``box`` (3 lengths) cut into ``ncell`` (3 counts, from ``data.cell_grid``); centres are atoms
     [0, n_centres) (owned atoms first)."""
-    n = pos.shape[0]
-    n_centres = n if n_centres is None else int(n_centres)
     box = [float(b) for b in box]
     origin = [0.0, 0.0, 0.0] if origin is None else [float(o) for o in origin]
     ncell = [int(c) for c in ncell]
-    g_box, g_org = (C.c_double * 3)(*box), (C.c_double * 3)(*origin)
-    g_pbc, g_nc = (C.c_int32 * 3)(*[int(bool(p)) for p in pbc]), (C.c_int32 * 3)(*ncell)
+    geom = ((C.c_double * 3)(*box), (C.c_double * 3)(*origin), (C.c_int32 * 3)(*[int(bool(p)) for p in pbc]), (C.c_int32 * 3)(*ncell),
+            float(r_max))
+    lib = load()
+    return _cell_list_csr(pos, n_centres, ncell, geom, "nl", lib.ab2_nl_bin, lib.ab2_nl_count, lib.ab2_nl_fill)
+
+
+def neighbor_csr_lattice(pos: torch.Tensor, r_max: float, rows, origin, ncell, reach, pbc=(True, True, True), n_centres: Optional[int] = None):
+    """The same search on a general lattice (ab2_nl_lattice_bin / count / fill): ``rows`` the 3x3 binning rows, ``origin``
+    fractional, ``ncell`` bins and ``reach`` bins walked either side per axis, all from ``data.lattice_grid``."""
+    flat = [float(v) for row in rows for v in row]
+    ncell = [int(c) for c in ncell]
+    geom = ((C.c_double * 9)(*flat), (C.c_double * 3)(*[float(o) for o in origin]), (C.c_int32 * 3)(*[int(bool(p)) for p in pbc]),
+            (C.c_int32 * 3)(*ncell), (C.c_int32 * 3)(*[int(k) for k in reach]), float(r_max))
+    lib = load()
+    return _cell_list_csr(pos, n_centres, ncell, geom, "nl_lattice", lib.ab2_nl_lattice_bin, lib.ab2_nl_lattice_count, lib.ab2_nl_lattice_fill)
+
+
+def _cell_list_csr(pos, n_centres, ncell, geom, name, bin_fn, count_fn, fill_fn):
+    """bin -> sort by bin -> count -> prefix sum -> fill; ``geom`` the host-side geometry arguments of the three calls."""
+    n = pos.shape[0]
+    n_centres = n if n_centres is None else int(n_centres)
     dt = DTYPE_ENUM[pos.dtype]
     pos = _contig(pos, "pos")
     cell_id = torch.empty(n, dtype=torch.int32, device=pos.device)
-    with _timed("nl_bin"):
-        _check(load().ab2_nl_bin(dt, n, _ptr(pos), g_box, g_org, g_pbc, g_nc, float(r_max), _ptr(cell_id), _stream()))
+    with _timed(name + "_bin"):
+        _check(bin_fn(dt, n, _ptr(pos), *geom, _ptr(cell_id), _stream()))
     order = torch.argsort(cell_id, stable=True).to(torch.int32)
     ncells = ncell[0] * ncell[1] * ncell[2]
     cell_start = torch.zeros(ncells + 1, dtype=torch.int32, device=pos.device)
     cell_start[1:] = torch.cumsum(torch.bincount(cell_id.long(), minlength=ncells), 0).to(torch.int32)
     counts = torch.empty(n_centres, dtype=torch.int32, device=pos.device)
-    with _timed("nl_count"):
-        _check(load().ab2_nl_count(dt, n_centres, _ptr(pos), g_box, g_org, g_pbc, g_nc, float(r_max), _ptr(cell_start), _ptr(order), _ptr(counts), _stream()))
+    with _timed(name + "_count"):
+        _check(count_fn(dt, n_centres, _ptr(pos), *geom, _ptr(cell_start), _ptr(order), _ptr(counts), _stream()))
     row_ptr = torch.zeros(n_centres + 1, dtype=torch.int32, device=pos.device)
     row_ptr[1:] = torch.cumsum(counts, 0).to(torch.int32)
     E = int(row_ptr[-1])
     nbr = torch.empty(E, dtype=torch.int32, device=pos.device)
     shift = torch.empty(E, 3, dtype=pos.dtype, device=pos.device)
     if E:
-        with _timed("nl_fill"):
-            _check(load().ab2_nl_fill(dt, n_centres, _ptr(pos), g_box, g_org, g_pbc, g_nc, float(r_max), _ptr(cell_start), _ptr(order), _ptr(row_ptr),
-                                      _ptr(nbr), _ptr(shift), _stream()))
+        with _timed(name + "_fill"):
+            _check(fill_fn(dt, n_centres, _ptr(pos), *geom, _ptr(cell_start), _ptr(order), _ptr(row_ptr), _ptr(nbr), _ptr(shift), _stream()))
     return row_ptr, nbr, shift
 
 

@@ -68,13 +68,17 @@ class AllegroCalculator:
             if self._data is None:
                 raise ValueError("atom_types are needed for the first evaluation")
             atom_types = self._data[D.ATOM_TYPE_KEY]
+        if self.compute_stress and cell is not None:
+            if not D.is_regular_cell(cell):
+                raise ValueError("compute_stress=True needs a non-singular cell: stress is the virial over the cell volume")
         data = {D.POSITIONS_KEY: pos.clone(), D.ATOM_TYPE_KEY: atom_types.reshape(-1).clone()}
         inner = getattr(self.model, "model", self.model)
         if hasattr(inner, "energy_and_forces") and D.csr_supported(pos, self.r_max + self.skin, cell, self.pbc):
-            # CUDA cell list straight into the kernels' CSR (no int64 COO list, no sort by centre)
+            # CUDA cell list straight into the kernels' CSR (no int64 COO list, no sort by centre); any cell, or none
             csr, shift_vec = D.neighbor_csr(pos, self.r_max + self.skin, cell, self.pbc)
             data[D.CSR_KEY], data[D.EDGE_SHIFT_VEC_KEY] = csr, shift_vec
-            data[D.CELL_KEY] = cell.view(3, 3).clone()
+            if cell is not None:
+                data[D.CELL_KEY] = cell.view(3, 3).clone()
             self._n_edges = csr.num_edges
         else:
             ei, shift = D.neighbor_list(pos, self.r_max + self.skin, cell, self.pbc)
@@ -100,7 +104,9 @@ class AllegroCalculator:
     # ---- evaluation ----------------------------------------------------------------------------
     def compute(self, pos: torch.Tensor, cell: Optional[torch.Tensor] = None, atom_types: Optional[torch.Tensor] = None,
                 velocities: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
-        """-> {"energy" [1,1], "forces" [N,3], "atomic_energy" [N,1]} (+ "stress", "virial" [1,3,3] if asked for;
+        """-> {"energy" [1,1], "forces" [N,3], "atomic_energy" [N,1]} (+ "stress", "virial" [1,3,3] if asked for and a cell
+        is given: with ``cell=None`` no stress is returned, a singular cell (``data.is_regular_cell``) raises ValueError, and
+        any other cell, however thin an open axis, divides the virial by its own volume;
         "atomic_virial" [N,3,3] with compute_atomic_virial; "heat_current" [1,3] with compute_heat_current, which needs
         ``velocities`` [N,3]).  The returned tensors are the model's output buffers: with graph replay they are
         overwritten by the next call."""

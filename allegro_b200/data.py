@@ -325,35 +325,189 @@ def to_ghost_format(data: Type) -> Type:
     return data
 
 
+def _lattice_metrics(h):
+    """-> (det, heights [3], regular) of the rows ``h``, with the operations of nl_lattice_geom (csrc/nlist.cu) in the same
+    order, so that the host and the device agree on every quotient: H_a = |det| / |h_p x h_q|; regular = finite and
+    |det| > 1e-12 |h_0| |h_1| |h_2| (rows not within 1e-12 rad of a common plane)."""
+    cr, norm = [], []
+    for a in range(3):
+        p, q = h[(a + 1) % 3], h[(a + 2) % 3]
+        cr.append((p[1] * q[2] - p[2] * q[1], p[2] * q[0] - p[0] * q[2], p[0] * q[1] - p[1] * q[0]))
+        norm.append(math.sqrt(h[a][0] * h[a][0] + h[a][1] * h[a][1] + h[a][2] * h[a][2]))
+    det = h[0][0] * cr[0][0] + h[0][1] * cr[0][1] + h[0][2] * cr[0][2]
+    regular = math.isfinite(det) and abs(det) > 1e-12 * norm[0] * norm[1] * norm[2]
+    if not regular:
+        return det, None, False
+    heights = [abs(det) / math.sqrt(c[0] * c[0] + c[1] * c[1] + c[2] * c[2]) for c in cr]
+    return det, heights, True
+
+
+def is_regular_cell(cell: torch.Tensor) -> bool:
+    """Finite rows not within 1e-12 rad of a common plane: the test the lattice search (nl_lattice_geom) and the
+    calculator's stress apply."""
+    return _lattice_metrics(cell.detach().reshape(3, 3).to(device="cpu", dtype=torch.float64).tolist())[2]
+
+
+def _unit(v):
+    n = math.sqrt(sum(x * x for x in v))
+    return [x / n for x in v] if n > 0 and math.isfinite(n) else None
+
+
+def _cross(p, q):
+    return [p[1] * q[2] - p[2] * q[1], p[2] * q[0] - p[0] * q[2], p[0] * q[1] - p[1] * q[0]]
+
+
+def _complete_open_rows(h, pbc):
+    """Rows with every open axis replaced: the unit normal of the two periodic rows (one open axis), an orthonormal
+    completion of the one periodic row (two), the identity (three).  None when the periodic rows are degenerate."""
+    per = [a for a in range(3) if pbc[a]]
+    opn = [a for a in range(3) if not pbc[a]]
+    h = [list(r) for r in h]
+    if len(per) == 2:
+        u = _unit(_cross(h[per[0]], h[per[1]]))
+        if u is None:
+            return None
+        h[opn[0]] = u
+    elif len(per) == 1:
+        v = _unit(h[per[0]])
+        if v is None:
+            return None
+        e = [0.0, 0.0, 0.0]
+        e[min(range(3), key=lambda x: abs(v[x]))] = 1.0  # the axis least aligned with v
+        d = sum(e[x] * v[x] for x in range(3))
+        u1 = _unit([e[x] - d * v[x] for x in range(3)])
+        h[opn[0]], h[opn[1]] = u1, _cross(v, u1)
+    elif len(per) == 0:
+        h = [[1.0, 0.0, 0.0], [0.0, 1.0, 0.0], [0.0, 0.0, 1.0]]
+    return h
+
+
+def _reach_along(height: float, n: int, r_max: float) -> int:
+    """Fewest bins k with (height / n) * k >= r_max (to CELL_WIDTH_TOL), on the quotient nl_lattice_geom computes."""
+    w = r_max * CELL_WIDTH_TOL
+    k = max(1, math.ceil(w / (height / n)))
+    while height / n * k < w:
+        k += 1
+    while k > 1 and height / n * (k - 1) >= w:
+        k -= 1
+    return k
+
+
+def lattice_grid(pos: torch.Tensor, r_max: float, cell: Optional[torch.Tensor], pbc=(True, True, True)):
+    """Grid of the general-lattice cell list (``neighbor_csr`` for the frames ``cell_grid`` does not take) -> (rows [3][3],
+    origin [3], ncell [3], reach [3]) as Python numbers, or None.
+
+    * Atoms are binned in fractional coordinates f = pos . rows^-1 - origin; bins are parallelepipeds of thickness
+      t_a = H_a / ncell_a (H_a the height of the rows along a) and a centre walks reach_a = ceil(r_max / t_a) bins
+      either side (to CELL_WIDTH_TOL).  Periodic axes keep the cell's rows and take the most bins with t_a >= r_max:
+      one bin and reach > 1 when the cell is thinner than r_max.
+    * Open-axis rows that are zero (ASE's 2-D and 1-D cells), or that leave the cell singular, and all rows of a frame
+      with ``cell=None`` and no periodic axis, are replaced: by the unit normal of the periodic rows (one open axis) or an
+      orthonormal completion (more).  Shifts along open axes are 0, so a replaced row never reaches an output.
+    * An open axis spans the occupied fractional extent, widened to r_max: its row is scaled so that the atoms lie in
+      [0, 1) from ``origin``.
+    * The bin count stays at most max(27, 4 N): open axes are coarsened first, then periodic ones, down to 1 bin.
+    None when a periodic axis has no cell (``cell=None``), the periodic rows are singular or not finite, or the walk
+    would visit 2^31 - 1 or more bins per centre.  Every grid returned passes the device check (nl_lattice_geom)."""
+    r = float(r_max)
+    pbc = [bool(p) for p in pbc]
+    n = int(pos.shape[0])
+    if cell is None:
+        if any(pbc):
+            return None
+        h = [[0.0] * 3 for _ in range(3)]
+    else:
+        h = cell.detach().reshape(3, 3).to(device="cpu", dtype=torch.float64).tolist()
+    open_axes = [a for a in range(3) if not pbc[a]]
+    if not all(math.isfinite(v) for a in range(3) if pbc[a] for v in h[a]):
+        return None
+    if open_axes and (any(not any(h[a]) for a in open_axes) or not all(math.isfinite(v) for row in h for v in row)
+                      or not _lattice_metrics(h)[2]):
+        h = _complete_open_rows(h, pbc)
+        if h is None:
+            return None
+    det, heights, regular = _lattice_metrics(h)
+    if not regular:
+        return None
+    origin = [0.0, 0.0, 0.0]
+    if open_axes:
+        # fractional extent of the atoms along the open axes (hinv column a = (h_p x h_q) / det)
+        cols = [_cross(h[(a + 1) % 3], h[(a + 2) % 3]) for a in open_axes]
+        hinv = torch.tensor(cols, dtype=torch.float64, device=pos.device).T / det
+        if n > 0:
+            f = pos.detach().to(torch.float64) @ hinv
+            lo, hi = f.amin(0).tolist(), f.amax(0).tolist()
+        else:
+            lo, hi = [0.0] * len(open_axes), [0.0] * len(open_axes)
+        for k, a in enumerate(open_axes):
+            # in length units across the axis; half the margin goes below the lowest atom
+            span = max((hi[k] - lo[k]) * heights[a] * (1 + 1e-9) + 1e-6, r)
+            s = span / heights[a]
+            h[a] = [v * s for v in h[a]]
+            origin[a] = (lo[k] - 0.5e-9 * (hi[k] - lo[k]) - 0.5e-6 / heights[a]) / s
+        det, heights, regular = _lattice_metrics(h)
+        if not regular:
+            return None
+    ncell = [_cells_along(heights[a], r) for a in range(3)]
+    limit = max(27, 4 * n)
+    while ncell[0] * ncell[1] * ncell[2] > limit:
+        cand = [a for a in open_axes if ncell[a] > 1] or [a for a in range(3) if ncell[a] > 1]
+        a = max(cand, key=lambda x: ncell[x])
+        ncell[a] = max(1, ncell[a] // 2)
+    reach = [_reach_along(heights[a], ncell[a], r) for a in range(3)]
+    if math.prod(2 * k + 1 for k in reach) >= 2**31 - 1 or math.prod(ncell) >= 2**31 - 1:
+        return None
+    return h, origin, ncell, reach
+
+
 def csr_supported(pos: torch.Tensor, r_max: float, cell: Optional[torch.Tensor], pbc=(True, True, True)) -> bool:
-    """Can ``neighbor_csr`` (CUDA cell list) take this frame?  CUDA positions and an orthorhombic box with >= 3 cells of
-    edge r_max on every periodic axis (``cell_grid`` decides, with the device's tolerance).  Open axes take any extent:
-    a sheet, a wire or a molecule thinner than r_max gets one cell on that axis, and far-flung atoms coarsen the grid."""
+    """Can ``neighbor_csr`` (CUDA cell list) take this frame?  CUDA positions and any cell ``lattice_grid`` accepts:
+    orthorhombic or triclinic, periodic axes of any height, open axes of any extent (zero rows included), or no cell
+    at all when no axis is periodic.  Frames ``cell_grid`` accepts (an orthorhombic box with >= 3 r_max on every
+    periodic axis) take the orthorhombic grid, every other frame the general-lattice one."""
     return _csr_grid(pos, r_max, cell, pbc) is not None
 
 
+def search_grid(pos, r_max, cell, pbc):
+    """The grid ``neighbor_csr`` searches this frame on (for positions on any device) -> ("ortho", ``cell_grid``),
+    ("lattice", ``lattice_grid``) or None."""
+    if cell is not None:
+        c = cell.view(3, 3)
+        if bool((c - torch.diag(torch.diagonal(c))).abs().max() == 0):
+            grid = cell_grid(pos, r_max, torch.diagonal(c).tolist(), pbc)
+            if grid is not None:
+                return "ortho", grid
+    grid = lattice_grid(pos, r_max, cell, pbc)
+    return None if grid is None else ("lattice", grid)
+
+
 def _csr_grid(pos, r_max, cell, pbc):
-    if not pos.is_cuda or cell is None:
+    if not pos.is_cuda:
         return None
-    c = cell.view(3, 3)
-    if bool((c - torch.diag(torch.diagonal(c))).abs().max() != 0):
-        return None
-    return cell_grid(pos, r_max, torch.diagonal(c).tolist(), pbc)
+    return search_grid(pos, r_max, cell, pbc)
 
 
-def neighbor_csr(pos: torch.Tensor, r_max: float, cell: torch.Tensor, pbc=(True, True, True), n_centres: Optional[int] = None):
-    """Neighbour search on the device straight into the kernels' format (ab2_nl_bin / count / fill, SURVEY 8 row f2).
-    -> (EdgeCSR, shift_vec [E,3] in the positions' dtype).  Centres are atoms [0, n_centres) (owned atoms first)."""
+def neighbor_csr(pos: torch.Tensor, r_max: float, cell: Optional[torch.Tensor], pbc=(True, True, True), n_centres: Optional[int] = None):
+    """Neighbour search on the device straight into the kernels' format -> (EdgeCSR, shift_vec [E,3] in the positions'
+    dtype).  Centres are atoms [0, n_centres) (owned atoms first).  An orthorhombic box with >= 3 r_max per periodic
+    axis takes ab2_nl_bin / count / fill (SURVEY 8 row f2); any other cell, and ``cell=None`` for a frame without
+    periodic axes, takes ab2_nl_lattice_bin / count / fill.  r = pos[nbr] + shift - pos[ctr] holds for the raw positions."""
     from . import _lib
 
     pbc = tuple(bool(p) for p in (pbc if not isinstance(pbc, bool) else (pbc,) * 3))
-    grid = _csr_grid(pos, r_max, cell, pbc)
-    if grid is None:
-        raise ValueError("neighbor_csr needs CUDA positions and an orthorhombic box with >= 3 r_max per periodic axis")
-    box, origin, ncell = grid
+    route = _csr_grid(pos, r_max, cell, pbc)
+    if route is None:
+        raise ValueError("neighbor_csr needs CUDA positions and a finite non-singular cell on the periodic axes (or cell=None "
+                         "with no periodic axis)")
+    kind, grid = route
     n = pos.shape[0]
     nc = n if n_centres is None else int(n_centres)
-    row_ptr, nbr, shift = _lib.neighbor_csr(pos, r_max, box, ncell, pbc, origin, nc)
+    if kind == "ortho":
+        box, origin, ncell = grid
+        row_ptr, nbr, shift = _lib.neighbor_csr(pos, r_max, box, ncell, pbc, origin, nc)
+    else:
+        rows, origin, ncell, reach = grid
+        row_ptr, nbr, shift = _lib.neighbor_csr_lattice(pos, r_max, rows, origin, ncell, reach, pbc, nc)
     counts = (row_ptr[1:] - row_ptr[:-1])
     ctr = torch.repeat_interleave(torch.arange(nc, device=pos.device, dtype=torch.int32), counts.long())
     maxdeg = int(counts.max()) if nc > 0 else 0

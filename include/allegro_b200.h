@@ -335,6 +335,31 @@ int ab2_nl_fill(int pos_dtype, int64_t n_centres, const void* pos, const double*
                 const int32_t* cell_start, const int32_t* order, const int32_t* row_ptr, int32_t* nbr,
                 void* shift, void* stream);
 
+/* The same search on a general lattice: triclinic or left-handed cells, periodic axes of any height (also below r_max),
+ * open axes whose cell rows are replaced for binning.  Host-side geometry: rows[9] (row-major 3x3 binning rows a, b,
+ * c, doubles; the inverse is computed inside), origin[3] (fractional, in units of the rows), pbc[3], ncell[3] bins per
+ * axis and reach[3] bins walked either side of a centre's bin.  Atoms are binned by f = pos . rows^-1 - origin; on a
+ * periodic axis img0 = floor(f) and the wrapped position is pos - img0 . rows; on an open axis every f must lie in
+ * [0, 1).  With H_a = |det| / |row_p x row_q| the height of the cell along a and t_a = H_a / ncell[a] the bin thickness,
+ * every axis needs t_a * reach[a] >= r_max (to 1 - 1e-12); the rows must be finite and non-singular, and there must be
+ * fewer than 2^31 - 1 bins in all and fewer than 2^31 - 1 bins visited per centre.  Each call checks all of this
+ * before it launches anything.  Wrap, bin and distance test run in fp64 for fp32 positions too; a row's shift
+ * (im - img0[nbr] + img0[centre]) . rows is rounded once to the positions' dtype and is exactly 0 along axes with
+ * pbc = 0, so  r = pos[nbr] + shift - pos[centre]  holds for the raw positions.  Rows come out in bin-walk order, fixed
+ * for a given frame.  Call order, host steps and centres as for ab2_nl_*: ab2_nl_lattice_bin -> (order, cell_start)
+ * -> ab2_nl_lattice_count -> (row_ptr) -> ab2_nl_lattice_fill. */
+int ab2_nl_lattice_bin(int pos_dtype, int64_t n, const void* pos, const double* rows_host, const double* origin_host,
+                       const int32_t* pbc_host, const int32_t* ncell_host, const int32_t* reach_host, double r_max,
+                       int32_t* cell_id, void* stream);
+int ab2_nl_lattice_count(int pos_dtype, int64_t n_centres, const void* pos, const double* rows_host,
+                         const double* origin_host, const int32_t* pbc_host, const int32_t* ncell_host,
+                         const int32_t* reach_host, double r_max, const int32_t* cell_start, const int32_t* order,
+                         int32_t* counts, void* stream);
+int ab2_nl_lattice_fill(int pos_dtype, int64_t n_centres, const void* pos, const double* rows_host,
+                        const double* origin_host, const int32_t* pbc_host, const int32_t* ncell_host,
+                        const int32_t* reach_host, double r_max, const int32_t* cell_start, const int32_t* order,
+                        const int32_t* row_ptr, int32_t* nbr, void* shift, void* stream);
+
 /* ---- batches of frames: many small frames concatenated into one graph ------------------------ */
 
 /* All-pairs search for a batch of frames (nequip's batched data: `batch`, `num_atoms`, one cell per frame), for any
