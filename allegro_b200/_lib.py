@@ -83,8 +83,8 @@ _SIGNATURES = {
     "ab2_nl_lattice_count": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_nl_lattice_fill": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_radial_bwd": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
-    "ab2_nl_frames_count": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
-    "ab2_nl_frames_fill": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_nl_frames_count": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
+    "ab2_nl_frames_fill": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_frame_scratch_elems": ([_i64, _i64], C.c_int64),
     "ab2_frame_sum": ([_i32, _i64, _i64, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_frame_virial": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
@@ -759,12 +759,19 @@ def radial_pq_bwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table,
 def nl_frames(pos: torch.Tensor, frame_ptr: torch.Tensor, cell: torch.Tensor, inv_cell: torch.Tensor, pbc: torch.Tensor, r_max: float):
     """All-pairs search per frame (ab2_nl_frames_count / fill) -> (row_ptr [n+1] int32, nbr [E] int32, shift_vec [E,3] pos
     dtype).  frame_ptr [B+1] int32, cell / inv_cell [B,3,3] in the positions' dtype, pbc [B,3] int32, all on the device.
-    Rows are ordered by neighbour, then by image (x, y, z) lexicographically."""
+    Rows are ordered by neighbour, then by image (x, y, z) lexicographically.  The images searched on each side of every
+    periodic axis (the kernels' nimg [B,3]) are computed here, on the host, from the cell as given
+    (``data.frames_geometry``), so no frame reaches the kernels with an unbounded image range: a periodic frame whose cell
+    is not regular, or that needs more than data.FRAMES_MAX_IMAGES images per pair, raises ValueError before any launch."""
+    from . import data as D
+
     n, B = pos.shape[0], frame_ptr.shape[0] - 1
     dt = DTYPE_ENUM[pos.dtype]
+    _, nimg = D.frames_geometry(cell.reshape(B, 3, 3), pbc.reshape(B, 3) != 0, r_max, pos.dtype)
+    nimg = nimg.to(device=pos.device, dtype=torch.int32)
     pos = _contig(pos, "pos")
     args = (_ptr(_contig(frame_ptr, "frame_ptr")), _ptr(pos), _ptr(_contig(cell, "cell")), _ptr(_contig(inv_cell, "inv_cell")),
-            _ptr(_contig(pbc, "pbc")), float(r_max))
+            _ptr(_contig(pbc, "pbc")), _ptr(nimg), float(r_max))
     counts = torch.empty(n, dtype=torch.int32, device=pos.device)
     with _timed("nl_frames_count"):
         _check(load().ab2_nl_frames_count(dt, n, B, *args, _ptr(counts), _stream()))

@@ -10,10 +10,12 @@
 // So a row is ordered by neighbour index, then by image (x, y, z) lexicographically: the order of
 // data.neighbor_list(..., method="brute").
 //
-// Geometry per frame, all on the device: cell[b] (rows = lattice vectors), its inverse, pbc[b][3].  Positions are wrapped
-// into the cell along the periodic axes in fractional coordinates (frac = pos @ inv, image = floor(frac)), and the raw
-// image offsets are folded back into the shift, so  r = pos[nbr] + shift - pos[ctr]  holds for the RAW positions.  An
-// axis a needs n_a = ceil(r_max / h_a) images on each side, h_a = |det cell| / |b x c| the cell height along that axis.
+// Geometry per frame, all on the device: cell[b] (rows = lattice vectors), its inverse, pbc[b][3] and nimg[b][3].  Positions
+// are wrapped into the cell along the periodic axes in fractional coordinates (frac = pos @ inv, image = floor(frac)), and
+// the raw image offsets are folded back into the shift, so  r = pos[nbr] + shift - pos[ctr]  holds for the RAW positions.
+// An axis a needs n_a = ceil(r_max / h_a) images on each side, h_a = |det cell| / |b x c| the cell height along that axis;
+// the host computes n_a (_lib.nl_frames through data.frames_geometry, in fp64 from the cell as rounded to the positions'
+// dtype), refuses near-singular cells and bounds the images per pair, so the walk below is bounded by what it is given.
 // A frame with no periodic axis is searched as it is (no wrap, one image): a molecule.
 #include "common.cuh"
 
@@ -41,7 +43,7 @@ struct NlfFrame {
 
 template <typename T>
 __device__ __forceinline__ void nlf_load_frame(NlfFrame<T>& f, const T* __restrict__ cell, const T* __restrict__ inv,
-                                               const int32_t* __restrict__ pbc, int64_t b, double r_max) {
+                                               const int32_t* __restrict__ pbc, const int32_t* __restrict__ nimg, int64_t b) {
 #pragma unroll
     for (int k = 0; k < 9; ++k) {
         f.c[k] = cell[b * 9 + k];
@@ -52,22 +54,7 @@ __device__ __forceinline__ void nlf_load_frame(NlfFrame<T>& f, const T* __restri
     for (int a = 0; a < 3; ++a) {
         f.pbc[a] = pbc[b * 3 + a] != 0;
         f.periodic |= f.pbc[a];
-    }
-    // image range per periodic axis: ceil(r_max / height), height = |det| / |cross of the other two rows| (fp64)
-    double m[9];
-#pragma unroll
-    for (int k = 0; k < 9; ++k) m[k] = (double)f.c[k];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        f.nimg[a] = 0;
-        if (!f.pbc[a]) continue;
-        const int p = (a + 1) % 3, q = (a + 2) % 3;
-        const double x = m[p * 3 + 1] * m[q * 3 + 2] - m[p * 3 + 2] * m[q * 3 + 1];
-        const double y = m[p * 3 + 2] * m[q * 3 + 0] - m[p * 3 + 0] * m[q * 3 + 2];
-        const double z = m[p * 3 + 0] * m[q * 3 + 1] - m[p * 3 + 1] * m[q * 3 + 0];
-        const double vol = fabs(m[a * 3 + 0] * x + m[a * 3 + 1] * y + m[a * 3 + 2] * z);
-        const double h = vol / sqrt(x * x + y * y + z * z);
-        f.nimg[a] = (int)ceil(r_max / h);
+        f.nimg[a] = f.pbc[a] ? nimg[b * 3 + a] : 0;  // images on each side (host: ceil(r_max / height))
     }
 }
 
@@ -115,7 +102,7 @@ template <typename T, bool FILL>
 __global__ void __launch_bounds__(NLF_WARPS * 32) nlf_walk_kernel(int64_t n, int64_t B, const int32_t* __restrict__ frame_ptr,
                                                                   const T* __restrict__ pos, const T* __restrict__ cell,
                                                                   const T* __restrict__ inv, const int32_t* __restrict__ pbc,
-                                                                  double r_max, int32_t* __restrict__ counts,
+                                                                  const int32_t* __restrict__ nimg, double r_max, int32_t* __restrict__ counts,
                                                                   const int32_t* __restrict__ row_ptr, int32_t* __restrict__ nbr,
                                                                   T* __restrict__ shift) {
     const int lane = threadIdx.x & 31;
@@ -124,7 +111,7 @@ __global__ void __launch_bounds__(NLF_WARPS * 32) nlf_walk_kernel(int64_t n, int
     const int64_t b = nlf_frame_of(frame_ptr, B, i);
     const int64_t j0 = frame_ptr[b], j1 = frame_ptr[b + 1];
     NlfFrame<T> f;
-    nlf_load_frame(f, cell, inv, pbc, b, r_max);
+    nlf_load_frame(f, cell, inv, pbc, nimg, b);
     T wi[3];
     int imgi[3];
     nlf_wrap(f, pos, i, wi, imgi);
@@ -173,20 +160,21 @@ __global__ void __launch_bounds__(NLF_WARPS * 32) nlf_walk_kernel(int64_t n, int
 
 template <bool FILL>
 int nlf_launch(int pos_dtype, int64_t n, int64_t B, const int32_t* frame_ptr, const void* pos, const void* cell, const void* inv,
-               const int32_t* pbc, double r_max, int32_t* counts, const int32_t* row_ptr, int32_t* nbr, void* shift, void* stream) {
+               const int32_t* pbc, const int32_t* nimg, double r_max, int32_t* counts, const int32_t* row_ptr, int32_t* nbr, void* shift,
+               void* stream) {
     if (n == 0) return 0;
     AB2_CHECK_ARG(pos_dtype == AB2_F64 || pos_dtype == AB2_F32, "positions must be fp64 or fp32");
-    AB2_CHECK_ARG(B >= 1 && frame_ptr && pos && cell && inv && pbc, "null pointer or no frame");
+    AB2_CHECK_ARG(B >= 1 && frame_ptr && pos && cell && inv && pbc && nimg, "null pointer or no frame");
     AB2_CHECK_ARG(r_max > 0, "r_max must be positive");
     AB2_CHECK_ARG(FILL ? (row_ptr && nbr && shift) : (counts != nullptr), "null output pointer");
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned grid = ab2_blocks(n, NLF_WARPS);
     if (pos_dtype == AB2_F64)
         nlf_walk_kernel<double, FILL><<<grid, NLF_WARPS * 32, 0, st>>>(n, B, frame_ptr, (const double*)pos, (const double*)cell,
-                                                                      (const double*)inv, pbc, r_max, counts, row_ptr, nbr, (double*)shift);
+                                                                      (const double*)inv, pbc, nimg, r_max, counts, row_ptr, nbr, (double*)shift);
     else
         nlf_walk_kernel<float, FILL><<<grid, NLF_WARPS * 32, 0, st>>>(n, B, frame_ptr, (const float*)pos, (const float*)cell,
-                                                                     (const float*)inv, pbc, r_max, counts, row_ptr, nbr, (float*)shift);
+                                                                     (const float*)inv, pbc, nimg, r_max, counts, row_ptr, nbr, (float*)shift);
     AB2_CUDA_LAUNCH_CHECK();
     return 0;
 }
@@ -194,13 +182,14 @@ int nlf_launch(int pos_dtype, int64_t n, int64_t B, const int32_t* frame_ptr, co
 }  // namespace
 
 extern "C" int ab2_nl_frames_count(int pos_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* pos,
-                                   const void* cell, const void* inv_cell, const int32_t* pbc, double r_max, int32_t* counts,
-                                   void* stream) {
-    return nlf_launch<false>(pos_dtype, n, n_frames, frame_ptr, pos, cell, inv_cell, pbc, r_max, counts, nullptr, nullptr, nullptr, stream);
+                                   const void* cell, const void* inv_cell, const int32_t* pbc, const int32_t* nimg, double r_max,
+                                   int32_t* counts, void* stream) {
+    return nlf_launch<false>(pos_dtype, n, n_frames, frame_ptr, pos, cell, inv_cell, pbc, nimg, r_max, counts, nullptr, nullptr, nullptr,
+                             stream);
 }
 
 extern "C" int ab2_nl_frames_fill(int pos_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* pos,
-                                  const void* cell, const void* inv_cell, const int32_t* pbc, double r_max, const int32_t* row_ptr,
-                                  int32_t* nbr, void* shift, void* stream) {
-    return nlf_launch<true>(pos_dtype, n, n_frames, frame_ptr, pos, cell, inv_cell, pbc, r_max, nullptr, row_ptr, nbr, shift, stream);
+                                  const void* cell, const void* inv_cell, const int32_t* pbc, const int32_t* nimg, double r_max,
+                                  const int32_t* row_ptr, int32_t* nbr, void* shift, void* stream) {
+    return nlf_launch<true>(pos_dtype, n, n_frames, frame_ptr, pos, cell, inv_cell, pbc, nimg, r_max, nullptr, row_ptr, nbr, shift, stream);
 }

@@ -13,6 +13,7 @@ from __future__ import annotations
 import math
 from typing import Dict, Optional, Tuple
 
+import numpy as np
 import torch
 
 POSITIONS_KEY = "pos"
@@ -348,6 +349,29 @@ def is_regular_cell(cell: torch.Tensor) -> bool:
     return _lattice_metrics(cell.detach().reshape(3, 3).to(device="cpu", dtype=torch.float64).tolist())[2]
 
 
+def _lattice_metrics_batched(h: torch.Tensor):
+    """``_lattice_metrics`` of every frame of h [B,3,3] (fp64, CPU), the same operations in the same order, so bitwise
+    the same -> (regular [B] bool, heights [B,3], NaN where not regular).  numpy, whose square root is correctly rounded
+    (torch's vectorised CPU square root is not always)."""
+    h = h.numpy()
+    cr, sq = [], []
+    with np.errstate(all="ignore"):
+        for a in range(3):
+            p, q, r = h[:, (a + 1) % 3], h[:, (a + 2) % 3], h[:, a]
+            cr.append((p[:, 1] * q[:, 2] - p[:, 2] * q[:, 1], p[:, 2] * q[:, 0] - p[:, 0] * q[:, 2], p[:, 0] * q[:, 1] - p[:, 1] * q[:, 0]))
+            sq.append(r[:, 0] * r[:, 0] + r[:, 1] * r[:, 1] + r[:, 2] * r[:, 2])
+        det = h[:, 0, 0] * cr[0][0] + h[:, 0, 1] * cr[0][1] + h[:, 0, 2] * cr[0][2]
+        regular = np.isfinite(det) & (np.abs(det) > 1e-12 * np.sqrt(sq[0]) * np.sqrt(sq[1]) * np.sqrt(sq[2]))
+        heights = np.stack([np.abs(det) / np.sqrt(c[0] * c[0] + c[1] * c[1] + c[2] * c[2]) for c in cr], 1)
+    heights[~regular] = np.nan
+    return torch.from_numpy(regular), torch.from_numpy(heights)
+
+
+def regular_cells(cell: torch.Tensor) -> torch.Tensor:
+    """``is_regular_cell`` of every frame of a batch: cell [B,3,3] -> bool [B] on the CPU."""
+    return _lattice_metrics_batched(cell.detach().reshape(-1, 3, 3).to(device="cpu", dtype=torch.float64))[0]
+
+
 def _unit(v):
     n = math.sqrt(sum(x * x for x in v))
     return [x / n for x in v] if n > 0 and math.isfinite(n) else None
@@ -517,6 +541,9 @@ def neighbor_csr(pos: torch.Tensor, r_max: float, cell: Optional[torch.Tensor], 
 # Largest frame neighbor_csr_frames takes: its search is all-pairs per frame, O(N_b^2 * images).  Larger frames belong to
 # neighbor_csr (cell list) or neighbor_list.
 FRAMES_MAX_ATOMS = 4096
+# Most images per pair, prod_a (2 n_a + 1), neighbor_csr_frames searches: a cell 0.01 r_max high on every axis needs
+# 201^3 = 8.1e6.  Such frames belong to neighbor_csr, whose cell list visits bins instead of images.
+FRAMES_MAX_IMAGES = 1 << 20
 
 
 def _frames_pbc(pbc, B: int, device) -> torch.Tensor:
@@ -532,16 +559,74 @@ def _frames_pbc(pbc, B: int, device) -> torch.Tensor:
     return t
 
 
+def frames_geometry(cell: Optional[torch.Tensor], pbc: torch.Tensor, r_max: float, dtype=torch.float64):
+    """Geometry of every frame of a batch for ab2_nl_frames_* -> (rows [B,3,3] fp64, nimg [B,3] int64), both on the CPU.
+
+    ``cell`` [B,3,3] or None, ``pbc`` [B,3] booleans, ``dtype`` the positions' dtype: the rows are those the search sees,
+    the cell rounded to ``dtype``.
+    * A frame with no periodic axis gets zero rows and no images: a molecule, its cell is not used.
+    * Open-axis rows that are zero (ASE's 2-D and 1-D cells), not finite, or that leave the cell singular are replaced as
+      ``lattice_grid`` replaces them (``_complete_open_rows``).  Shifts along open axes are 0, so a replaced row never
+      reaches an output.
+    * A periodic axis a searches nimg_a = ceil(r_max / H_a) images on each side, H_a the height of the rows along a,
+      computed in fp64 with the operations of ``_lattice_metrics``.
+    Raises ValueError, before any search, for a periodic frame without a cell, a non-finite periodic row, rows that
+    ``is_regular_cell`` rejects (a zero periodic row, rows within 1e-12 rad of a common plane), or more than
+    FRAMES_MAX_IMAGES images per pair.  Applied to its own rows it returns them unchanged, with the same counts:
+    ``_lib.nl_frames`` takes the kernels' image counts from it."""
+    pbc = pbc.to(device="cpu", dtype=torch.bool).numpy()
+    B = pbc.shape[0]
+    periodic = pbc.any(axis=1)
+    if cell is None:
+        if periodic.any():
+            raise ValueError("periodic frames need a cell")
+        return torch.zeros(B, 3, 3, dtype=torch.float64), torch.zeros(B, 3, dtype=torch.int64)
+    if cell.numel() != 9 * B:
+        raise ValueError(f"cell has {cell.numel()} entries for {B} frames")
+    h = cell.detach().reshape(B, 3, 3).to(device="cpu", dtype=dtype).to(torch.float64).numpy().copy()
+    h[~periodic] = 0.0
+    finite = np.isfinite(h).all(axis=2)
+    bad = (pbc & ~finite).any(axis=1)
+    if bad.any():
+        raise ValueError(f"frame {int(np.flatnonzero(bad)[0])} has a periodic cell row that is not finite")
+    regular, heights = _lattice_metrics_batched(torch.from_numpy(np.where(finite[:, :, None], h, 0.0)))
+    regular = regular.numpy()
+    zero_open = ((h == 0).all(axis=2) & ~pbc).any(axis=1)
+    fix = periodic & (~pbc).any(axis=1) & (zero_open | ~finite.all(axis=1) | ~regular)
+    if fix.any():
+        for b in np.flatnonzero(fix).tolist():
+            rows = _complete_open_rows(h[b].tolist(), pbc[b].tolist())
+            if rows is not None:
+                h[b] = torch.tensor(rows, dtype=torch.float64).to(dtype).to(torch.float64).numpy()
+        regular, heights = _lattice_metrics_batched(torch.from_numpy(h))
+        regular = regular.numpy()
+    bad = periodic & ~regular
+    if bad.any():
+        raise ValueError(f"frame {int(np.flatnonzero(bad)[0])} has a singular or near-coplanar periodic cell "
+                         "(rows within 1e-12 rad of a common plane)")
+    with np.errstate(invalid="ignore"):
+        nimg = np.where(pbc, np.ceil(float(r_max) / heights.numpy()), 0.0)
+    images = (2 * nimg + 1).prod(axis=1)
+    bad = ~(images <= FRAMES_MAX_IMAGES)
+    if bad.any():
+        b = int(np.flatnonzero(bad)[0])
+        raise ValueError(f"frame {b} needs {float(images[b]):.3g} periodic images per pair (cell heights "
+                         f"{heights[b].tolist()} for r_max {r_max}); neighbor_csr_frames searches at most {FRAMES_MAX_IMAGES}: "
+                         "use neighbor_csr")
+    return torch.from_numpy(h), torch.from_numpy(nimg.astype(np.int64))
+
+
 def neighbor_csr_frames(pos: torch.Tensor, frame_ptr, cell: Optional[torch.Tensor], pbc, r_max: float):
     """Neighbour lists of a batch of small frames in one pass on the device (ab2_nl_frames_count / fill), straight into the
     kernels' format -> (EdgeCSR over all atoms of the batch, shift_vec [E,3] in the positions' dtype).
 
     ``frame_ptr`` [B+1]: the atoms of frame b are [frame_ptr[b], frame_ptr[b+1]).  ``cell`` [B,3,3] (or None: no frame is
-    periodic), ``pbc`` [B,3] or (3,) booleans.  Any cell ``neighbor_list`` takes: triclinic, narrower than r_max, mixed
-    periodicity; a frame with no periodic axis is a molecule (its cell is not used).  Rows are those of
-    ``neighbor_list(frame, method="brute")`` in the same order (by neighbour, then by image), with the frame's atom offset
-    added;  r = pos[nbr] + shift - pos[ctr]  holds for the raw positions.  Frames above FRAMES_MAX_ATOMS atoms are rejected:
-    the search is all-pairs per frame."""
+    periodic), ``pbc`` [B,3] or (3,) booleans.  Any regular cell: triclinic, left-handed, narrower than r_max, mixed
+    periodicity, ASE's zero rows on open axes; a frame with no periodic axis is a molecule (its cell is not used).  Rows
+    are those of ``neighbor_list(frame, method="brute")`` in the same order (by neighbour, then by image), with the frame's
+    atom offset added;  r = pos[nbr] + shift - pos[ctr]  holds for the raw positions.  Refused with ValueError before any
+    search (``frames_geometry``): frames above FRAMES_MAX_ATOMS atoms (the search is all-pairs per frame), periodic frames
+    with a non-finite, singular or near-coplanar cell, and frames needing more than FRAMES_MAX_IMAGES images per pair."""
     from . import _lib
 
     dev = pos.device
@@ -554,25 +639,14 @@ def neighbor_csr_frames(pos: torch.Tensor, frame_ptr, cell: Optional[torch.Tenso
     if big > FRAMES_MAX_ATOMS:
         raise ValueError(f"neighbor_csr_frames takes frames of at most {FRAMES_MAX_ATOMS} atoms (got {big}); "
                          "use neighbor_csr or neighbor_list for large frames")
-    pbc_t = _frames_pbc(pbc, B, dev)
-    periodic = pbc_t.any(dim=1)
-    if cell is None:
-        if bool(periodic.any()):
-            raise ValueError("periodic frames need a cell")
-        cell64 = torch.zeros(B, 3, 3, dtype=torch.float64, device=dev)
-    else:
-        if cell.numel() != 9 * B:
-            raise ValueError(f"cell has {cell.numel()} entries for {B} frames")
-        cell64 = cell.reshape(B, 3, 3).to(device=dev, dtype=torch.float64)
-    # a frame with no periodic axis is searched as it is: its cell never enters (zeros keep the shift vectors exactly 0)
-    cell64 = torch.where(periodic.view(B, 1, 1), cell64, torch.zeros_like(cell64))
+    pbc_t = _frames_pbc(pbc, B, "cpu")
+    rows, _ = frames_geometry(cell, pbc_t, r_max, pos.dtype)  # refuses before any device work; _lib.nl_frames derives nimg
+    rows = rows.to(dev)
+    periodic = pbc_t.any(dim=1).view(B, 1, 1).to(dev)
     eye = torch.eye(3, dtype=torch.float64, device=dev).expand(B, 3, 3)
-    det = torch.linalg.det(torch.where(periodic.view(B, 1, 1), cell64, eye))
-    if not bool(torch.isfinite(det).all()) or bool((det == 0).any()):
-        raise ValueError("a periodic frame has a singular cell")
-    inv64 = torch.where(periodic.view(B, 1, 1), torch.linalg.inv(torch.where(periodic.view(B, 1, 1), cell64, eye)), torch.zeros_like(cell64))
-    row_ptr, nbr, shift = _lib.nl_frames(pos.contiguous(), fp.to(device=dev, dtype=torch.int32), cell64.to(pos.dtype).contiguous(),
-                                         inv64.to(pos.dtype).contiguous(), pbc_t.to(torch.int32).contiguous(), float(r_max))
+    inv = torch.where(periodic, torch.linalg.inv(torch.where(periodic, rows, eye)), torch.zeros_like(rows))
+    row_ptr, nbr, shift = _lib.nl_frames(pos.contiguous(), fp.to(device=dev, dtype=torch.int32), rows.to(pos.dtype).contiguous(),
+                                         inv.to(pos.dtype).contiguous(), pbc_t.to(device=dev, dtype=torch.int32), float(r_max))
     counts = row_ptr[1:] - row_ptr[:-1]
     ctr = torch.repeat_interleave(torch.arange(n, device=dev, dtype=torch.int32), counts.long())
     maxdeg = int(counts.max()) if n > 0 else 0

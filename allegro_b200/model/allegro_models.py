@@ -302,7 +302,8 @@ class FusedAllegroEnergy(torch.nn.Module):
         ``edge_csr`` + ``edge_shift_vec`` of ``data.neighbor_csr_frames`` (``batch.collate`` builds either).  Writes
         ``atomic_energy`` [N,1], ``forces`` [N,3], ``edge_energy`` / ``edge_features`` (input edge order) and
         ``total_energy`` [B,1]; with ``stress=True`` also ``stress`` / ``virial`` [B,3,3], which need a non-singular cell
-        on every frame.  ``atomic_virial`` / ``heat_current`` as in ``energy_and_forces``: ``atomic_virial`` [N,3,3] and
+        on every frame (``data.is_regular_cell``: a frame with ASE's zero rows or rows within 1e-12 rad of a common plane
+        raises ValueError).  ``atomic_virial`` / ``heat_current`` as in ``energy_and_forces``: ``atomic_virial`` [N,3,3] and
         ``heat_current`` [B,3], one row per frame (ab2_frame_heat_current)."""
         pos = data[D.POSITIONS_KEY]
         if not pos.is_cuda:
@@ -384,11 +385,12 @@ class FusedAllegroEnergy(torch.nn.Module):
                 raise ValueError("stress=True needs a cell on every frame")
 
             def _volume():
+                bad = ~D.regular_cells(cell)
+                if bool(bad.any()):
+                    raise ValueError(f"stress=True needs a non-singular cell on every frame (data.is_regular_cell); frame "
+                                     f"{int(bad.nonzero()[0, 0])} has none: stress is the virial over the cell volume")
                 c = cell.reshape(B, 3, 3).to(core.acc)
-                v = (c[:, 0] * torch.linalg.cross(c[:, 1], c[:, 2])).sum(-1).abs()
-                if bool((v == 0).any()):
-                    raise ValueError("stress=True needs a non-singular cell on every frame")
-                return v
+                return (c[:, 0] * torch.linalg.cross(c[:, 1], c[:, 2])).sum(-1).abs()
 
             volume = self._cached("frames_volume", (cell,), (B, core.acc), _volume)
         types_in = data[D.ATOM_TYPE_KEY]

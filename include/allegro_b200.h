@@ -369,18 +369,22 @@ int ab2_nl_lattice_fill(int pos_dtype, int64_t n_centres, const void* pos, const
  * range, so the work of frame b is O(N_b^2 * images): meant for small frames (the Python wrapper caps them).
  * Geometry, all device buffers: frame_ptr[n_frames+1] int32 (atoms of frame b are [frame_ptr[b], frame_ptr[b+1]),
  * frame_ptr[0] = 0, frame_ptr[n_frames] = n), cell / inv_cell [n_frames][3][3] (rows = lattice vectors; inv_cell its
- * inverse, any finite values for a frame with no periodic axis), pbc [n_frames][3] int32.  pos: [n][3] fp64 or fp32
+ * inverse, any finite values for a frame with no periodic axis), pbc [n_frames][3] int32, nimg [n_frames][3] int32 the
+ * images searched on each side of every periodic axis (ceil(r_max / h_a); ignored on open axes).  The kernels walk
+ * prod(2 nimg_a + 1) images per pair as given: the caller bounds them (the Python wrapper _lib.nl_frames computes them
+ * on the host with data.frames_geometry, which refuses near-singular cells and caps the product at
+ * data.FRAMES_MAX_IMAGES).  pos: [n][3] fp64 or fp32
  * raw (unwrapped) coordinates; cell, inv_cell and shift in the same dtype.  Positions are wrapped along the periodic
  * axes in fractional coordinates (frac = pos @ inv_cell, image = floor(frac)) and the raw images folded back, so
  *   r = pos[nbr] + shift - pos[centre]  holds for the raw positions; shift = (integer image) @ cell.
  * Rows are ordered by neighbour index, then by image (x, y, z) lexicographically.  Every atom is a centre.
  * Call order: ab2_nl_frames_count -> (host: row_ptr = prefix sum of counts) -> ab2_nl_frames_fill. */
 int ab2_nl_frames_count(int pos_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* pos,
-                        const void* cell, const void* inv_cell, const int32_t* pbc, double r_max, int32_t* counts,
-                        void* stream);
+                        const void* cell, const void* inv_cell, const int32_t* pbc, const int32_t* nimg, double r_max,
+                        int32_t* counts, void* stream);
 int ab2_nl_frames_fill(int pos_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* pos,
-                       const void* cell, const void* inv_cell, const int32_t* pbc, double r_max, const int32_t* row_ptr,
-                       int32_t* nbr, void* shift, void* stream);
+                       const void* cell, const void* inv_cell, const int32_t* pbc, const int32_t* nimg, double r_max,
+                       const int32_t* row_ptr, int32_t* nbr, void* shift, void* stream);
 
 /* Per-frame reductions (nequip's per-graph sums of a batch):
  *   ab2_frame_sum     out[b] = sum_{a in [frame_ptr[b], frame_ptr[b+1])} x[a]                 x [n], out [n_frames]

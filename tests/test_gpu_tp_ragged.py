@@ -300,25 +300,19 @@ def _kernels_launched(fn, runs=5):
     names is None when the profiler sees no kernel at all.
 
     One trace is not complete evidence: now and then it is empty, or it lacks the records of some kernels that ran (in a
-    long pytest process, a forward or backward tensor-product kernel was missing while the values were right).  So fn
-    runs under the profiler until two consecutive non-empty traces name the same set of kernels (at most ``runs``
-    times), and names is the union of what the traces saw: it holds only kernels that ran, so a family that was not
-    launched can never appear in it."""
+    long pytest process, a forward or backward tensor-product kernel was missing while the values were right, in two
+    consecutive traces).  So fn runs under the profiler ``runs`` times, and names is the union of what the traces saw:
+    it holds only kernels that ran, so a family that was not launched can never appear in it, and a kernel is missed
+    only if every trace drops it."""
     from torch.profiler import ProfilerActivity, profile
 
-    out, prev, union = None, None, set()
+    out, union = None, set()
     for _ in range(runs):
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             res = fn()
         out = res if out is None else out
         names = {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
-        names = {n for n in names if not n.startswith(("Memset", "Memcpy"))}
-        if not names:
-            continue
-        union |= names
-        if names == prev:
-            break
-        prev = names
+        union |= {n for n in names if not n.startswith(("Memset", "Memcpy"))}
     return out, (sorted(union) if union else None)
 
 
