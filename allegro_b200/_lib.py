@@ -76,6 +76,10 @@ _SIGNATURES = {
     "ab2_p2p_push_rows": ([_i32, _i32, _i32, _vp, _vp, _i32, _dbl, _vp, _i32, _i32, _vp, _vp, _vp], C.c_int),
     "ab2_p2p_wait_unpack": ([_i32, _i32, _i32, _vp, _i32, _i32, _vp, _i32, _vp, _vp, _i32, _vp], C.c_int),
     "ab2_p2p_allreduce_energy": ([_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_p2p_mailbox_bytes_ex": ([_i32, _i32, _i32], C.c_int64),
+    "ab2_p2p_push_rows_w": ([_i32, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _vp, _vp, _vp], C.c_int),
+    "ab2_p2p_wait_unpack_w": ([_i32, _i32, _vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_p2p_allreduce_vec": ([_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_nl_bin": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_nl_count": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_nl_fill": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),

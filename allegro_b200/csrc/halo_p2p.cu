@@ -15,6 +15,12 @@
 //   [parity][side] boundary gradients (3 * max_rows doubles)
 //   [parity][rank] energies (double)
 //   flags (uint32 step numbers): pos[parity][side], grad[parity][side], energy[parity][rank]; then an error word
+//
+// Extended mailbox (ab2_p2p_mailbox_bytes_ex with AB2_P2P_EXT_VIRIAL): the base layout above, unchanged (so the error
+// word stays where ab2_p2p_error looks), then, from the next 256-byte boundary
+//   [parity][side] reverse rows of width 12 (3 gradient + 9 per-atom virial values, fp64; 12 * max_rows doubles)
+//   [parity][rank] a vector of up to AB2_P2P_VEC_MAX doubles (energy, virial, heat current)
+//   flags: wrows[parity][side], vec[parity][rank]
 #include "common.cuh"
 
 namespace {
@@ -31,6 +37,22 @@ struct MailboxLayout {
     __host__ __device__ int e_flag(int par, int rank) const { return 8 + par * world + rank; }
     __host__ __device__ int err_word() const { return 8 + 2 * world; }
     __host__ __device__ size_t bytes() const { return flag_off() + (size_t)(err_word() + 1) * 4 + 64; }
+};
+
+struct ExtLayout {
+    MailboxLayout B;
+    __host__ __device__ size_t base() const { return (B.bytes() + 255) & ~(size_t)255; }
+    __host__ __device__ size_t wrows_bytes() const { return (size_t)12 * B.max_rows * 8; }
+    __host__ __device__ size_t wrows_off(int par, int side) const { return base() + (size_t)(par * 2 + side) * wrows_bytes(); }
+    __host__ __device__ size_t vec_off(int par, int rank) const {
+        return base() + 4 * wrows_bytes() + ((size_t)par * B.world + rank) * AB2_P2P_VEC_MAX * 8;
+    }
+    __host__ __device__ size_t flag_off() const { return base() + 4 * wrows_bytes() + (size_t)2 * B.world * AB2_P2P_VEC_MAX * 8; }
+    __host__ __device__ int wrows_flag(int par, int side) const { return par * 2 + side; }
+    __host__ __device__ int vec_flag(int par, int rank) const { return 4 + par * B.world + rank; }
+    __host__ __device__ size_t bytes() const { return flag_off() + (size_t)(4 + 2 * B.world) * 4 + 64; }
+    // the one error word of the mailbox, in the base layout
+    __host__ __device__ uint32_t* err(uint8_t* mailbox) const { return reinterpret_cast<uint32_t*>(mailbox + B.flag_off()) + B.err_word(); }
 };
 
 __device__ __forceinline__ void st_release_sys(uint32_t* p, uint32_t v) {
@@ -136,6 +158,93 @@ __global__ void p2p_sum_energy_kernel(MailboxLayout L, uint8_t* __restrict__ min
     *out = tot;
 }
 
+// Reverse rows of width 12: gradient row i (g[3i..3i+2]) and per-atom virial row i (W[9i..9i+8]) -> the PEER's wrows
+// slot `side`, one element per thread so that the stores over NVLink are contiguous; then the flag, as above.
+template <typename TSrc>
+__global__ void __launch_bounds__(256) p2p_push_wrows_kernel(ExtLayout L, int side, const TSrc* __restrict__ g, const TSrc* __restrict__ W,
+                                                             int n, uint8_t* __restrict__ peer, const uint32_t* __restrict__ step,
+                                                             uint32_t* __restrict__ done_ctr) {
+    const uint32_t s = *step;
+    const int par = (int)(s & 1u);
+    double* __restrict__ dst = reinterpret_cast<double*>(peer + L.wrows_off(par, side));
+    const int64_t e = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (e < (int64_t)12 * n) {
+        const int64_t i = e / 12;
+        const int c = (int)(e - 12 * i);
+        dst[e] = c < 3 ? (double)g[3 * i + c] : (double)W[9 * i + (c - 3)];
+    }
+    __threadfence_system();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const uint32_t prev = atomicAdd(done_ctr, 1u);
+        if (prev == gridDim.x - 1) {
+            *done_ctr = 0;
+            __threadfence_system();
+            uint32_t* flags = reinterpret_cast<uint32_t*>(peer + L.flag_off());
+            st_release_sys(flags + L.wrows_flag(par, side), s);
+        }
+    }
+}
+
+// wait for this step's width-12 rows in MY mailbox slot `side`, then g_dst[idx[i]] += gradient row i and
+// W_dst[idx[i]] += virial row i (idx unique within one call, so one launch adds both without atomics)
+template <typename TDst>
+__global__ void __launch_bounds__(256) p2p_wait_unpack_wrows_kernel(ExtLayout L, int side, uint8_t* __restrict__ mine, const uint32_t* __restrict__ step,
+                                                                    int n, TDst* __restrict__ g_dst, TDst* __restrict__ W_dst,
+                                                                    const int64_t* __restrict__ idx) {
+    __shared__ int ok;
+    const uint32_t s = *step;
+    const int par = (int)(s & 1u);
+    const uint32_t* flags = reinterpret_cast<const uint32_t*>(mine + L.flag_off());
+    if (threadIdx.x == 0) ok = wait_flag(flags + L.wrows_flag(par, side), s, L.err(mine)) ? 1 : 0;
+    __syncthreads();
+    if (!ok) return;
+    const double* __restrict__ box = reinterpret_cast<const double*>(mine + L.wrows_off(par, side));
+    const int64_t e = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (e < (int64_t)12 * n) {
+        const int64_t i = e / 12;
+        const int c = (int)(e - 12 * i);
+        const int64_t r = idx ? idx[i] : i;
+        const double v = box[e];
+        if (c < 3) g_dst[3 * r + c] += (TDst)v;
+        else W_dst[9 * r + (c - 3)] += (TDst)v;
+    }
+}
+
+// thread r stores my n_values doubles into rank r's vec slot [parity][my rank], then publishes the step number
+__global__ void p2p_push_vec_kernel(ExtLayout L, const double* __restrict__ v_local, int n_values, int rank, uint8_t* const* __restrict__ peers,
+                                    const uint32_t* __restrict__ step) {
+    const int r = threadIdx.x;
+    if (r >= L.B.world) return;
+    const uint32_t s = *step;
+    const int par = (int)(s & 1u);
+    uint8_t* peer = peers[r];
+    double* dst = reinterpret_cast<double*>(peer + L.vec_off(par, rank));
+    for (int k = 0; k < n_values; ++k) dst[k] = v_local[k];
+    __threadfence_system();
+    st_release_sys(reinterpret_cast<uint32_t*>(peer + L.flag_off()) + L.vec_flag(par, rank), s);
+}
+
+// thread 0 waits for every rank's vector; then thread k sums component k over the ranks in rank order (bitwise
+// identical on every rank, and component 0 bitwise equal to what p2p_sum_energy_kernel gives for the same values)
+__global__ void p2p_sum_vec_kernel(ExtLayout L, uint8_t* __restrict__ mine, const uint32_t* __restrict__ step, int n_values, double* __restrict__ out) {
+    __shared__ int ok;
+    const uint32_t s = *step;
+    const int par = (int)(s & 1u);
+    const uint32_t* flags = reinterpret_cast<const uint32_t*>(mine + L.flag_off());
+    if (threadIdx.x == 0) {
+        ok = 1;
+        for (int r = 0; r < L.B.world && ok; ++r) ok = wait_flag(flags + L.vec_flag(par, r), s, L.err(mine)) ? 1 : 0;
+    }
+    __syncthreads();
+    if (!ok) return;
+    const int k = threadIdx.x;
+    if (k >= n_values) return;
+    double tot = 0.0;
+    for (int r = 0; r < L.B.world; ++r) tot += reinterpret_cast<const double*>(mine + L.vec_off(par, r))[k];
+    out[k] = tot;
+}
+
 }  // namespace
 
 // ---- host API (C ABI) -----------------------------------------------------------------------------------------
@@ -232,6 +341,69 @@ extern "C" int ab2_p2p_allreduce_energy(const void* e_local, int rank, int world
     cudaStream_t st = (cudaStream_t)stream;
     p2p_push_energy_kernel<<<1, 64, 0, st>>>(L, (const double*)e_local, rank, (uint8_t* const*)peers_dev, (const uint32_t*)step_counter);
     p2p_sum_energy_kernel<<<1, 1, 0, st>>>(L, (uint8_t*)my_mailbox, (const uint32_t*)step_counter, (double*)e_total);
+    AB2_CUDA_LAUNCH_CHECK();
+    return 0;
+}
+
+/* Size of a mailbox with the optional sections of `flags` (0: exactly ab2_p2p_mailbox_bytes; AB2_P2P_EXT_VIRIAL: the
+ * width-12 reverse rows and the vector all-reduce).  -1 for unknown flag bits. */
+extern "C" int64_t ab2_p2p_mailbox_bytes_ex(int max_rows, int world, int flags) {
+    if (flags & ~AB2_P2P_EXT_VIRIAL) return -1;
+    MailboxLayout B{max_rows, world};
+    if (!flags) return (int64_t)B.bytes();
+    return (int64_t)ExtLayout{B}.bytes();
+}
+
+/* Push n reverse rows of width 12 -- gradient rows g[i][3] and per-atom virial rows W[i][3][3], i < n, both fp64 or both
+ * fp32 -- into the PEER's (extended) mailbox slot `side`. */
+extern "C" int ab2_p2p_push_rows_w(int src_dtype, int side, const void* g_src, const void* W_src, int n, void* peer_mailbox, int max_rows,
+                                   int world, const void* step_counter, void* done_counter, void* stream) {
+    AB2_CHECK_ARG(g_src && W_src && peer_mailbox && step_counter && done_counter && n >= 0 && n <= max_rows && (side == 0 || side == 1),
+                  "bad arguments");
+    AB2_CHECK_ARG(src_dtype == AB2_F64 || src_dtype == AB2_F32, "rows must be fp64 or fp32");
+    ExtLayout L{MailboxLayout{max_rows, world}};
+    cudaStream_t st = (cudaStream_t)stream;
+    const unsigned grid = n > 0 ? ab2_blocks((int64_t)12 * n, 256) : 1;
+    if (src_dtype == AB2_F64)
+        p2p_push_wrows_kernel<double><<<grid, 256, 0, st>>>(L, side, (const double*)g_src, (const double*)W_src, n, (uint8_t*)peer_mailbox,
+                                                           (const uint32_t*)step_counter, (uint32_t*)done_counter);
+    else
+        p2p_push_wrows_kernel<float><<<grid, 256, 0, st>>>(L, side, (const float*)g_src, (const float*)W_src, n, (uint8_t*)peer_mailbox,
+                                                          (const uint32_t*)step_counter, (uint32_t*)done_counter);
+    AB2_CUDA_LAUNCH_CHECK();
+    return 0;
+}
+
+/* Wait for this step's width-12 rows in MY (extended) mailbox slot `side` and add them: g_dst[idx[i]] += gradient row i,
+ * W_dst[idx[i]] += virial row i (idx null: row i). */
+extern "C" int ab2_p2p_wait_unpack_w(int dst_dtype, int side, void* my_mailbox, int max_rows, int world, const void* step_counter, int n,
+                                     void* g_dst, void* W_dst, const int64_t* idx, void* stream) {
+    AB2_CHECK_ARG(my_mailbox && step_counter && g_dst && W_dst && n >= 0 && n <= max_rows && (side == 0 || side == 1), "bad arguments");
+    AB2_CHECK_ARG(dst_dtype == AB2_F64 || dst_dtype == AB2_F32, "rows must be fp64 or fp32");
+    ExtLayout L{MailboxLayout{max_rows, world}};
+    cudaStream_t st = (cudaStream_t)stream;
+    const unsigned grid = n > 0 ? ab2_blocks((int64_t)12 * n, 256) : 1;
+    if (dst_dtype == AB2_F64)
+        p2p_wait_unpack_wrows_kernel<double><<<grid, 256, 0, st>>>(L, side, (uint8_t*)my_mailbox, (const uint32_t*)step_counter, n, (double*)g_dst,
+                                                                  (double*)W_dst, idx);
+    else
+        p2p_wait_unpack_wrows_kernel<float><<<grid, 256, 0, st>>>(L, side, (uint8_t*)my_mailbox, (const uint32_t*)step_counter, n, (float*)g_dst,
+                                                                 (float*)W_dst, idx);
+    AB2_CUDA_LAUNCH_CHECK();
+    return 0;
+}
+
+/* All-reduce of n_values <= AB2_P2P_VEC_MAX doubles through the extended mailboxes: the ab2_p2p_allreduce_energy protocol
+ * for a vector; v_total[k] = sum over ranks in rank order of v_local[k], bitwise identical on every rank. */
+extern "C" int ab2_p2p_allreduce_vec(const void* v_local, int n_values, int rank, int world, int max_rows, void* const* peers_dev,
+                                     void* my_mailbox, const void* step_counter, void* v_total, void* stream) {
+    AB2_CHECK_ARG(v_local && peers_dev && my_mailbox && step_counter && v_total && world >= 1 && world <= 64 && rank >= 0 && rank < world,
+                  "bad arguments");
+    AB2_CHECK_ARG(n_values >= 1 && n_values <= AB2_P2P_VEC_MAX, "n_values must be in [1, 16]");
+    ExtLayout L{MailboxLayout{max_rows, world}};
+    cudaStream_t st = (cudaStream_t)stream;
+    p2p_push_vec_kernel<<<1, 64, 0, st>>>(L, (const double*)v_local, n_values, rank, (uint8_t* const*)peers_dev, (const uint32_t*)step_counter);
+    p2p_sum_vec_kernel<<<1, 32, 0, st>>>(L, (uint8_t*)my_mailbox, (const uint32_t*)step_counter, n_values, (double*)v_total);
     AB2_CUDA_LAUNCH_CHECK();
     return 0;
 }

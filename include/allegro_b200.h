@@ -465,6 +465,32 @@ int ab2_p2p_wait_unpack(int dst_dtype, int kind, int side, void* my_mailbox, int
 int ab2_p2p_allreduce_energy(const void* e_local, int rank, int world, int max_rows, void* const* peers_dev,
                              void* my_mailbox, const void* step_counter, void* e_total, void* stream);
 
+/* Extended mailbox for the stress, per-atom virial and heat current of a slab-decomposed step.  With
+ * flags = AB2_P2P_EXT_VIRIAL, ab2_p2p_mailbox_bytes_ex sizes the base mailbox (same offsets, same error word, so every
+ * call above works on it unchanged) followed by
+ *   [parity][side] reverse rows of width 12, fp64: 3 gradient then 9 per-atom virial values W[a][p][q] (row-major),
+ *   [parity][rank] a vector of up to AB2_P2P_VEC_MAX doubles,
+ *   their flags;
+ * flags = 0 gives exactly ab2_p2p_mailbox_bytes, unknown bits -1.  Every rank must allocate with the same flags: peers
+ * compute offsets into each other's mailboxes from (max_rows, world, flags).
+ * ab2_p2p_push_rows_w / ab2_p2p_wait_unpack_w are ab2_p2p_push_rows / ab2_p2p_wait_unpack (kind 1, accumulate) for the
+ * width-12 rows: the push reads n gradient rows g_src[n][3] and n virial rows W_src[n][3][3] (both fp64 or both fp32;
+ * the ghost rows, contiguous), the unpack adds them into g_dst[idx[i]] and W_dst[idx[i]] in one launch (idx entries
+ * unique, null = row i).  A ghost's W row is what its owner must receive (ab2_force_virial_scatter), so after the two
+ * unpacks (left neighbour's slot 0 first, then slot 1: fixed order) W_dst holds the owned atoms' full W.
+ * ab2_p2p_allreduce_vec sums n_values (1..AB2_P2P_VEC_MAX) doubles over the ranks, in rank order: bitwise the same
+ * result on every rank, and for n_values = 1 bitwise what ab2_p2p_allreduce_energy gives.  All waits are bounded and set
+ * the mailbox's one error word (ab2_p2p_error). */
+#define AB2_P2P_EXT_VIRIAL 1
+#define AB2_P2P_VEC_MAX 16
+int64_t ab2_p2p_mailbox_bytes_ex(int max_rows, int world, int flags);
+int ab2_p2p_push_rows_w(int src_dtype, int side, const void* g_src, const void* W_src, int n, void* peer_mailbox,
+                        int max_rows, int world, const void* step_counter, void* done_counter, void* stream);
+int ab2_p2p_wait_unpack_w(int dst_dtype, int side, void* my_mailbox, int max_rows, int world,
+                          const void* step_counter, int n, void* g_dst, void* W_dst, const int64_t* idx, void* stream);
+int ab2_p2p_allreduce_vec(const void* v_local, int n_values, int rank, int world, int max_rows, void* const* peers_dev,
+                          void* my_mailbox, const void* step_counter, void* v_total, void* stream);
+
 /* layout helpers between the reference strided layout [z][u][i] and the internal [z][i][u] */
 int ab2_transpose_ui(int dtype, int64_t E, int U, int d, const void* src, void* dst, int to_internal,
                      void* stream);
