@@ -80,6 +80,8 @@ _SIGNATURES = {
     "ab2_p2p_push_rows_w": ([_i32, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _vp, _vp, _vp], C.c_int),
     "ab2_p2p_wait_unpack_w": ([_i32, _i32, _vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_p2p_allreduce_vec": ([_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_slab_plan_count": ([_i32, _i32, _i64, _vp, _vp, _vp, _i32, _i32, _dbl, _dbl, _dbl, _vp, _vp, _vp], C.c_int),
+    "ab2_slab_plan_fill": ([_i64, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_nl_bin": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_nl_count": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_nl_fill": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
@@ -755,6 +757,50 @@ def radial_pq_bwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table,
             _ptr(_contig(aux, "aux")) if aux is not None else None, _ptr(gvec), _stream())
     with _timed("radial_bwd"):
         _check(load().ab2_radial_pq_bwd(*args) if nonlin == NL_SILU else load().ab2_radial_pq_bwd_nl(*args, nonlin))
+
+
+# --------------------------------------------------------------------------- #
+# slab decomposition plan (ab2_slab_plan_count / fill)
+# --------------------------------------------------------------------------- #
+def _slab_plan(mode: int, pos: torch.Tensor, image: Optional[torch.Tensor], box, rank: int, world: int, width: float, jump: float,
+               r_list: float, n_lists: int):
+    """count -> prefix sum over the blocks -> fill; -> (lists [n_lists] int64, refused count).  The totals are the one
+    device-to-host read."""
+    n = pos.shape[0]
+    if n == 0:
+        return [torch.empty(0, dtype=torch.int64, device=pos.device) for _ in range(n_lists)], 0
+    nblk = (n + 255) // 256
+    cls = torch.empty(n, dtype=torch.uint8, device=pos.device)
+    counts = torch.empty(nblk, 4, dtype=torch.int32, device=pos.device)
+    boxa = (C.c_double * 3)(*[float(b) for b in box])
+    with _timed("slab_plan_count"):
+        _check(load().ab2_slab_plan_count(DTYPE_ENUM[pos.dtype], mode, n, _ptr(_contig(pos, "pos")), _ptr(image), boxa, int(rank), int(world),
+                                          float(width), float(jump), float(r_list), _ptr(cls), _ptr(counts), _stream()))
+    incl = torch.cumsum(counts, 0, dtype=torch.int32)
+    offsets = (incl - counts).contiguous()
+    lists = [torch.empty(n, dtype=torch.int64, device=pos.device) for _ in range(n_lists)]
+    ptrs = [_ptr(t) for t in lists] + [None] * (3 - n_lists)
+    with _timed("slab_plan_fill"):
+        _check(load().ab2_slab_plan_fill(n, _ptr(cls), _ptr(offsets), *ptrs, _stream()))
+    totals = incl[-1].tolist()
+    return [t[:c] for t, c in zip(lists, totals)], int(totals[3])
+
+
+def slab_wrap_classify(pos: torch.Tensor, image: torch.Tensor, box, rank: int, world: int, width: float, jump: float = float("inf")):
+    """Wrap ``pos`` [n,3] into [0, box) in place, add the boxes removed to ``image`` [n,3] int32, and classify every atom
+    by its slab clamp(floor(x / width), 0, world - 1) -> (stay, to_left, to_right, n_refused): ascending int64 index
+    lists, and the number of atoms bound for a non-adjacent slab or whose x before the wrap lay outside
+    [lo - jump, hi + jump) (ab2_slab_plan_count / fill, mode 0)."""
+    assert image.dtype == torch.int32 and image.shape == pos.shape
+    (stay, left, right), refused = _slab_plan(0, pos, _contig(image, "image"), box, rank, world, width, jump, 0.0, 3)
+    return stay, left, right, refused
+
+
+def slab_faces(pos: torch.Tensor, box, rank: int, world: int, width: float, r_list: float):
+    """Atoms of the slab within ``r_list`` of its faces -> (low, high): ascending int64 index lists of x < lo + r_list (the
+    left neighbour's ghosts) and x >= hi - r_list (the right neighbour's), compared in fp64 (mode 1)."""
+    (low, high), _ = _slab_plan(1, pos, None, box, rank, world, width, 0.0, r_list, 2)
+    return low, high
 
 
 # --------------------------------------------------------------------------- #

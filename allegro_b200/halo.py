@@ -20,6 +20,8 @@ generate deterministically, so set-up needs no communication.
 """
 from __future__ import annotations
 
+import math
+import time
 from typing import Callable, Dict, List, Optional, Tuple
 
 import torch
@@ -177,11 +179,14 @@ class P2PHalo:
     ``atomic_virial=True`` allocates the extended mailbox (AB2_P2P_EXT_VIRIAL): reverse rows that carry the per-atom virial
     next to the gradient (``reverse_w``) and a vector all-reduce (``reduce``) for energy, virial and heat current.  Peers
     compute offsets into each other's mailboxes from the layout, so every rank must pass the same flag: it is compared
-    across ranks before anything is allocated, and a mismatch raises ValueError on every rank."""
+    across ranks before anything is allocated, and a mismatch raises ValueError on every rank.
+
+    ``headroom`` >= 1 sizes the mailbox for that many times the rows the plan needs now (1: exactly, the static case).  A
+    changing plan is re-bound with ``rebind``; ``close`` releases the mailbox.  Both are collective."""
 
     VEC_MAX = 16  # AB2_P2P_VEC_MAX
 
-    def __init__(self, dec: SlabDecomposition, device, atomic_virial: bool = False):
+    def __init__(self, dec: SlabDecomposition, device, atomic_virial: bool = False, headroom: float = 1.0):
         import ctypes as C
 
         from . import _lib
@@ -189,37 +194,14 @@ class P2PHalo:
         self._lib, self._C = _lib, C
         self.dec, self.dev = dec, torch.device(device)
         self.extended = bool(atomic_virial)
-        lib = _lib.load()
         world, rank = dec.world, dec.rank
         # max of (flag, -flag) over the ranks: they agree iff max == min (one all-reduce, any backend)
         fl = torch.tensor([int(self.extended), -int(self.extended)], dtype=torch.int32, device=self.dev)
         dist.all_reduce(fl, op=dist.ReduceOp.MAX)
         if int(fl[0]) != -int(fl[1]):
             raise ValueError("P2PHalo: ranks disagree on atomic_virial; the mailbox layout must be the same on every rank")
-        mx = torch.tensor([max(int(dec.send_right_idx.shape[0]), int(dec.send_left_idx.shape[0]), dec.n_ghost_left, dec.n_ghost_right, 1)],
-                          device=self.dev)
-        dist.all_reduce(mx, op=dist.ReduceOp.MAX)
-        self.max_rows = int(mx)
-        if self.extended:
-            nbytes = int(lib.ab2_p2p_mailbox_bytes_ex(self.max_rows, world, 1))
-        else:
-            nbytes = int(lib.ab2_p2p_mailbox_bytes(self.max_rows, world))
-        ptr = C.c_void_p()
-        _lib._check(lib.ab2_p2p_alloc(nbytes, C.byref(ptr)))
-        self.mailbox = ptr.value
-        hbuf = C.create_string_buffer(64)
-        _lib._check(lib.ab2_p2p_get_handle(C.c_void_p(self.mailbox), hbuf))
-        handles = [None] * world
-        dist.all_gather_object(handles, bytes(hbuf.raw))
-        self.peers = []
-        for r, h in enumerate(handles):
-            if r == rank:
-                self.peers.append(self.mailbox)
-            else:
-                q = C.c_void_p()
-                _lib._check(lib.ab2_p2p_open_handle(C.create_string_buffer(h, 64), C.byref(q)))
-                self.peers.append(q.value)
-        self.peers_dev = torch.tensor(self.peers, dtype=torch.int64, device=self.dev)
+        self.mailbox, self.peers, self.n_grown, self._err_before = None, [], 0, 0
+        self._open(self._with_headroom(self._rows_needed(dec), headroom))
         self.step = torch.zeros(1, dtype=torch.int32, device=self.dev)
         self.done = torch.zeros(4, dtype=torch.int32, device=self.dev)
         self.e_tot = torch.zeros(1, dtype=torch.float64, device=self.dev)
@@ -232,6 +214,79 @@ class P2PHalo:
         self.shift_to_left = dec.Lx if rank == 0 else 0.0
         torch.cuda.synchronize(self.dev)
         dist.barrier()
+
+    def _rows_needed(self, dec) -> int:
+        """the longest send or ghost list of any rank (one all-reduce MAX)"""
+        mx = torch.tensor([max(int(dec.send_right_idx.shape[0]), int(dec.send_left_idx.shape[0]), dec.n_ghost_left, dec.n_ghost_right, 1)],
+                          device=self.dev)
+        dist.all_reduce(mx, op=dist.ReduceOp.MAX)
+        return int(mx)
+
+    @staticmethod
+    def _with_headroom(rows: int, headroom: float) -> int:
+        if not headroom >= 1.0:
+            raise ValueError(f"P2PHalo: headroom must be >= 1, got {headroom}")
+        return max(rows, int(math.ceil(rows * headroom)))
+
+    def _open(self, max_rows: int):
+        """allocate my mailbox for ``max_rows`` rows and map every peer's (all ranks, same max_rows)"""
+        C, lib = self._C, self._lib.load()
+        self.max_rows = int(max_rows)
+        world, rank = self.dec.world, self.dec.rank
+        if self.extended:
+            nbytes = int(lib.ab2_p2p_mailbox_bytes_ex(self.max_rows, world, 1))
+        else:
+            nbytes = int(lib.ab2_p2p_mailbox_bytes(self.max_rows, world))
+        ptr = C.c_void_p()
+        self._lib._check(lib.ab2_p2p_alloc(nbytes, C.byref(ptr)))
+        self.mailbox = ptr.value
+        hbuf = C.create_string_buffer(64)
+        self._lib._check(lib.ab2_p2p_get_handle(C.c_void_p(self.mailbox), hbuf))
+        handles = [None] * world
+        dist.all_gather_object(handles, bytes(hbuf.raw))
+        self.peers = []
+        for r, h in enumerate(handles):
+            if r == rank:
+                self.peers.append(self.mailbox)
+            else:
+                q = C.c_void_p()
+                self._lib._check(lib.ab2_p2p_open_handle(C.create_string_buffer(h, 64), C.byref(q)))
+                self.peers.append(q.value)
+        self.peers_dev = torch.tensor(self.peers, dtype=torch.int64, device=self.dev)
+
+    def _release(self):
+        """unmap the peers' mailboxes and free mine, once no rank has a step in flight (collective)"""
+        lib, C = self._lib.load(), self._C
+        torch.cuda.synchronize(self.dev)
+        self._err_before = max(self._err_before, self.error())
+        dist.barrier()  # every rank's last step is complete: nothing is stored into any mailbox any more
+        for r, p in enumerate(self.peers):
+            if r != self.dec.rank:
+                self._lib._check(lib.ab2_p2p_close_handle(C.c_void_p(p)))
+        dist.barrier()  # no peer maps my mailbox any more
+        self._lib._check(lib.ab2_p2p_free(C.c_void_p(self.mailbox)))
+        self.mailbox, self.peers, self.peers_dev = None, [], None
+
+    def rebind(self, dec: SlabDecomposition, headroom: float = 1.0):
+        """Point the exchanges at a new plan of the same ranks (new send lists and ghost counts).  The rows it needs are
+        agreed with one all-reduce MAX; when they exceed the mailbox, every rank re-allocates for ``headroom`` times that
+        (peers re-mapped, step counter kept).  Collective: every rank calls it, between steps."""
+        need = self._rows_needed(dec)
+        self.dec = dec
+        self.send_right = dec.send_right_idx.to(self.dev).contiguous()
+        self.send_left = dec.send_left_idx.to(self.dev).contiguous()
+        self.pos_local = None
+        if need > self.max_rows:
+            self._release()
+            self._open(self._with_headroom(need, headroom))
+            self.n_grown += 1
+            torch.cuda.synchronize(self.dev)
+            dist.barrier()
+
+    def close(self):
+        """Close the peers' IPC handles and free my mailbox (collective; the halo is unusable afterwards)."""
+        if self.mailbox is not None:
+            self._release()
 
     def _ptr(self, t, row_offset=0):
         return self._C.c_void_p(t.data_ptr() + row_offset * 3 * t.element_size())
@@ -337,7 +392,11 @@ class P2PHalo:
         return self.e_tot
 
     def error(self) -> int:
-        return int(self._lib.load().ab2_p2p_error(self._C.c_void_p(self.mailbox), self.max_rows, self.dec.world, self._lib._stream()))
+        """the mailbox's error word (1: a wait timed out), including that of any mailbox a ``rebind`` replaced"""
+        if self.mailbox is None:
+            return self._err_before
+        now = int(self._lib.load().ab2_p2p_error(self._C.c_void_p(self.mailbox), self.max_rows, self.dec.world, self._lib._stream()))
+        return max(now, self._err_before)
 
 
 class DistributedAllegro:
@@ -401,6 +460,13 @@ class DistributedAllegro:
         if not self.has_flags:
             e_tot, f, e_atoms = self(pos_owned)
             return {D.TOTAL_ENERGY_KEY: e_tot, D.FORCE_KEY: f, D.PER_ATOM_ENERGY_KEY: e_atoms}
+        return self._evaluate_vec(pos_owned, velocities)
+
+    def _evaluate_vec(self, pos_owned: torch.Tensor, velocities: Optional[torch.Tensor], extra: Optional[torch.Tensor] = None) -> D.Type:
+        """``evaluate`` through the one fp64 vector reduction, whatever the flags (a model with ``energy_and_forces``).
+        ``extra`` (at most 3 values) rides in slots 13.. of that reduction and comes back summed over the ranks as
+        ``res["extra"]``."""
+        dec = self.dec
         data = self._local_data(pos_owned)
         data[D.POSITIONS_KEY] = data[D.POSITIONS_KEY].detach()
         out = self.model.energy_and_forces(data, stress=self.stress, atomic_virial=self.atomic_virial)
@@ -436,6 +502,8 @@ class DistributedAllegro:
             parts.append(J.double().reshape(3))
         else:
             parts.append(e_local.new_zeros(3, dtype=torch.float64))
+        if extra is not None:
+            parts.append(extra.detach().double().reshape(-1))
         vec = torch.cat(parts)
         if self.p2p is not None:
             tot = self.p2p.reduce(vec).clone()
@@ -452,6 +520,8 @@ class DistributedAllegro:
             res[D.ATOMIC_VIRIAL_KEY] = W_owned
         if self.heat_current:
             res[D.HEAT_CURRENT_KEY] = tot[10:13].view(1, 3).to(dt)
+        if extra is not None:
+            res["extra"] = tot[13:]
         return res
 
     def __call__(self, pos_owned: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
@@ -536,3 +606,351 @@ class GraphedDistributedAllegro:
         self.graph.replay()
         self._lib.PROF.launches += self.launches_per_replay
         return self.out
+
+
+# ---- molecular dynamics on several GPUs -------------------------------------------------------------------------------
+
+# a grown mailbox holds this many times the rows the rebuild that grew it needed (fewer re-allocations on a drifting plan)
+MAILBOX_HEADROOM = 1.25
+
+
+class _SlabPlan(SlabDecomposition):
+    """The exchange plan of one rank built by ``DistributedCalculator``'s rebuild from the rank's own atoms: the
+    attributes of a ``SlabDecomposition`` (so its torch.distributed exchanges, ``P2PHalo`` and ``DistributedAllegro``
+    take it unchanged), with the local neighbour list built for ``r_list = r_max + skin``."""
+
+    def __init__(self, rank, world, Lx, cell, ids, types, send_left_idx, send_right_idx, ghost_ids_left, ghost_ids_right, ghost_types):
+        self.rank, self.world, self.Lx = rank, world, float(Lx)
+        self.left, self.right = (rank - 1) % world, (rank + 1) % world
+        self.owned = ids
+        self.n_owned = int(ids.shape[0])
+        self.send_right_idx, self.send_left_idx = send_right_idx, send_left_idx
+        self.n_ghost_left, self.n_ghost_right = int(ghost_ids_left.shape[0]), int(ghost_ids_right.shape[0])
+        self.n_ghost = self.n_ghost_left + self.n_ghost_right
+        self.ghost_global = torch.cat([ghost_ids_left, ghost_ids_right])
+        self.shift_left = -self.Lx if rank == 0 else 0.0
+        self.shift_right = self.Lx if rank == world - 1 else 0.0
+        self.types_local = torch.cat([types, ghost_types])
+        self.global_ids_local = torch.cat([ids, self.ghost_global])
+        self.cell = cell
+        self.pbc = (False, True, True)
+        self.csr = self.shift_vec = self.edge_index = self.edge_cell_shift = None
+        self.n_edges = 0
+
+    def build_list(self, pos_local: torch.Tensor, r_list: float):
+        """neighbour list of the owned centres over owned + ghost atoms, x open, y and z periodic"""
+        if pos_local.is_cuda:
+            self.csr, self.shift_vec = D.neighbor_csr(pos_local, r_list, self.cell, self.pbc, n_centres=self.n_owned)
+            self.n_edges = self.csr.num_edges
+        else:  # CPU (the gloo tests): the pair search, rows of owned centres only
+            ei, sh = D.neighbor_list(pos_local, r_list, self.cell, self.pbc)
+            keep = ei[0] < self.n_owned
+            self.edge_index, self.edge_cell_shift = ei[:, keep].contiguous(), sh[keep].contiguous()
+            self.n_edges = int(self.edge_index.shape[1])
+
+
+class LocalAtoms:
+    """The atoms one rank owns: ``pos`` [n,3] (wrapped into the box at the last rebuild, unwrapped since), ``types`` [n],
+    ``ids`` [n] int64 (index in the global frame), ``image`` [n,3] int32 (boxes removed by wrapping: the unwrapped
+    position is pos + image * box) and ``arrays`` {name: [n, ...]} (velocities, masses, ... of the same atoms).
+    ``DistributedCalculator.compute`` may replace all of them together (re-partition)."""
+
+    def __init__(self, pos, types, ids, image, arrays):
+        self.pos, self.types, self.ids, self.image, self.arrays = pos, types, ids, image, arrays
+
+    def __len__(self):
+        return int(self.pos.shape[0])
+
+
+class _MDStep:
+    """the step ``GraphedDistributedAllegro`` captures: the model on the skin list plus the rebuild check, in one
+    vector reduction"""
+
+    has_flags = True
+
+    def __init__(self, calc: "DistributedCalculator"):
+        self.calc = calc
+
+    def evaluate(self, pos_owned, velocities=None):
+        return self.calc._step(pos_owned, velocities)
+
+
+class DistributedCalculator:
+    """Molecular dynamics on several GPUs: a 1-D slab decomposition along x that follows the trajectory.
+
+    Every rank keeps a neighbour list of its owned centres built with ``r_list = r_max + skin`` over its atoms and the
+    ghosts within ``r_list`` of its two faces.  Between rebuilds a step is one CUDA graph replay -- forward halo, the
+    model on the skin list, reverse halo, and one fp64 vector reduction that carries the energy, virial and heat current
+    and also the number of owned atoms that moved more than ``skin / 2`` since the last rebuild.  The host reads that
+    number (8 bytes) after every step; if any rank has such an atom, the step's outputs are discarded, every rank
+    rebuilds at the current positions and the step is recomputed, so no force ever comes from a stale list.
+
+    A rebuild, on every rank in the same order: wrap positions into the box and classify each owned atom by its slab
+    (ab2_slab_plan, mode 0); refuse atoms that jumped more than a slab (ValueError on every rank, agreed by one
+    all-reduce before any exchange); migrate the emigrants to the adjacent ranks (torch.distributed, staged through the
+    host on gloo; new owned order = stayers in their old order, then arrivals from the left, then from the right); select
+    the ghosts (mode 1) and exchange their ids, types and positions; build the neighbour list; re-bind (and, when it is
+    too small, re-allocate) the peer-memory mailbox; re-capture the step graph.
+
+    ``transport``: "p2p" (P2PHalo, extended mailbox: the step always uses the vector reduction) or "nccl" (the
+    torch.distributed exchanges of SlabDecomposition, whatever the backend: gloo on CPU).  ``stress`` /
+    ``heat_current`` as in ``DistributedAllegro`` (heat_current implies the per-atom virial and needs a "velocities"
+    array).  The cell is fixed for the calculator's lifetime.  Set-up refuses (ValueError, on every rank, since every
+    rank checks the same arguments) a cell that is not orthorhombic and slabs thinner than ``r_max + skin`` (ghosts then
+    come from adjacent slabs only), and a model without ``energy_and_forces`` (NotImplementedError)."""
+
+    def __init__(self, model, cell: torch.Tensor, r_max: float, skin: float = 0.5, rank: int = 0, world: int = 1, device=None,
+                 transport: str = "p2p", stress: bool = False, heat_current: bool = False, use_graph: bool = True, warmup: int = 2):
+        inner = getattr(model, "model", model)
+        if not hasattr(inner, "energy_and_forces"):
+            raise NotImplementedError("DistributedCalculator needs a model with energy_and_forces (the fused CUDA model)")
+        if transport not in ("p2p", "nccl"):
+            raise ValueError(f"transport must be 'p2p' or 'nccl', got {transport!r}")
+        if world < 2:
+            raise ValueError("DistributedCalculator needs world >= 2 (use AllegroCalculator on one GPU)")
+        if not skin >= 0.0:
+            raise ValueError(f"skin must be >= 0, got {skin}")
+        c = cell.detach().reshape(3, 3).double().cpu()
+        if not bool((c - torch.diag(torch.diagonal(c))).abs().max() == 0) or not bool((torch.diagonal(c) > 0).all()):
+            raise ValueError("DistributedCalculator: the slab decomposition needs an orthorhombic cell with positive lengths")
+        self.box = [float(v) for v in torch.diagonal(c)]
+        self.r_max, self.skin = float(r_max), float(skin)
+        self.r_list = self.r_max + self.skin
+        self.width = self.box[0] / world
+        if self.width < self.r_list:
+            raise ValueError(f"DistributedCalculator: slab width Lx / world = {self.width:.4g} is below r_max + skin = {self.r_list:.4g}: "
+                             "ghosts would come from beyond the adjacent slabs; use fewer ranks or a smaller skin")
+        self.model, self.rank, self.world = inner, int(rank), int(world)
+        self.dev = torch.device(device) if device is not None else torch.device("cpu")
+        self.transport = transport
+        self.stress, self.heat_current = bool(stress), bool(heat_current)
+        self.use_graph = bool(use_graph) and self.dev.type == "cuda"
+        self.warmup = int(warmup)
+        self._cell_arg = cell.detach().reshape(3, 3).clone()
+        self.cell = None
+        self.p2p: Optional[P2PHalo] = None
+        self.runner: Optional[DistributedAllegro] = None
+        self.plan: Optional[_SlabPlan] = None
+        self._graphed = None
+        self._ref = None
+        self._thr2 = (0.5 * self.skin) ** 2
+        self._stage_cpu = dist.get_backend() == "gloo"
+        self.n_rebuilds = self.n_redone = self.n_steps = 0
+        self.n_sent_left = self.n_sent_right = 0  # emigrants this rank sent, over the run
+        self.rebuild_seconds = {"plan": 0.0, "migration": 0.0, "ghosts": 0.0, "neighbour_list": 0.0, "capture": 0.0}
+
+    # ---- set-up ------------------------------------------------------------------------------------------------------
+    def distribute(self, pos: torch.Tensor, types: torch.Tensor, **arrays: torch.Tensor) -> LocalAtoms:
+        """The atoms of this rank's slab, from a global frame every rank holds (set-up only: the one time a rank reads
+        the whole frame).  Keyword arrays ([N, ...], e.g. velocities=v, masses=m) travel with their atoms.  Builds the
+        first plan, neighbour list and step graph (collective)."""
+        n = pos.shape[0]
+        if types.shape[0] != n or any(a.shape[0] != n for a in arrays.values()):
+            raise ValueError("distribute: types and every array need one row per atom")
+        if self.heat_current and (D.VELOCITY_KEY not in arrays or tuple(arrays[D.VELOCITY_KEY].shape) != (n, 3)):
+            raise ValueError(f"heat_current=True needs a `{D.VELOCITY_KEY}` array of shape ({n}, 3)")
+        self.cell = self._cell_arg.to(self.dev, pos.dtype)
+        p = pos.detach().to(self.dev).clone().contiguous()
+        image = torch.zeros(n, 3, dtype=torch.int32, device=self.dev)
+        from . import _lib
+
+        mine, _, _, _ = _lib.slab_wrap_classify(p, image, self.box, self.rank, self.world, self.width)
+        sel = mine.to(p.device)
+        local = LocalAtoms(p.index_select(0, sel), types.to(self.dev).index_select(0, sel), sel.clone(), image.index_select(0, sel),
+                           {k: v.detach().to(self.dev).index_select(0, sel).contiguous() for k, v in arrays.items()})
+        self._rebuild(local)
+        return local
+
+    # ---- per step ----------------------------------------------------------------------------------------------------
+    def _step(self, pos_owned, velocities):
+        moved = ((pos_owned - self._ref).square().sum(-1) > self._thr2).sum().reshape(1)
+        return self.runner._evaluate_vec(pos_owned, velocities, extra=moved)
+
+    def _run(self, local: LocalAtoms):
+        vel = local.arrays.get(D.VELOCITY_KEY) if self.heat_current else None
+        if self._graphed is not None:
+            out = self._graphed(local.pos, vel)
+        else:
+            with torch.no_grad():
+                out = self._step(local.pos, vel)
+        return out, float(out["extra"][0])  # the one 8-byte device-to-host read of the step
+
+    def compute(self, local: LocalAtoms, cell: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
+        """One force evaluation at ``local.pos`` (collective).  -> ``total_energy`` [1] (fp64, every rank), ``forces``
+        [n,3], ``atomic_energy`` [n,1]; with the flags also ``stress`` and ``virial`` [1,3,3], ``atomic_virial`` [n,3,3] and
+        ``heat_current`` [1,3] (from ``local.arrays["velocities"]``).
+
+        If an atom moved more than skin / 2 since the last rebuild, this call re-partitions: ``local.pos``, ``types``,
+        ``ids``, ``image`` and ``arrays`` are replaced by new tensors (atoms may have left or arrived), and the outputs
+        are in the row order of ``local`` after the call.  So a caller must read them from ``local`` again after each
+        call and must not keep references to the old tensors.  The outputs are the step's buffers: the next call
+        overwrites them.  A cell other than the one given at construction raises ValueError."""
+        if cell is not None and not torch.equal(cell.detach().reshape(3, 3).to(self._cell_arg.device, self._cell_arg.dtype), self._cell_arg):
+            raise ValueError("DistributedCalculator: the cell is fixed for the calculator's lifetime")
+        if self.runner is None:
+            raise RuntimeError("DistributedCalculator.compute before distribute")
+        out, moved = self._run(local)
+        if moved > 0:
+            # the list may miss a pair: discard, rebuild everywhere at the current positions, redo the step
+            self.n_redone += 1
+            self._rebuild(local)
+            out, moved = self._run(local)
+        self.n_steps += 1
+        return {k: v for k, v in out.items() if k != "extra"}
+
+    # ---- rebuild -----------------------------------------------------------------------------------------------------
+    def _comm(self, t: torch.Tensor) -> torch.Tensor:
+        return t.cpu() if self._stage_cpu else t
+
+    def _neighbours(self, to_right: torch.Tensor, to_left: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        """float64 rows [m, k] to the right and to the left neighbour -> (rows from the left one, rows from the right
+        one), counts first; in the canonical peer order of SlabDecomposition._peers (world 2: one peer, right-going
+        rows first)."""
+        k = to_right.shape[1]
+        left, right = (self.rank - 1) % self.world, (self.rank + 1) % self.world
+        sr, sl = self._comm(to_right), self._comm(to_left)
+
+        def swap(send_r, send_l, n_from_l, n_from_r, make):
+            if left == right:
+                rbuf = make(n_from_l + n_from_r)
+                ops = [dist.P2POp(dist.isend, torch.cat([send_r, send_l]).contiguous(), right), dist.P2POp(dist.irecv, rbuf, right)]
+                for w in dist.batch_isend_irecv(ops):
+                    w.wait()
+                return rbuf[:n_from_l], rbuf[n_from_l:]
+            rl, rr = make(n_from_l), make(n_from_r)
+            ops = [dist.P2POp(dist.isend, send_r.contiguous(), right), dist.P2POp(dist.irecv, rr, right),
+                   dist.P2POp(dist.isend, send_l.contiguous(), left), dist.P2POp(dist.irecv, rl, left)]
+            for w in dist.batch_isend_irecv(ops):
+                w.wait()
+            return rl, rr
+
+        dev = sr.device
+        cnt = lambda m: torch.empty(m, dtype=torch.int64, device=dev)  # noqa: E731
+        c_l, c_r = swap(torch.tensor([sr.shape[0]], device=dev), torch.tensor([sl.shape[0]], device=dev), 1, 1, cnt)
+        n_l, n_r = int(c_l[0]), int(c_r[0])
+        # one padding row each way: no empty message on any backend
+        pad = lambda t: torch.cat([t, t.new_zeros(1, k)])  # noqa: E731
+        rows = lambda m: torch.empty(m, k, dtype=torch.float64, device=dev)  # noqa: E731
+        gl, gr = swap(pad(sr), pad(sl), n_l + 1, n_r + 1, rows)
+        return gl[:n_l].to(self.dev), gr[:n_r].to(self.dev)
+
+    def _allreduce_max(self, v: int) -> int:
+        t = self._comm(torch.tensor([int(v)], dtype=torch.int64, device=self.dev))
+        dist.all_reduce(t, op=dist.ReduceOp.MAX)
+        return int(t[0])
+
+    def _pack(self, local: LocalAtoms, idx: torch.Tensor) -> torch.Tensor:
+        """rows of the atoms idx as float64: pos, image, type, id, then every array flattened (exact for fp32 / fp64
+        values, int32 images and ids below 2^53)"""
+        m = int(idx.shape[0])
+        cols = [local.pos.index_select(0, idx).double(), local.image.index_select(0, idx).double(),
+                local.types.index_select(0, idx).double().reshape(m, 1), local.ids.index_select(0, idx).double().reshape(m, 1)]
+        for k in sorted(local.arrays):
+            a = local.arrays[k]
+            cols.append(a.index_select(0, idx).double().reshape(m, int(math.prod(a.shape[1:]))))
+        return torch.cat(cols, 1)
+
+    def _unpack(self, local: LocalAtoms, rows: torch.Tensor):
+        m = int(rows.shape[0])
+        out = [rows[:, 0:3].to(local.pos.dtype), rows[:, 3:6].to(torch.int32), rows[:, 6].to(local.types.dtype), rows[:, 7].to(torch.int64)]
+        o, arrs = 8, {}
+        for k in sorted(local.arrays):
+            a = local.arrays[k]
+            w = int(math.prod(a.shape[1:]))
+            arrs[k] = rows[:, o : o + w].to(a.dtype).reshape((m,) + tuple(a.shape[1:]))
+            o += w
+        return out, arrs
+
+    def _rebuild(self, local: LocalAtoms):
+        from . import _lib
+
+        sync = (lambda: torch.cuda.synchronize(self.dev)) if self.dev.type == "cuda" else (lambda: None)
+        self._graphed = None
+        t0 = time.perf_counter()
+        # 1. wrap and classify (one read of the counts)
+        stay, to_left, to_right, n_far = _lib.slab_wrap_classify(local.pos, local.image, self.box, self.rank, self.world, self.width,
+                                                                 jump=self.width)
+        # 2. an atom bound for a non-adjacent slab: agreed first, so every rank raises and nobody waits on an exchange
+        far = self._allreduce_max(n_far)
+        if far > 0:
+            raise ValueError(f"DistributedCalculator: an atom moved more than one slab width ({self.width:.4g}) since the last "
+                             "rebuild; the time step or the skin is too large")
+        t1 = time.perf_counter()
+        self.rebuild_seconds["plan"] += t1 - t0
+        # 3. migrate: stayers in their old order, then arrivals from the left, then from the right
+        self.n_sent_left += int(to_left.shape[0])
+        self.n_sent_right += int(to_right.shape[0])
+        from_l, from_r = self._neighbours(self._pack(local, to_right), self._pack(local, to_left))
+        (pl, il, tl, dl), al = self._unpack(local, from_l)
+        (pr, ir, tr, dr), ar = self._unpack(local, from_r)
+        local.pos = torch.cat([local.pos.index_select(0, stay), pl, pr]).contiguous()
+        local.image = torch.cat([local.image.index_select(0, stay), il, ir]).contiguous()
+        local.types = torch.cat([local.types.index_select(0, stay), tl, tr]).contiguous()
+        local.ids = torch.cat([local.ids.index_select(0, stay), dl, dr]).contiguous()
+        local.arrays = {k: torch.cat([v.index_select(0, stay), al[k], ar[k]]).contiguous() for k, v in local.arrays.items()}
+        t2 = time.perf_counter()
+        self.rebuild_seconds["migration"] += t2 - t1
+        # 4. ghosts: my atoms within r_list of the low face go to the left neighbour, of the high face to the right one
+        low, high = _lib.slab_faces(local.pos, self.box, self.rank, self.world, self.width, self.r_list)
+
+        def ghost_rows(idx):
+            m = int(idx.shape[0])
+            return torch.cat([local.pos.index_select(0, idx).double(), local.types.index_select(0, idx).double().reshape(m, 1),
+                              local.ids.index_select(0, idx).double().reshape(m, 1)], 1)
+
+        g_l, g_r = self._neighbours(ghost_rows(high), ghost_rows(low))
+        shift_left = -self.box[0] if self.rank == 0 else 0.0
+        shift_right = self.box[0] if self.rank == self.world - 1 else 0.0
+        g_l[:, 0] += shift_left
+        g_r[:, 0] += shift_right
+        # ghost rows: pos (3), type, id
+        plan = _SlabPlan(self.rank, self.world, self.box[0], self.cell, local.ids, local.types, low, high, g_l[:, 4].to(torch.int64),
+                         g_r[:, 4].to(torch.int64), torch.cat([g_l[:, 3], g_r[:, 3]]).to(local.types.dtype))
+        pos_ghost = torch.cat([g_l[:, :3], g_r[:, :3]]).to(local.pos.dtype)
+        if self.transport == "p2p":
+            if self.p2p is None:
+                self.p2p = P2PHalo(plan, self.dev, atomic_virial=True, headroom=MAILBOX_HEADROOM)
+            else:
+                self.p2p.rebind(plan, headroom=MAILBOX_HEADROOM)
+        sync()
+        t3 = time.perf_counter()
+        self.rebuild_seconds["ghosts"] += t3 - t2
+        # 5. neighbour list on owned + ghosts with r_max + skin, rows for the owned centres
+        plan.build_list(torch.cat([local.pos, pos_ghost]).contiguous(), self.r_list)
+        self.plan = plan
+        self.runner = DistributedAllegro(self.model, plan, p2p=self.p2p, stress=self.stress, atomic_virial=self.heat_current,
+                                         heat_current=self.heat_current)
+        self._ref = local.pos.detach().clone()
+        self.n_rebuilds += 1
+        sync()
+        t4 = time.perf_counter()
+        self.rebuild_seconds["neighbour_list"] += t4 - t3
+        # 6. re-capture the step
+        if self.use_graph:
+            vel = local.arrays.get(D.VELOCITY_KEY) if self.heat_current else None
+            self._graphed = GraphedDistributedAllegro(_MDStep(self), local.pos, warmup=self.warmup, velocities=vel)
+        self.rebuild_seconds["capture"] += time.perf_counter() - t4
+
+    # ---- output ------------------------------------------------------------------------------------------------------
+    def gather(self, local: LocalAtoms) -> Optional[Dict[str, torch.Tensor]]:
+        """The whole frame on rank 0, in global-id order (trajectory output; collective, through the host): ``pos``
+        [N,3] fp64 unwrapped (pos + image * box), ``image``, ``types``, ``ids`` and every array, as CPU tensors.  None on
+        the other ranks."""
+        box = torch.tensor(self.box, dtype=torch.float64, device=local.pos.device)
+        mine = {"pos": (local.pos.double() + local.image.double() * box).cpu(), "image": local.image.cpu(), "types": local.types.cpu(),
+                "ids": local.ids.cpu()}
+        mine.update({k: v.detach().cpu() for k, v in local.arrays.items()})
+        got = [None] * self.world if self.rank == 0 else None
+        dist.gather_object(mine, got, dst=0)
+        if self.rank != 0:
+            return None
+        frame = {k: torch.cat([g[k] for g in got]) for k in mine}
+        order = torch.argsort(frame["ids"])
+        return {k: v.index_select(0, order) for k, v in frame.items()}
+
+    def close(self):
+        """Release the step graph and the peer-memory mailbox (collective)."""
+        self._graphed = None
+        if self.p2p is not None:
+            self.p2p.close()
+            self.p2p = None

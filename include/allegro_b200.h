@@ -491,6 +491,24 @@ int ab2_p2p_wait_unpack_w(int dst_dtype, int side, void* my_mailbox, int max_row
 int ab2_p2p_allreduce_vec(const void* v_local, int n_values, int rank, int world, int max_rows, void* const* peers_dev,
                           void* my_mailbox, const void* step_counter, void* v_total, void* stream);
 
+/* Exchange plan of a 1-D slab decomposition along x, built on the device from one rank's atoms (slab rank of world,
+ * each `width` wide, lo = rank * width, hi = lo + width).  ab2_slab_plan_count writes one class byte per atom into
+ * cls[n] and per-block member counts into block_counts[ceil(n / 256)][4]; the caller turns the counts into exclusive
+ * per-list prefix sums over the blocks (block_offsets, same shape), and ab2_slab_plan_fill writes each list k (null:
+ * skipped) as int64 atom indices in ascending order, list k of block b starting at block_offsets[b][k].
+ *   mode 0: wraps pos [n][3] (fp64 / fp32, in place) into [0, box[a]) on every axis, adding the boxes removed to
+ *           image [n][3] int32, and classifies by s = clamp(floor(x / width), 0, world - 1): list 0 = stays (s == rank),
+ *           list 1 = to the left neighbour, list 2 = to the right one (world 2: by the side of [lo, hi) the atom left
+ *           by); column 3 counts refused atoms: bound for a non-adjacent slab, or with x before the wrap outside
+ *           [lo - jump, hi + jump).  Refused atoms are in no list.
+ *   mode 1: pos read only, image unused: list 0 = atoms with x < lo + r_list, list 1 = atoms with x >= hi - r_list
+ *           (compared in fp64), list 2 empty.
+ * n = 0 launches nothing.  Both launch on `stream`. */
+int ab2_slab_plan_count(int pos_dtype, int mode, int64_t n, void* pos, int32_t* image, const double* box_host, int rank, int world,
+                        double width, double jump, double r_list, uint8_t* cls, int32_t* block_counts, void* stream);
+int ab2_slab_plan_fill(int64_t n, const uint8_t* cls, const int32_t* block_offsets, int64_t* list0, int64_t* list1, int64_t* list2,
+                       void* stream);
+
 /* layout helpers between the reference strided layout [z][u][i] and the internal [z][i][u] */
 int ab2_transpose_ui(int dtype, int64_t E, int U, int d, const void* src, void* dst, int to_internal,
                      void* stream);
