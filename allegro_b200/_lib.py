@@ -74,6 +74,7 @@ _SIGNATURES = {
     "ab2_p2p_error": ([_vp, _i32, _i32, _vp], C.c_int),
     "ab2_p2p_begin": ([_vp, _vp], C.c_int),
     "ab2_p2p_push_rows": ([_i32, _i32, _i32, _vp, _vp, _i32, _dbl, _vp, _i32, _i32, _vp, _vp, _vp], C.c_int),
+    "ab2_p2p_push_rows_v": ([_i32, _i32, _i32, _vp, _vp, _i32, _dbl, _dbl, _dbl, _vp, _i32, _i32, _vp, _vp, _vp], C.c_int),
     "ab2_p2p_wait_unpack": ([_i32, _i32, _i32, _vp, _i32, _i32, _vp, _i32, _vp, _vp, _i32, _vp], C.c_int),
     "ab2_p2p_allreduce_energy": ([_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_p2p_mailbox_bytes_ex": ([_i32, _i32, _i32], C.c_int64),
@@ -82,6 +83,7 @@ _SIGNATURES = {
     "ab2_p2p_allreduce_vec": ([_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_slab_plan_count": ([_i32, _i32, _i64, _vp, _vp, _vp, _i32, _i32, _dbl, _dbl, _dbl, _vp, _vp, _vp], C.c_int),
     "ab2_slab_plan_fill": ([_i64, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_slab_plan_count_lattice": ([_i32, _i32, _i64, _vp, _vp, _vp, _i32, _i32, _dbl, _dbl, _vp, _vp, _vp], C.c_int),
     "ab2_nl_bin": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_nl_count": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_nl_fill": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
@@ -763,19 +765,30 @@ def radial_pq_bwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table,
 # slab decomposition plan (ab2_slab_plan_count / fill)
 # --------------------------------------------------------------------------- #
 def _slab_plan(mode: int, pos: torch.Tensor, image: Optional[torch.Tensor], box, rank: int, world: int, width: float, jump: float,
-               r_list: float, n_lists: int):
+               r_list: float, n_lists: int, rows=None):
     """count -> prefix sum over the blocks -> fill; -> (lists [n_lists] int64, refused count).  The totals are the one
-    device-to-host read."""
+    device-to-host read.  ``rows`` (the 3x3 cell rows) selects ab2_slab_plan_count_lattice instead (``box`` and ``width``
+    unused); it checks the cell even when there are no atoms."""
     n = pos.shape[0]
+    if rows is not None:
+        rowsa = (C.c_double * 9)(*[float(v) for row in rows for v in row])
+        count = lambda cls, counts: load().ab2_slab_plan_count_lattice(  # noqa: E731
+            DTYPE_ENUM[pos.dtype], mode, n, _ptr(_contig(pos, "pos")) if n else None, _ptr(image) if n else None, rowsa, int(rank), int(world),
+            float(jump), float(r_list), _ptr(cls), _ptr(counts), _stream())
+        if n == 0:
+            _check(count(None, None))
+    else:
+        boxa = (C.c_double * 3)(*[float(b) for b in box])
+        count = lambda cls, counts: load().ab2_slab_plan_count(  # noqa: E731
+            DTYPE_ENUM[pos.dtype], mode, n, _ptr(_contig(pos, "pos")), _ptr(image), boxa, int(rank), int(world), float(width), float(jump),
+            float(r_list), _ptr(cls), _ptr(counts), _stream())
     if n == 0:
         return [torch.empty(0, dtype=torch.int64, device=pos.device) for _ in range(n_lists)], 0
     nblk = (n + 255) // 256
     cls = torch.empty(n, dtype=torch.uint8, device=pos.device)
     counts = torch.empty(nblk, 4, dtype=torch.int32, device=pos.device)
-    boxa = (C.c_double * 3)(*[float(b) for b in box])
     with _timed("slab_plan_count"):
-        _check(load().ab2_slab_plan_count(DTYPE_ENUM[pos.dtype], mode, n, _ptr(_contig(pos, "pos")), _ptr(image), boxa, int(rank), int(world),
-                                          float(width), float(jump), float(r_list), _ptr(cls), _ptr(counts), _stream()))
+        _check(count(cls, counts))
     incl = torch.cumsum(counts, 0, dtype=torch.int32)
     offsets = (incl - counts).contiguous()
     lists = [torch.empty(n, dtype=torch.int64, device=pos.device) for _ in range(n_lists)]
@@ -800,6 +813,24 @@ def slab_faces(pos: torch.Tensor, box, rank: int, world: int, width: float, r_li
     """Atoms of the slab within ``r_list`` of its faces -> (low, high): ascending int64 index lists of x < lo + r_list (the
     left neighbour's ghosts) and x >= hi - r_list (the right neighbour's), compared in fp64 (mode 1)."""
     (low, high), _ = _slab_plan(1, pos, None, box, rank, world, width, 0.0, r_list, 2)
+    return low, high
+
+
+def slab_wrap_classify_lattice(pos: torch.Tensor, image: torch.Tensor, rows, rank: int, world: int, jump: float = float("inf")):
+    """``slab_wrap_classify`` for any regular cell with rows ``rows`` [3][3], cut along lattice row 0 in fractional
+    coordinates s = pos . h^-1: wrap on all three axes (img_a = floor(s_a), pos -= sum_a img_a h_a in fp64, rounded once;
+    image += img), classify by clamp(floor(s_0 world), 0, world - 1) -> (stay, to_left, to_right, n_refused); refused:
+    a non-adjacent slab, or an unwrapped s_0 outside [lo - jump, hi + jump), ``jump`` in fractional units
+    (ab2_slab_plan_count_lattice / ab2_slab_plan_fill, mode 0).  A singular or non-finite cell raises before any launch."""
+    assert image.dtype == torch.int32 and image.shape == pos.shape
+    (stay, left, right), refused = _slab_plan(0, pos, _contig(image, "image"), None, rank, world, 0.0, jump, 0.0, 3, rows=rows)
+    return stay, left, right, refused
+
+
+def slab_faces_lattice(pos: torch.Tensor, rows, rank: int, world: int, r_list: float):
+    """``slab_faces`` for any regular cell: (low, high) = atoms with s_0 < lo + r_list / H_0 and s_0 >= hi - r_list / H_0,
+    H_0 = |det h| / |h_1 x h_2| the height of the cell along row 0 (fp64; mode 1)."""
+    (low, high), _ = _slab_plan(1, pos, None, None, rank, world, 0.0, 0.0, r_list, 2, rows=rows)
     return low, high
 
 

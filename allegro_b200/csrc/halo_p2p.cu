@@ -21,6 +21,8 @@
 //   [parity][side] reverse rows of width 12 (3 gradient + 9 per-atom virial values, fp64; 12 * max_rows doubles)
 //   [parity][rank] a vector of up to AB2_P2P_VEC_MAX doubles (energy, virial, heat current)
 //   flags: wrows[parity][side], vec[parity][rank]
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace {
@@ -81,19 +83,30 @@ __global__ void p2p_begin_kernel(uint32_t* step) { *step += 1; }
 
 // kind 0: positions (x shifted), 1: gradients.  rows src[idx[i]] (or src[i]) -> the PEER's mailbox slot `side` of the
 // current step's parity, then publish the step number (last block, after a system-scope fence).
-template <typename TSrc>
+// VEC = true (ab2_p2p_push_rows_v): the shift is a vector (a lattice row of a triclinic cell), added to all three components
+struct Shift3 {
+    double v[3];
+};
+
+template <typename TSrc, bool VEC>
 __global__ void __launch_bounds__(256) p2p_push_rows_kernel(MailboxLayout L, int kind, int side, const TSrc* __restrict__ src,
-                                                            const int64_t* __restrict__ idx, int n, double shift_x, uint8_t* __restrict__ peer,
-                                                            const uint32_t* __restrict__ step, uint32_t* __restrict__ done_ctr) {
+                                                            const int64_t* __restrict__ idx, int n, std::conditional_t<VEC, Shift3, double> shift_x,
+                                                            uint8_t* __restrict__ peer, const uint32_t* __restrict__ step, uint32_t* __restrict__ done_ctr) {
     const uint32_t s = *step;
     const int par = (int)(s & 1u);
     double* __restrict__ dst = reinterpret_cast<double*>(peer + (kind == 0 ? L.pos_off(par, side) : L.grad_off(par, side)));
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i < n) {
         const int64_t r = idx ? idx[i] : i;
-        dst[3 * i + 0] = (double)src[3 * r + 0] + shift_x;
-        dst[3 * i + 1] = (double)src[3 * r + 1];
-        dst[3 * i + 2] = (double)src[3 * r + 2];
+        if constexpr (VEC) {
+            dst[3 * i + 0] = (double)src[3 * r + 0] + shift_x.v[0];
+            dst[3 * i + 1] = (double)src[3 * r + 1] + shift_x.v[1];
+            dst[3 * i + 2] = (double)src[3 * r + 2] + shift_x.v[2];
+        } else {
+            dst[3 * i + 0] = (double)src[3 * r + 0] + shift_x;
+            dst[3 * i + 1] = (double)src[3 * r + 1];
+            dst[3 * i + 2] = (double)src[3 * r + 2];
+        }
     }
     __threadfence_system();
     __syncthreads();
@@ -307,11 +320,32 @@ extern "C" int ab2_p2p_push_rows(int src_dtype, int kind, int side, const void* 
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned grid = n > 0 ? ab2_blocks(n, 256) : 1;
     if (src_dtype == AB2_F64)
-        p2p_push_rows_kernel<double><<<grid, 256, 0, st>>>(L, kind, side, (const double*)src, idx, n, shift_x, (uint8_t*)peer_mailbox,
+        p2p_push_rows_kernel<double, false><<<grid, 256, 0, st>>>(L, kind, side, (const double*)src, idx, n, shift_x, (uint8_t*)peer_mailbox,
                                                           (const uint32_t*)step_counter, (uint32_t*)done_counter);
     else
-        p2p_push_rows_kernel<float><<<grid, 256, 0, st>>>(L, kind, side, (const float*)src, idx, n, shift_x, (uint8_t*)peer_mailbox,
+        p2p_push_rows_kernel<float, false><<<grid, 256, 0, st>>>(L, kind, side, (const float*)src, idx, n, shift_x, (uint8_t*)peer_mailbox,
                                                          (const uint32_t*)step_counter, (uint32_t*)done_counter);
+    AB2_CUDA_LAUNCH_CHECK();
+    return 0;
+}
+
+/* ab2_p2p_push_rows with the shift (shift_x, shift_y, shift_z) added to every component: a ghost crossing the periodic
+ * face of lattice row 0 of a triclinic cell moves by that row.  The shift is passed by value (graph-capturable). */
+extern "C" int ab2_p2p_push_rows_v(int src_dtype, int kind, int side, const void* src, const int64_t* idx, int n, double shift_x, double shift_y,
+                                   double shift_z, void* peer_mailbox, int max_rows, int world, const void* step_counter, void* done_counter,
+                                   void* stream) {
+    AB2_CHECK_ARG(src && peer_mailbox && step_counter && done_counter && n >= 0 && n <= max_rows, "bad arguments");
+    AB2_CHECK_ARG(src_dtype == AB2_F64 || src_dtype == AB2_F32, "rows must be fp64 or fp32");
+    MailboxLayout L{max_rows, world};
+    cudaStream_t st = (cudaStream_t)stream;
+    const unsigned grid = n > 0 ? ab2_blocks(n, 256) : 1;
+    const Shift3 sh{{shift_x, shift_y, shift_z}};
+    if (src_dtype == AB2_F64)
+        p2p_push_rows_kernel<double, true><<<grid, 256, 0, st>>>(L, kind, side, (const double*)src, idx, n, sh, (uint8_t*)peer_mailbox,
+                                                                (const uint32_t*)step_counter, (uint32_t*)done_counter);
+    else
+        p2p_push_rows_kernel<float, true><<<grid, 256, 0, st>>>(L, kind, side, (const float*)src, idx, n, sh, (uint8_t*)peer_mailbox,
+                                                               (const uint32_t*)step_counter, (uint32_t*)done_counter);
     AB2_CUDA_LAUNCH_CHECK();
     return 0;
 }

@@ -23,6 +23,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "lattice.cuh"
 
 namespace {
 
@@ -226,36 +227,27 @@ int nl_geom(NlGeom& g, const double* box, const double* origin, const int32_t* p
 }
 
 // Checks and completes a general-lattice grid on the host, in double / int64 before anything is launched.  The
-// inverse is computed here so that no caller can pass one inconsistent with the rows.  data.lattice_grid mirrors the
+// inverse is computed here (lattice.cuh) so that no caller can pass one inconsistent with the rows.  data.lattice_grid mirrors the
 // height and reach arithmetic operation for operation, so the grids it returns pass on the same quotients.
 int nl_lattice_geom(NlLatticeGeom& g, const double* rows, const double* origin, const int32_t* pbc, const int32_t* ncell,
                     const int32_t* reach, double r_max) {
     if (!(r_max > 0) || !std::isfinite(r_max)) return 1;
-    for (int k = 0; k < 9; ++k) {
-        if (!std::isfinite(rows[k])) return 1;
-        g.h[k / 3][k % 3] = rows[k];
-    }
-    double cr[3][3], norm[3];  // cr[a] = h[a+1] x h[a+2]: det . hinv column a
-    for (int a = 0; a < 3; ++a) {
-        const double* p = g.h[(a + 1) % 3];
-        const double* q = g.h[(a + 2) % 3];
-        cr[a][0] = p[1] * q[2] - p[2] * q[1];
-        cr[a][1] = p[2] * q[0] - p[0] * q[2];
-        cr[a][2] = p[0] * q[1] - p[1] * q[0];
-        norm[a] = std::sqrt(g.h[a][0] * g.h[a][0] + g.h[a][1] * g.h[a][1] + g.h[a][2] * g.h[a][2]);
-    }
-    const double det = g.h[0][0] * cr[0][0] + g.h[0][1] * cr[0][1] + g.h[0][2] * cr[0][2];
-    // singular (or a cell whose rows are within 1e-12 rad of a common plane)
-    if (!std::isfinite(det) || !(std::fabs(det) > 1e-12 * norm[0] * norm[1] * norm[2])) return 2;
+    Ab2Lattice lat;
+    // 1: a row is not finite; 2: singular (or a cell whose rows are within 1e-12 rad of a common plane)
+    const int bad = ab2_lattice_inverse(rows, lat);
+    if (bad) return bad;
     int64_t cells = 1, visits = 1;
     for (int a = 0; a < 3; ++a) {
         if (!std::isfinite(origin[a])) return 1;
-        for (int x = 0; x < 3; ++x) g.hinv[x][a] = cr[a][x] / det;
+        for (int x = 0; x < 3; ++x) {
+            g.h[a][x] = lat.h[a][x];
+            g.hinv[x][a] = lat.hinv[x][a];
+        }
         g.origin[a] = origin[a]; g.pbc[a] = pbc[a] != 0; g.ncell[a] = ncell[a]; g.reach[a] = reach[a];
         if (ncell[a] < 1 || reach[a] < 1) return 3;
         // bin c_a + d of the walk stays an int
         if ((int64_t)ncell[a] + reach[a] >= (int64_t)0x7fffffff) return 4;
-        const double height = std::fabs(det) / std::sqrt(cr[a][0] * cr[a][0] + cr[a][1] * cr[a][1] + cr[a][2] * cr[a][2]);
+        const double height = ab2_lattice_height(lat, a);
         if (height / ncell[a] * reach[a] < r_max * (1 - 1e-12)) return 5;  // k_a bins of thickness t_a reach r_max
         cells *= ncell[a];
         if (cells >= (int64_t)0x7fffffff) return 6;  // int32 cell ids and cell_start offsets

@@ -3,7 +3,7 @@
 Allegro is strictly local: E_i depends only on atoms within r_max of i
 (/root/reference/tests/model/test_allegro.py:68-70; the environment sum only runs over edges
 centred on i, allegro/nn/_strided/_contract.py:199-205).  So atoms are split into 1-D slabs
-along x, one per rank / GPU; each rank evaluates the edges of its OWNED centres, with
+along lattice row 0 (x for an orthorhombic box; ``SlabGeometry``), one per rank / GPU; each rank evaluates the edges of its OWNED centres, with
 neighbours taken from owned + ghost atoms in exactly the reference's ghost-atom data format
 (ghosts appended after the locals, neighbour index >= N_local,
 /root/reference/allegro/_compile.py:41-61).
@@ -30,19 +30,85 @@ import torch.distributed as dist
 from . import data as D
 
 
+class SlabGeometry:
+    """How a cell is cut into ``world`` slabs along lattice row 0: the one rule the static decomposition, the MD rebuild
+    and both transports read.  Any regular cell (``data.is_regular_cell``) is accepted; anything else raises ValueError.
+
+    * ``diagonal`` (zero off-diagonal entries, positive lengths): slabs along x of width Lx / world in length units, ghosts
+      that cross the periodic x face shifted by -+Lx along x (ab2_slab_plan_count, ab2_p2p_push_rows).
+    * Every other cell: fractional coordinates s = pos . h^-1, the inverse as nl_lattice_geom computes it.  Rank r owns
+      s_0 in [r / world, (r + 1) / world).  The slab thickness is a height, ``thickness`` = H_0 / world with
+      H_0 = |det h| / |h_1 x h_2| (not |h_0| / world): a pair closer than r has |ds_0| H_0 < r, so ghosts within r of a
+      face are the atoms with s_0 within r / H_0 of it.  A ghost that crosses the periodic face of row 0 moves by -+h_0
+      (ab2_slab_plan_count_lattice, ab2_p2p_push_rows_v).
+    The local frame of every rank is the cell h with pbc (False, True, True)."""
+
+    axis = 0
+
+    def __init__(self, cell: torch.Tensor, world: int):
+        h = cell.detach().reshape(3, 3).to(device="cpu", dtype=torch.float64)
+        self.rows = h.tolist()
+        self.world = int(world)
+        _, heights, regular = D._lattice_metrics(self.rows)
+        if not regular:
+            raise ValueError("slab decomposition: the cell is not regular (a row is not finite, or the rows are singular or within "
+                             "1e-12 rad of a common plane)")
+        self.height = heights[0]  # H_0
+        self.diagonal = bool((h - torch.diag(torch.diagonal(h))).abs().max() == 0) and bool((torch.diagonal(h) > 0).all())
+        if self.diagonal:
+            self.Lx = self.rows[0][0]
+            self.thickness = self.Lx / world
+        else:
+            self.Lx = None
+            self.thickness = self.height / world
+            cr = [D._cross(self.rows[(a + 1) % 3], self.rows[(a + 2) % 3]) for a in range(3)]
+            det = sum(self.rows[0][x] * cr[0][x] for x in range(3))
+            self.hinv = [[cr[a][x] / det for a in range(3)] for x in range(3)]  # hinv[x][a], as lattice.cuh
+
+    def frac0(self, pos: torch.Tensor) -> torch.Tensor:
+        """s_0 = (p_0 hinv[0][0] + p_1 hinv[1][0]) + p_2 hinv[2][0] in fp64 (lattice cells)"""
+        p = pos.double()
+        hi = self.hinv
+        return (p[:, 0] * hi[0][0] + p[:, 1] * hi[1][0]) + p[:, 2] * hi[2][0]
+
+    def faces(self, rank: int) -> Tuple[float, float]:
+        """(lo, hi) of the slab of ``rank``: x in length units (diagonal) or s_0"""
+        if self.diagonal:
+            return rank * self.thickness, (rank + 1) * self.thickness
+        return rank / self.world, (rank + 1) / self.world
+
+    def reach(self, r: float) -> float:
+        """a distance r across the faces, in the units of ``faces``"""
+        return float(r) if self.diagonal else float(r) / self.height
+
+    def ghost_shifts(self, rank: int):
+        """(shift of the ghosts from the left neighbour, from the right one): -+Lx (diagonal, along x) or -+h_0 (3 fp64
+        components), zero away from the periodic face"""
+        if self.diagonal:
+            return (-self.Lx if rank == 0 else 0.0), (self.Lx if rank == self.world - 1 else 0.0)
+        zero = [0.0, 0.0, 0.0]
+        return ([-v for v in self.rows[0]] if rank == 0 else zero), (list(self.rows[0]) if rank == self.world - 1 else zero)
+
+
 class SlabDecomposition:
-    """Static exchange plan of one rank (valid as long as the neighbour list is)."""
+    """Static exchange plan of one rank (valid as long as the neighbour list is), for any regular cell (``SlabGeometry``)."""
 
     def __init__(self, pos: torch.Tensor, cell: torch.Tensor, types: torch.Tensor, r_max: float, rank: int, world: int, device=None):
         assert world >= 2, "use the plain periodic path on one rank"
         cell = cell.view(3, 3)
-        assert bool((cell - torch.diag(torch.diagonal(cell))).abs().max() == 0), "slab decomposition needs an orthorhombic box"
-        Lx = float(cell[0, 0])
-        width = Lx / world
+        geo = SlabGeometry(cell, world)
+        width = geo.thickness
         assert width >= r_max, "slab thinner than r_max: neighbours beyond the adjacent slab"
-        self.rank, self.world, self.r_max, self.Lx = rank, world, float(r_max), Lx
-        x = pos[:, 0] - torch.floor(pos[:, 0] / Lx) * Lx
-        slab = torch.clamp((x / width).long(), max=world - 1)
+        self.rank, self.world, self.r_max = rank, world, float(r_max)
+        self._set_geometry(geo)
+        if geo.diagonal:
+            Lx = self.Lx
+            x = pos[:, 0] - torch.floor(pos[:, 0] / Lx) * Lx
+            slab = torch.clamp((x / width).long(), max=world - 1)
+        else:
+            x = geo.frac0(self._wrap0(pos))
+            slab = torch.clamp(torch.floor(x * world).long(), 0, world - 1)
+        reach = geo.reach(r_max)
 
         def owned_of(r):
             return torch.nonzero(slab == r).squeeze(-1)
@@ -50,8 +116,8 @@ class SlabDecomposition:
         def send_lists(r):
             ids = owned_of(r)
             xr = x[ids]
-            lo, hi = r * width, (r + 1) * width
-            return ids[xr >= hi - r_max], ids[xr < lo + r_max]  # (to the right neighbour, to the left neighbour)
+            lo, hi = geo.faces(r)
+            return ids[xr >= hi - reach], ids[xr < lo + reach]  # (to the right neighbour, to the left neighbour)
 
         self.left, self.right = (rank - 1) % world, (rank + 1) % world
         self.owned = owned_of(rank)
@@ -68,12 +134,9 @@ class SlabDecomposition:
         self.n_ghost_left, self.n_ghost_right = int(left_ids.shape[0]), int(right_ids.shape[0])
         self.ghost_global = torch.cat([left_ids, right_ids])
         self.n_ghost = self.n_ghost_left + self.n_ghost_right
-        # periodic wrap of the ghost images along x
-        self.shift_left = -Lx if rank == 0 else 0.0
-        self.shift_right = Lx if rank == world - 1 else 0.0
         self.types_local = torch.cat([types[self.owned], types[self.ghost_global]])
         self.global_ids_local = torch.cat([self.owned, self.ghost_global])
-        # local periodic cell: x is open (ghosts cover it), y and z stay periodic
+        # local periodic cell: row 0 is open (ghosts cover it), rows 1 and 2 stay periodic
         self.cell = cell.clone()
         self.pbc = (False, True, True)
         # unwrapped x so that slab + ghosts form one contiguous block along x
@@ -93,15 +156,43 @@ class SlabDecomposition:
             self.edge_cell_shift = sh[keep].contiguous()
             self.n_edges = int(self.edge_index.shape[1])
 
+    def _set_geometry(self, geo: SlabGeometry):
+        """the geometry's decisions for this rank: the ghosts' periodic shifts as I receive them (``shift_left`` /
+        ``shift_right``) and as my neighbours receive my atoms (``push_shift_left`` / ``push_shift_right``); scalars
+        along x for a diagonal cell, 3-vectors otherwise"""
+        self.geom = geo
+        self.Lx = geo.Lx
+        self.shift_left, self.shift_right = geo.ghost_shifts(self.rank)
+        # my atoms are the right neighbour's left ghosts and the left neighbour's right ghosts
+        self.push_shift_right = geo.ghost_shifts((self.rank + 1) % self.world)[0]
+        self.push_shift_left = geo.ghost_shifts((self.rank - 1) % self.world)[1]
+
+    def _wrap0(self, pos: torch.Tensor) -> torch.Tensor:
+        """positions wrapped along lattice row 0 only (set-up; lattice cells): p - floor(s_0) h_0 in fp64, rounded once"""
+        h0 = torch.tensor(self.geom.rows[0], dtype=torch.float64, device=pos.device)
+        return (pos.double() - torch.floor(self.geom.frac0(pos))[:, None] * h0).to(pos.dtype)
+
+    def shift_ghosts(self, g: torch.Tensor, side: str) -> torch.Tensor:
+        """ghost rows [m, 3] from the left (``side`` "left") or right neighbour -> their periodic images in my frame.  A
+        lattice shift is added in fp64 and rounded once, as the peer-memory push does."""
+        sh = self.shift_left if side == "left" else self.shift_right
+        if self.geom.diagonal:
+            g[:, 0] += sh
+            return g
+        return (g.double() + torch.tensor(sh, dtype=torch.float64, device=g.device)).to(g.dtype)
+
     # positions of owned + ghost atoms taken from a global frame (set-up / tests)
     def local_positions_from_global(self, pos: torch.Tensor) -> torch.Tensor:
-        Lx = self.Lx
-        p = pos.clone()
-        p[:, 0] = p[:, 0] - torch.floor(p[:, 0] / Lx) * Lx
+        if self.geom.diagonal:
+            Lx = self.Lx
+            p = pos.clone()
+            p[:, 0] = p[:, 0] - torch.floor(p[:, 0] / Lx) * Lx
+        else:
+            p = self._wrap0(pos)
         gl = p[self.ghost_global[: self.n_ghost_left]].clone()
         gr = p[self.ghost_global[self.n_ghost_left :]].clone()
-        gl[:, 0] += self.shift_left
-        gr[:, 0] += self.shift_right
+        gl = self.shift_ghosts(gl, "left")
+        gr = self.shift_ghosts(gr, "right")
         return torch.cat([p[self.owned], gl, gr], 0)
 
     def to(self, device) -> "SlabDecomposition":
@@ -138,8 +229,8 @@ class SlabDecomposition:
                 got[r] = rbuf[o : o + n_in[r]]
                 o += n_in[r]
         gl, gr = got["from_left"].clone(), got["from_right"].clone()
-        gl[:, 0] += self.shift_left
-        gr[:, 0] += self.shift_right
+        gl = self.shift_ghosts(gl, "left")
+        gr = self.shift_ghosts(gr, "right")
         return torch.cat([gl, gr], 0)
 
     def exchange_reverse(self, g_ghost: torch.Tensor, g_owned: torch.Tensor) -> torch.Tensor:
@@ -209,9 +300,9 @@ class P2PHalo:
         self.pos_local = None
         self.send_right = dec.send_right_idx.to(self.dev).contiguous()
         self.send_left = dec.send_left_idx.to(self.dev).contiguous()
-        # periodic wrap along x as the RECEIVER sees my atoms (rank 0's left ghosts sit at x - Lx, ...)
-        self.shift_to_right = -dec.Lx if rank == world - 1 else 0.0
-        self.shift_to_left = dec.Lx if rank == 0 else 0.0
+        # periodic wrap as the RECEIVER sees my atoms (rank 0's left ghosts sit at x - Lx, or at s_0 - 1: pos - h_0), from
+        # the plan's geometry: a scalar along x (ab2_p2p_push_rows) or a lattice row (ab2_p2p_push_rows_v)
+        self.shift_to_right, self.shift_to_left = dec.push_shift_right, dec.push_shift_left
         torch.cuda.synchronize(self.dev)
         dist.barrier()
 
@@ -302,13 +393,16 @@ class P2PHalo:
         self.pos_local[: dec.n_owned].copy_(pos_owned)
         ck = self._lib._check
         ck(lib.ab2_p2p_begin(C.c_void_p(self.step.data_ptr()), st))
+        if dec.geom.diagonal:
+            push = lambda shift, *rest: lib.ab2_p2p_push_rows(*rest[:6], shift, *rest[6:])  # noqa: E731
+        else:
+            push = lambda shift, *rest: lib.ab2_p2p_push_rows_v(*rest[:6], *shift, *rest[6:])  # noqa: E731
         # I am the LEFT neighbour of my right peer (its slot 0) and the RIGHT neighbour of my left peer (its slot 1)
-        ck(lib.ab2_p2p_push_rows(dt, 0, 0, self._ptr(pos_owned), C.c_void_p(self.send_right.data_ptr()), int(self.send_right.shape[0]), self.shift_to_right,
-                                 C.c_void_p(self.peers[dec.right]), self.max_rows, dec.world, C.c_void_p(self.step.data_ptr()),
-                                 C.c_void_p(self.done.data_ptr()), st))
-        ck(lib.ab2_p2p_push_rows(dt, 0, 1, self._ptr(pos_owned), C.c_void_p(self.send_left.data_ptr()), int(self.send_left.shape[0]), self.shift_to_left,
-                                 C.c_void_p(self.peers[dec.left]), self.max_rows, dec.world, C.c_void_p(self.step.data_ptr()),
-                                 C.c_void_p(self.done.data_ptr() + 4), st))
+        ck(push(self.shift_to_right, dt, 0, 0, self._ptr(pos_owned), C.c_void_p(self.send_right.data_ptr()), int(self.send_right.shape[0]),
+                C.c_void_p(self.peers[dec.right]), self.max_rows, dec.world, C.c_void_p(self.step.data_ptr()), C.c_void_p(self.done.data_ptr()), st))
+        ck(push(self.shift_to_left, dt, 0, 1, self._ptr(pos_owned), C.c_void_p(self.send_left.data_ptr()), int(self.send_left.shape[0]),
+                C.c_void_p(self.peers[dec.left]), self.max_rows, dec.world, C.c_void_p(self.step.data_ptr()), C.c_void_p(self.done.data_ptr() + 4),
+                st))
         ck(lib.ab2_p2p_wait_unpack(dt, 0, 0, C.c_void_p(self.mailbox), self.max_rows, dec.world, C.c_void_p(self.step.data_ptr()), dec.n_ghost_left,
                                    self._ptr(self.pos_local, dec.n_owned), None, 0, st))
         ck(lib.ab2_p2p_wait_unpack(dt, 0, 1, C.c_void_p(self.mailbox), self.max_rows, dec.world, C.c_void_p(self.step.data_ptr()), dec.n_ghost_right,
@@ -619,8 +713,10 @@ class _SlabPlan(SlabDecomposition):
     attributes of a ``SlabDecomposition`` (so its torch.distributed exchanges, ``P2PHalo`` and ``DistributedAllegro``
     take it unchanged), with the local neighbour list built for ``r_list = r_max + skin``."""
 
-    def __init__(self, rank, world, Lx, cell, ids, types, send_left_idx, send_right_idx, ghost_ids_left, ghost_ids_right, ghost_types):
-        self.rank, self.world, self.Lx = rank, world, float(Lx)
+    def __init__(self, rank, world, geom: SlabGeometry, cell, ids, types, send_left_idx, send_right_idx, ghost_ids_left, ghost_ids_right,
+                 ghost_types):
+        self.rank, self.world = rank, world
+        self._set_geometry(geom)
         self.left, self.right = (rank - 1) % world, (rank + 1) % world
         self.owned = ids
         self.n_owned = int(ids.shape[0])
@@ -628,8 +724,6 @@ class _SlabPlan(SlabDecomposition):
         self.n_ghost_left, self.n_ghost_right = int(ghost_ids_left.shape[0]), int(ghost_ids_right.shape[0])
         self.n_ghost = self.n_ghost_left + self.n_ghost_right
         self.ghost_global = torch.cat([ghost_ids_left, ghost_ids_right])
-        self.shift_left = -self.Lx if rank == 0 else 0.0
-        self.shift_right = self.Lx if rank == world - 1 else 0.0
         self.types_local = torch.cat([types, ghost_types])
         self.global_ids_local = torch.cat([ids, self.ghost_global])
         self.cell = cell
@@ -638,7 +732,7 @@ class _SlabPlan(SlabDecomposition):
         self.n_edges = 0
 
     def build_list(self, pos_local: torch.Tensor, r_list: float):
-        """neighbour list of the owned centres over owned + ghost atoms, x open, y and z periodic"""
+        """neighbour list of the owned centres over owned + ghost atoms, row 0 open, rows 1 and 2 periodic"""
         if pos_local.is_cuda:
             self.csr, self.shift_vec = D.neighbor_csr(pos_local, r_list, self.cell, self.pbc, n_centres=self.n_owned)
             self.n_edges = self.csr.num_edges
@@ -650,10 +744,11 @@ class _SlabPlan(SlabDecomposition):
 
 
 class LocalAtoms:
-    """The atoms one rank owns: ``pos`` [n,3] (wrapped into the box at the last rebuild, unwrapped since), ``types`` [n],
-    ``ids`` [n] int64 (index in the global frame), ``image`` [n,3] int32 (boxes removed by wrapping: the unwrapped
-    position is pos + image * box) and ``arrays`` {name: [n, ...]} (velocities, masses, ... of the same atoms).
-    ``DistributedCalculator.compute`` may replace all of them together (re-partition)."""
+    """The atoms one rank owns: ``pos`` [n,3] (wrapped into the cell at the last rebuild, unwrapped since), ``types`` [n],
+    ``ids`` [n] int64 (index in the global frame), ``image`` [n,3] int32 (lattice vectors removed by wrapping: the
+    unwrapped position is pos + image @ h, h the cell's rows; pos + image * box for an orthorhombic box) and ``arrays``
+    {name: [n, ...]} (velocities, masses, ... of the same atoms).  ``DistributedCalculator.compute`` may replace all of
+    them together (re-partition)."""
 
     def __init__(self, pos, types, ids, image, arrays):
         self.pos, self.types, self.ids, self.image, self.arrays = pos, types, ids, image, arrays
@@ -676,7 +771,7 @@ class _MDStep:
 
 
 class DistributedCalculator:
-    """Molecular dynamics on several GPUs: a 1-D slab decomposition along x that follows the trajectory.
+    """Molecular dynamics on several GPUs: a 1-D slab decomposition along lattice row 0 that follows the trajectory.
 
     Every rank keeps a neighbour list of its owned centres built with ``r_list = r_max + skin`` over its atoms and the
     ghosts within ``r_list`` of its two faces.  Between rebuilds a step is one CUDA graph replay -- forward halo, the
@@ -695,9 +790,12 @@ class DistributedCalculator:
     ``transport``: "p2p" (P2PHalo, extended mailbox: the step always uses the vector reduction) or "nccl" (the
     torch.distributed exchanges of SlabDecomposition, whatever the backend: gloo on CPU).  ``stress`` /
     ``heat_current`` as in ``DistributedAllegro`` (heat_current implies the per-atom virial and needs a "velocities"
-    array).  The cell is fixed for the calculator's lifetime.  Set-up refuses (ValueError, on every rank, since every
-    rank checks the same arguments) a cell that is not orthorhombic and slabs thinner than ``r_max + skin`` (ghosts then
-    come from adjacent slabs only), and a model without ``energy_and_forces`` (NotImplementedError)."""
+    array).  The cell is fixed for the calculator's lifetime; it may be any regular cell (``SlabGeometry``: an
+    orthorhombic box is cut along x, any other cell in fractional coordinates along row 0, with ghosts that cross its
+    periodic face shifted by the row).  Set-up refuses (ValueError, on every rank, since every rank checks the same
+    arguments) a cell that is singular, not finite or near-coplanar, slabs thinner than ``r_max + skin`` (ghosts then
+    come from adjacent slabs only; the thickness of a triclinic slab is the height H_0 / world), and a model without
+    ``energy_and_forces`` (NotImplementedError)."""
 
     def __init__(self, model, cell: torch.Tensor, r_max: float, skin: float = 0.5, rank: int = 0, world: int = 1, device=None,
                  transport: str = "p2p", stress: bool = False, heat_current: bool = False, use_graph: bool = True, warmup: int = 2):
@@ -711,15 +809,21 @@ class DistributedCalculator:
         if not skin >= 0.0:
             raise ValueError(f"skin must be >= 0, got {skin}")
         c = cell.detach().reshape(3, 3).double().cpu()
-        if not bool((c - torch.diag(torch.diagonal(c))).abs().max() == 0) or not bool((torch.diagonal(c) > 0).all()):
-            raise ValueError("DistributedCalculator: the slab decomposition needs an orthorhombic cell with positive lengths")
-        self.box = [float(v) for v in torch.diagonal(c)]
+        try:
+            self.geom = SlabGeometry(c, world)
+        except ValueError as e:
+            raise ValueError(f"DistributedCalculator: {e}") from None
+        self.box = [float(v) for v in torch.diagonal(c)] if self.geom.diagonal else None
         self.r_max, self.skin = float(r_max), float(skin)
         self.r_list = self.r_max + self.skin
-        self.width = self.box[0] / world
+        self.width = self.geom.thickness
         if self.width < self.r_list:
-            raise ValueError(f"DistributedCalculator: slab width Lx / world = {self.width:.4g} is below r_max + skin = {self.r_list:.4g}: "
-                             "ghosts would come from beyond the adjacent slabs; use fewer ranks or a smaller skin")
+            if self.geom.diagonal:
+                raise ValueError(f"DistributedCalculator: slab width Lx / world = {self.width:.4g} is below r_max + skin = {self.r_list:.4g}: "
+                                 "ghosts would come from beyond the adjacent slabs; use fewer ranks or a smaller skin")
+            raise ValueError(f"DistributedCalculator: slab thickness H_0 / world = {self.width:.4g} is below r_max + skin = {self.r_list:.4g} "
+                             f"(H_0 = |det h| / |h_1 x h_2| = {self.geom.height:.4g} is the height of the cell along lattice row 0): ghosts "
+                             "would come from beyond the adjacent slabs; use fewer ranks or a smaller skin")
         self.model, self.rank, self.world = inner, int(rank), int(world)
         self.dev = torch.device(device) if device is not None else torch.device("cpu")
         self.transport = transport
@@ -754,7 +858,10 @@ class DistributedCalculator:
         image = torch.zeros(n, 3, dtype=torch.int32, device=self.dev)
         from . import _lib
 
-        mine, _, _, _ = _lib.slab_wrap_classify(p, image, self.box, self.rank, self.world, self.width)
+        if self.geom.diagonal:
+            mine, _, _, _ = _lib.slab_wrap_classify(p, image, self.box, self.rank, self.world, self.width)
+        else:
+            mine, _, _, _ = _lib.slab_wrap_classify_lattice(p, image, self.geom.rows, self.rank, self.world)
         sel = mine.to(p.device)
         local = LocalAtoms(p.index_select(0, sel), types.to(self.dev).index_select(0, sel), sel.clone(), image.index_select(0, sel),
                            {k: v.detach().to(self.dev).index_select(0, sel).contiguous() for k, v in arrays.items()})
@@ -867,9 +974,13 @@ class DistributedCalculator:
         sync = (lambda: torch.cuda.synchronize(self.dev)) if self.dev.type == "cuda" else (lambda: None)
         self._graphed = None
         t0 = time.perf_counter()
-        # 1. wrap and classify (one read of the counts)
-        stay, to_left, to_right, n_far = _lib.slab_wrap_classify(local.pos, local.image, self.box, self.rank, self.world, self.width,
-                                                                 jump=self.width)
+        # 1. wrap and classify (one read of the counts); a lattice cell's jump is one slab in s_0
+        if self.geom.diagonal:
+            stay, to_left, to_right, n_far = _lib.slab_wrap_classify(local.pos, local.image, self.box, self.rank, self.world, self.width,
+                                                                     jump=self.width)
+        else:
+            stay, to_left, to_right, n_far = _lib.slab_wrap_classify_lattice(local.pos, local.image, self.geom.rows, self.rank, self.world,
+                                                                             jump=1.0 / self.world)
         # 2. an atom bound for a non-adjacent slab: agreed first, so every rank raises and nobody waits on an exchange
         far = self._allreduce_max(n_far)
         if far > 0:
@@ -891,7 +1002,10 @@ class DistributedCalculator:
         t2 = time.perf_counter()
         self.rebuild_seconds["migration"] += t2 - t1
         # 4. ghosts: my atoms within r_list of the low face go to the left neighbour, of the high face to the right one
-        low, high = _lib.slab_faces(local.pos, self.box, self.rank, self.world, self.width, self.r_list)
+        if self.geom.diagonal:
+            low, high = _lib.slab_faces(local.pos, self.box, self.rank, self.world, self.width, self.r_list)
+        else:
+            low, high = _lib.slab_faces_lattice(local.pos, self.geom.rows, self.rank, self.world, self.r_list)
 
         def ghost_rows(idx):
             m = int(idx.shape[0])
@@ -899,14 +1013,11 @@ class DistributedCalculator:
                               local.ids.index_select(0, idx).double().reshape(m, 1)], 1)
 
         g_l, g_r = self._neighbours(ghost_rows(high), ghost_rows(low))
-        shift_left = -self.box[0] if self.rank == 0 else 0.0
-        shift_right = self.box[0] if self.rank == self.world - 1 else 0.0
-        g_l[:, 0] += shift_left
-        g_r[:, 0] += shift_right
         # ghost rows: pos (3), type, id
-        plan = _SlabPlan(self.rank, self.world, self.box[0], self.cell, local.ids, local.types, low, high, g_l[:, 4].to(torch.int64),
+        plan = _SlabPlan(self.rank, self.world, self.geom, self.cell, local.ids, local.types, low, high, g_l[:, 4].to(torch.int64),
                          g_r[:, 4].to(torch.int64), torch.cat([g_l[:, 3], g_r[:, 3]]).to(local.types.dtype))
-        pos_ghost = torch.cat([g_l[:, :3], g_r[:, :3]]).to(local.pos.dtype)
+        # the periodic images, in fp64 (the plan's shifts: -+Lx along x, or -+h_0)
+        pos_ghost = torch.cat([plan.shift_ghosts(g_l[:, :3].clone(), "left"), plan.shift_ghosts(g_r[:, :3].clone(), "right")]).to(local.pos.dtype)
         if self.transport == "p2p":
             if self.p2p is None:
                 self.p2p = P2PHalo(plan, self.dev, atomic_virial=True, headroom=MAILBOX_HEADROOM)
@@ -934,11 +1045,14 @@ class DistributedCalculator:
     # ---- output ------------------------------------------------------------------------------------------------------
     def gather(self, local: LocalAtoms) -> Optional[Dict[str, torch.Tensor]]:
         """The whole frame on rank 0, in global-id order (trajectory output; collective, through the host): ``pos``
-        [N,3] fp64 unwrapped (pos + image * box), ``image``, ``types``, ``ids`` and every array, as CPU tensors.  None on
-        the other ranks."""
-        box = torch.tensor(self.box, dtype=torch.float64, device=local.pos.device)
-        mine = {"pos": (local.pos.double() + local.image.double() * box).cpu(), "image": local.image.cpu(), "types": local.types.cpu(),
-                "ids": local.ids.cpu()}
+        [N,3] fp64 unwrapped (pos + image @ h, h the cell's rows; pos + image * box for an orthorhombic box), ``image``,
+        ``types``, ``ids`` and every array, as CPU tensors.  None on the other ranks."""
+        if self.geom.diagonal:
+            box = torch.tensor(self.box, dtype=torch.float64, device=local.pos.device)
+            unwrapped = local.pos.double() + local.image.double() * box
+        else:
+            unwrapped = local.pos.double() + local.image.double() @ torch.tensor(self.geom.rows, dtype=torch.float64, device=local.pos.device)
+        mine = {"pos": unwrapped.cpu(), "image": local.image.cpu(), "types": local.types.cpu(), "ids": local.ids.cpu()}
         mine.update({k: v.detach().cpu() for k, v in local.arrays.items()})
         got = [None] * self.world if self.rank == 0 else None
         dist.gather_object(mine, got, dst=0)

@@ -460,6 +460,11 @@ int ab2_p2p_begin(void* step_counter, void* stream);
 int ab2_p2p_push_rows(int src_dtype, int kind, int side, const void* src, const int64_t* idx, int n, double shift_x,
                       void* peer_mailbox, int max_rows, int world, const void* step_counter, void* done_counter,
                       void* stream);
+/* ab2_p2p_push_rows with a 3-component shift added to every row (positions of a triclinic cell, whose ghosts that cross
+ * the periodic face of lattice row 0 move by that row); passed by value, so a captured graph replays it. */
+int ab2_p2p_push_rows_v(int src_dtype, int kind, int side, const void* src, const int64_t* idx, int n, double shift_x, double shift_y,
+                        double shift_z, void* peer_mailbox, int max_rows, int world, const void* step_counter, void* done_counter,
+                        void* stream);
 int ab2_p2p_wait_unpack(int dst_dtype, int kind, int side, void* my_mailbox, int max_rows, int world,
                         const void* step_counter, int n, void* dst, const int64_t* idx, int accumulate, void* stream);
 int ab2_p2p_allreduce_energy(const void* e_local, int rank, int world, int max_rows, void* const* peers_dev,
@@ -506,6 +511,17 @@ int ab2_p2p_allreduce_vec(const void* v_local, int n_values, int rank, int world
  * n = 0 launches nothing.  Both launch on `stream`. */
 int ab2_slab_plan_count(int pos_dtype, int mode, int64_t n, void* pos, int32_t* image, const double* box_host, int rank, int world,
                         double width, double jump, double r_list, uint8_t* cls, int32_t* block_counts, void* stream);
+/* The same plan for any regular cell, cut along lattice row 0 in fractional coordinates s = pos . h^-1 (rows_host[9] =
+ * the rows h_0, h_1, h_2; the inverse is computed here, and a non-finite, singular or near-coplanar cell is refused
+ * before any launch).  Rank r owns s_0 in [lo, hi) = [r / world, (r + 1) / world).  Outputs as ab2_slab_plan_count;
+ * ab2_slab_plan_fill takes them unchanged.
+ *   mode 0: img_a = floor(s_a), pos <- pos - sum_a img_a h_a (fp64, rounded once to the positions' dtype), image += img;
+ *           classified by clamp(floor(s_0 world), 0, world - 1) of the wrapped position; refused (column 3): the
+ *           unwrapped s_0 outside [lo - jump, hi + jump) (jump in fractional units) or a non-adjacent slab.  world 2:
+ *           left when the unwrapped s_0 < lo.
+ *   mode 1: list 0 = s_0 < lo + r_list / H_0, list 1 = s_0 >= hi - r_list / H_0 (fp64; H_0 = |det h| / |h_1 x h_2|). */
+int ab2_slab_plan_count_lattice(int pos_dtype, int mode, int64_t n, void* pos, int32_t* image, const double* rows_host, int rank, int world,
+                                double jump, double r_list, uint8_t* cls, int32_t* block_counts, void* stream);
 int ab2_slab_plan_fill(int64_t n, const uint8_t* cls, const int32_t* block_offsets, int64_t* list0, int64_t* list1, int64_t* list2,
                        void* stream);
 
