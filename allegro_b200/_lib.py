@@ -93,6 +93,8 @@ _SIGNATURES = {
     "ab2_radial_bwd": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_nl_frames_count": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_nl_frames_fill": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_nl_prune_count": ([_i32, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_nl_prune_fill": ([_i32, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_frame_scratch_elems": ([_i64, _i64], C.c_int64),
     "ab2_frame_sum": ([_i32, _i64, _i64, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_frame_virial": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
@@ -865,6 +867,32 @@ def nl_frames(pos: torch.Tensor, frame_ptr: torch.Tensor, cell: torch.Tensor, in
         with _timed("nl_frames_fill"):
             _check(load().ab2_nl_frames_fill(dt, n, B, *args, _ptr(row_ptr), _ptr(nbr), _ptr(shift), _stream()))
     return row_ptr, nbr, shift
+
+
+def nl_prune(pos: torch.Tensor, row_ptr: torch.Tensor, nbr: torch.Tensor, shift: torch.Tensor, types: torch.Tensor, cut2: torch.Tensor):
+    """Keep the edges shorter than their pair's list radius (ab2_nl_prune_count / fill) -> (row_ptr [n_centres+1] int32,
+    nbr [E'] int32, shift [E',3] pos dtype), each row an ordered subsequence of the input row.  ``types`` [n] int32 in
+    [0, T), ``cut2`` [T,T] fp64 squared radii (row = centre type), all on the device; the caller checks them
+    (``data.prune_csr``).  No launch for zero centres or zero edges."""
+    nc, E, T = row_ptr.shape[0] - 1, nbr.shape[0], cut2.shape[0]
+    if nc == 0 or E == 0:
+        return row_ptr.clone(), nbr.clone(), shift.clone()
+    dt = DTYPE_ENUM[pos.dtype]
+    assert shift.dtype == pos.dtype and types.dtype == torch.int32 and cut2.dtype == torch.float64
+    args = (dt, nc, E, T, _ptr(_contig(pos, "pos")), _ptr(_contig(types, "types")), _ptr(_contig(cut2, "cut2")),
+            _ptr(_contig(row_ptr, "row_ptr")), _ptr(_contig(nbr, "nbr")), _ptr(_contig(shift, "shift")))
+    counts = torch.empty(nc, dtype=torch.int32, device=pos.device)
+    with _timed("nl_prune_count"):
+        _check(load().ab2_nl_prune_count(*args, _ptr(counts), _stream()))
+    out_ptr = torch.zeros(nc + 1, dtype=torch.int32, device=pos.device)
+    out_ptr[1:] = torch.cumsum(counts, 0).to(torch.int32)
+    E2 = int(out_ptr[-1])
+    out_nbr = torch.empty(E2, dtype=torch.int32, device=pos.device)
+    out_shift = torch.empty(E2, 3, dtype=pos.dtype, device=pos.device)
+    if E2:
+        with _timed("nl_prune_fill"):
+            _check(load().ab2_nl_prune_fill(*args, _ptr(out_ptr), _ptr(out_nbr), _ptr(out_shift), _stream()))
+    return out_ptr, out_nbr, out_shift
 
 
 def _frame_scratch(total: int, B: int, width: int, device):

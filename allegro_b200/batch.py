@@ -31,17 +31,20 @@ def _pbc_of(frame: D.Type) -> torch.Tensor:
     return p.expand(3).clone() if p.numel() == 1 else p
 
 
-def collate(frames: Sequence[D.Type], r_max: Optional[float] = None) -> D.Type:
+def collate(frames: Sequence[D.Type], r_max: Optional[float] = None, cutoffs=None) -> D.Type:
     """Single-frame dicts (``pos``, ``atom_types``, optional ``cell`` / ``pbc``, optional ``edge_index`` /
     ``edge_cell_shift``, optional ``velocities``, on every frame or none) -> one batched dict.  When every frame has ``edge_index`` the lists are offset and concatenated;
     when none has, the list is built on the device with ``data.neighbor_csr_frames`` (needs ``r_max``; frames of at most
     ``data.FRAMES_MAX_ATOMS`` atoms).  A mix of the two is rejected.  A frame without a cell gets a zero cell and no
-    periodic axis."""
+    periodic axis.  ``cutoffs`` [T,T] (e.g. the model's ``rmax_table``): the device-built list is pruned to those
+    per-type-pair radii (``data.prune_csr``); frames that bring their own ``edge_index`` are then refused."""
     if len(frames) == 0:
         raise ValueError("collate needs at least one frame")
     has_ei = [D.EDGE_INDEX_KEY in f for f in frames]
     if any(has_ei) and not all(has_ei):
         raise ValueError("collate: some frames carry edge_index and others do not; give every frame a neighbour list or none")
+    if cutoffs is not None and any(has_ei):
+        raise ValueError("collate: cutoffs prune the list collate builds on the device; these frames bring their own edge_index")
     pos = [f[D.POSITIONS_KEY] for f in frames]
     dev, dtype = pos[0].device, pos[0].dtype
     sizes = [int(p.shape[0]) for p in pos]
@@ -77,7 +80,8 @@ def collate(frames: Sequence[D.Type], r_max: Optional[float] = None) -> D.Type:
         raise ValueError("collate: the frames carry no edge_index, so r_max is needed to build the neighbour list")
     frame_ptr = torch.zeros(B + 1, dtype=torch.int64)
     frame_ptr[1:] = torch.cumsum(torch.tensor(sizes), 0)
-    csr, shift = D.neighbor_csr_frames(out[D.POSITIONS_KEY], frame_ptr, out.get(D.CELL_KEY), pbc, r_max)
+    types = out[D.ATOM_TYPE_KEY] if cutoffs is not None else None
+    csr, shift = D.neighbor_csr_frames(out[D.POSITIONS_KEY], frame_ptr, out.get(D.CELL_KEY), pbc, r_max, types=types, cutoffs=cutoffs)
     out[D.CSR_KEY], out[D.EDGE_SHIFT_VEC_KEY] = csr, shift
     return out
 

@@ -14,6 +14,12 @@ tests/test_calculator.py against evaluations on exact r_max lists).
 
 ``model`` is anything with the reference's ``forward(data) -> data`` contract; CUDA-graph replay is used
 when it exposes the fused ``energy_and_forces`` path (allegro_b200.model.AllegroModel).
+
+The same argument holds pair type by pair type.  With ``prune_edges=True`` and a model built with
+``per_edge_type_cutoff``, the list is searched at ``r_list = max(rmax_table) + skin`` and pruned to
+``rmax_table[t_i, t_j] + skin`` (``data.prune_csr``), so an H-H or Li-Li pair beyond its own cutoff is never evaluated.
+The rebuild rule (an atom moved more than ``skin / 2``) covers each pair with its own radius, so no kept-out pair can
+come within its cutoff before the next rebuild.
 """
 from __future__ import annotations
 
@@ -24,12 +30,24 @@ import torch
 from . import data as D
 
 
+def prune_table(model, skin: float) -> Optional[torch.Tensor]:
+    """``rmax_table + skin`` [T,T] fp64 on the CPU of a model built with per-edge-type cutoffs, else None."""
+    inner = getattr(model, "model", model)
+    norm = getattr(inner, "edge_norm", None)
+    if norm is None or not getattr(norm, "per_type", False):
+        return None
+    return norm.rmax_table.detach().to(device="cpu", dtype=torch.float64) + float(skin)
+
+
 class AllegroCalculator:
     def __init__(self, model, r_max: float, skin: float = 0.5, pbc=(True, True, True), use_graph: bool = True,
                  compute_stress: bool = False, check_every: int = 1, compute_atomic_virial: bool = False,
-                 compute_heat_current: bool = False):
+                 compute_heat_current: bool = False, prune_edges: bool = False):
         assert skin >= 0.0 and check_every >= 1
         self.model, self.r_max, self.skin = model, float(r_max), float(skin)
+        # per-type list radii (prune_edges with a per_edge_type_cutoff model), else one radius r_max + skin
+        self._cutoffs = prune_table(model, skin) if prune_edges else None
+        self.r_list = float(self._cutoffs.max()) if self._cutoffs is not None else self.r_max + self.skin
         self.pbc = tuple(bool(p) for p in (pbc if not isinstance(pbc, bool) else (pbc,) * 3))
         self.compute_stress = bool(compute_stress)
         # per-atom virial / heat current: skin edges have zero gradient, so they add nothing to either
@@ -73,15 +91,26 @@ class AllegroCalculator:
                 raise ValueError("compute_stress=True needs a non-singular cell: stress is the virial over the cell volume")
         data = {D.POSITIONS_KEY: pos.clone(), D.ATOM_TYPE_KEY: atom_types.reshape(-1).clone()}
         inner = getattr(self.model, "model", self.model)
-        if hasattr(inner, "energy_and_forces") and D.csr_supported(pos, self.r_max + self.skin, cell, self.pbc):
+        if hasattr(inner, "energy_and_forces") and D.csr_supported(pos, self.r_list, cell, self.pbc):
             # CUDA cell list straight into the kernels' CSR (no int64 COO list, no sort by centre); any cell, or none
-            csr, shift_vec = D.neighbor_csr(pos, self.r_max + self.skin, cell, self.pbc)
+            prune = {} if self._cutoffs is None else dict(types=data[D.ATOM_TYPE_KEY], cutoffs=self._cutoffs)
+            csr, shift_vec = D.neighbor_csr(pos, self.r_list, cell, self.pbc, **prune)
+            data[D.CSR_KEY], data[D.EDGE_SHIFT_VEC_KEY] = csr, shift_vec
+            if cell is not None:
+                data[D.CELL_KEY] = cell.view(3, 3).clone()
+            self._n_edges = csr.num_edges
+        elif self._cutoffs is not None and hasattr(inner, "energy_and_forces"):
+            # the pair search, then the same pruning on its CSR form
+            ei, shift = D.neighbor_list(pos, self.r_list, cell, self.pbc)
+            n = pos.shape[0]
+            shift_vec = shift @ cell.view(3, 3).to(pos.dtype) if cell is not None else torch.zeros(ei.shape[1], 3, dtype=pos.dtype, device=pos.device)
+            csr, shift_vec = D.prune_csr(D.build_csr(ei, n), shift_vec.contiguous(), pos, data[D.ATOM_TYPE_KEY], self._cutoffs, self.r_list)
             data[D.CSR_KEY], data[D.EDGE_SHIFT_VEC_KEY] = csr, shift_vec
             if cell is not None:
                 data[D.CELL_KEY] = cell.view(3, 3).clone()
             self._n_edges = csr.num_edges
         else:
-            ei, shift = D.neighbor_list(pos, self.r_max + self.skin, cell, self.pbc)
+            ei, shift = D.neighbor_list(pos, self.r_list, cell, self.pbc)
             data[D.EDGE_INDEX_KEY] = ei
             self._n_edges = int(ei.shape[1])
             if cell is not None:

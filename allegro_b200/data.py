@@ -250,15 +250,17 @@ def neighbor_list(
 # --------------------------------------------------------------------------- #
 class EdgeCSR:
     """Centre-sorted edge list. ``perm`` maps sorted position -> original edge (None if the
-    input was already sorted)."""
+    input was already sorted).  ``radius``: the single radius the list holds every pair within (set by the device
+    searches; None when unknown or after ``prune_csr``)."""
 
-    __slots__ = ("num_atoms", "num_edges", "ctr", "nbr", "row_ptr", "perm", "max_degree", "_transposed")
+    __slots__ = ("num_atoms", "num_edges", "ctr", "nbr", "row_ptr", "perm", "max_degree", "radius", "_transposed")
 
-    def __init__(self, num_atoms, ctr, nbr, row_ptr, perm, max_degree):
+    def __init__(self, num_atoms, ctr, nbr, row_ptr, perm, max_degree, radius: Optional[float] = None):
         self.num_atoms = int(num_atoms)
         self.num_edges = int(ctr.shape[0])
         self.ctr, self.nbr, self.row_ptr, self.perm = ctr, nbr, row_ptr, perm
         self.max_degree = int(max_degree)
+        self.radius = None if radius is None else float(radius)
         self._transposed = None
 
     def transposed(self, n_total: int):
@@ -511,11 +513,24 @@ def _csr_grid(pos, r_max, cell, pbc):
     return search_grid(pos, r_max, cell, pbc)
 
 
-def neighbor_csr(pos: torch.Tensor, r_max: float, cell: Optional[torch.Tensor], pbc=(True, True, True), n_centres: Optional[int] = None):
+def _csr_of(row_ptr: torch.Tensor, nbr: torch.Tensor, radius: Optional[float]) -> EdgeCSR:
+    """EdgeCSR of device rows (``ctr`` and ``max_degree`` rebuilt from row_ptr)."""
+    nc = row_ptr.shape[0] - 1
+    counts = (row_ptr[1:] - row_ptr[:-1])
+    ctr = torch.repeat_interleave(torch.arange(nc, device=row_ptr.device, dtype=torch.int32), counts.long())
+    maxdeg = int(counts.max()) if nc > 0 else 0
+    return EdgeCSR(nc, ctr.contiguous(), nbr, row_ptr, None, maxdeg, radius)
+
+
+def neighbor_csr(pos: torch.Tensor, r_max: float, cell: Optional[torch.Tensor], pbc=(True, True, True), n_centres: Optional[int] = None,
+                 types: Optional[torch.Tensor] = None, cutoffs: Optional[torch.Tensor] = None):
     """Neighbour search on the device straight into the kernels' format -> (EdgeCSR, shift_vec [E,3] in the positions'
     dtype).  Centres are atoms [0, n_centres) (owned atoms first).  An orthorhombic box with >= 3 r_max per periodic
     axis takes ab2_nl_bin / count / fill (SURVEY 8 row f2); any other cell, and ``cell=None`` for a frame without
-    periodic axes, takes ab2_nl_lattice_bin / count / fill.  r = pos[nbr] + shift - pos[ctr] holds for the raw positions."""
+    periodic axes, takes ab2_nl_lattice_bin / count / fill.  r = pos[nbr] + shift - pos[ctr] holds for the raw positions.
+
+    ``cutoffs`` [T,T] (with ``types`` [n], one per atom): the list searched at ``r_max`` is then pruned to the per-type-pair
+    radii (``prune_csr``; every refusal of ``prune_csr`` is raised before the search)."""
     from . import _lib
 
     pbc = tuple(bool(p) for p in (pbc if not isinstance(pbc, bool) else (pbc,) * 3))
@@ -523,8 +538,9 @@ def neighbor_csr(pos: torch.Tensor, r_max: float, cell: Optional[torch.Tensor], 
     if route is None:
         raise ValueError("neighbor_csr needs CUDA positions and a finite non-singular cell on the periodic axes (or cell=None "
                          "with no periodic axis)")
-    kind, grid = route
     n = pos.shape[0]
+    prune = _prune_args(types, cutoffs, n, r_max, pos.device)
+    kind, grid = route
     nc = n if n_centres is None else int(n_centres)
     if kind == "ortho":
         box, origin, ncell = grid
@@ -532,10 +548,69 @@ def neighbor_csr(pos: torch.Tensor, r_max: float, cell: Optional[torch.Tensor], 
     else:
         rows, origin, ncell, reach = grid
         row_ptr, nbr, shift = _lib.neighbor_csr_lattice(pos, r_max, rows, origin, ncell, reach, pbc, nc)
-    counts = (row_ptr[1:] - row_ptr[:-1])
-    ctr = torch.repeat_interleave(torch.arange(nc, device=pos.device, dtype=torch.int32), counts.long())
-    maxdeg = int(counts.max()) if nc > 0 else 0
-    return EdgeCSR(nc, ctr.contiguous(), nbr, row_ptr, None, maxdeg), shift
+    if prune is not None:
+        return _prune(pos, row_ptr, nbr, shift, *prune)
+    return _csr_of(row_ptr, nbr, r_max), shift
+
+
+def _prune_args(types: Optional[torch.Tensor], cutoffs: Optional[torch.Tensor], n: int, r_list: Optional[float], device):
+    """Checks of ``prune_csr``, all made with ONE device-to-host read -> (types [n] int32, cut2 [T*T] fp64) on ``device``, or
+    None when neither ``types`` nor ``cutoffs`` is given."""
+    if cutoffs is None and types is None:
+        return None
+    if cutoffs is None or types is None:
+        raise ValueError("pruning needs both the per-atom types and the [T, T] cutoff table")
+    if r_list is None:
+        raise ValueError("prune_csr: the radius the list was built with is unknown; pass r_list")
+    c = torch.as_tensor(cutoffs)
+    if c.dim() != 2 or c.shape[0] != c.shape[1] or c.shape[0] < 1:
+        raise ValueError(f"the cutoff table must be [T, T] with T >= 1, got shape {tuple(c.shape)}")
+    T = int(c.shape[0])
+    t = torch.as_tensor(types).reshape(-1)
+    if t.shape[0] != n:
+        raise ValueError(f"types has {t.shape[0]} entries for {n} atoms: one type per atom (neighbours included)")
+    if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+        raise ValueError(f"types must be integers, got {t.dtype}")
+    c64 = c.detach().to(torch.float64).reshape(-1)
+    # one read: the table and the type range
+    ext = torch.stack([t.min(), t.max()]).to(device=c64.device, dtype=torch.float64) if n else c64.new_zeros(0)
+    host = torch.cat([c64, ext]).cpu()
+    tab, trange = host[: T * T], host[T * T:].tolist()
+    if not bool(torch.isfinite(tab).all()) or not bool((tab > 0).all()):
+        raise ValueError(f"every cutoff must be finite and > 0, got {tab.view(T, T).tolist()}")
+    if float(tab.max()) > float(r_list):
+        raise ValueError(f"a cutoff ({float(tab.max())!r}) exceeds the radius the list was built with ({float(r_list)!r}): pairs "
+                         "between them are not in the list")
+    if trange and (trange[0] < 0 or trange[1] >= T):
+        raise ValueError(f"types must lie in [0, {T}), got [{int(trange[0])}, {int(trange[1])}]")
+    cut2 = (tab * tab).view(T, T).to(device)
+    return t.to(device=device, dtype=torch.int32).contiguous(), cut2
+
+
+def _prune(pos, row_ptr, nbr, shift, types_i32, cut2):
+    from . import _lib
+
+    row_ptr, nbr, shift = _lib.nl_prune(pos, row_ptr, nbr, shift, types_i32, cut2)
+    return _csr_of(row_ptr, nbr, None), shift
+
+
+def prune_csr(csr: EdgeCSR, shift_vec: torch.Tensor, pos: torch.Tensor, types: torch.Tensor, cutoffs: torch.Tensor,
+              r_list: Optional[float] = None) -> Tuple[EdgeCSR, torch.Tensor]:
+    """Drop the edges at or beyond their own pair's radius (ab2_nl_prune_count / fill) -> (EdgeCSR, shift_vec).
+
+    Edge z (centre i, neighbour j, shift s) is kept iff d2 < cutoffs[t_i, t_j]^2, d2 = sum_x (pos[j] + s - pos[i])_x^2 in
+    fp64 with the operations of include/allegro_b200.h.  ``cutoffs`` [T,T] is directed (row = centre type), indexed as the
+    model's ``rmax_table``; ``types`` [n] holds one type per atom of ``pos`` (neighbours included).  Each row of the result
+    is an ordered subsequence of the input row, with nbr and shift copied bitwise; ``ctr`` and ``max_degree`` are rebuilt,
+    ``perm`` is dropped (per-edge outputs of a pruned list are in its own order).  ``r_list``: the radius the list was
+    built with (default ``csr.radius``).  Raises ValueError before any launch when the table is not [T,T], an entry is
+    not finite or <= 0 or exceeds ``r_list``, or ``types`` has the wrong length or values outside [0, T).  The checks cost
+    one device-to-host read."""
+    n = pos.shape[0]
+    if csr.row_ptr.shape[0] != csr.num_atoms + 1 or csr.num_atoms > n:
+        raise ValueError(f"the list has {csr.num_atoms} centres for {n} atoms")
+    prune = _prune_args(types, cutoffs, n, csr.radius if r_list is None else r_list, pos.device)
+    return _prune(pos, csr.row_ptr, csr.nbr, shift_vec, *prune)
 
 
 # Largest frame neighbor_csr_frames takes: its search is all-pairs per frame, O(N_b^2 * images).  Larger frames belong to
@@ -616,7 +691,8 @@ def frames_geometry(cell: Optional[torch.Tensor], pbc: torch.Tensor, r_max: floa
     return torch.from_numpy(h), torch.from_numpy(nimg.astype(np.int64))
 
 
-def neighbor_csr_frames(pos: torch.Tensor, frame_ptr, cell: Optional[torch.Tensor], pbc, r_max: float):
+def neighbor_csr_frames(pos: torch.Tensor, frame_ptr, cell: Optional[torch.Tensor], pbc, r_max: float, types: Optional[torch.Tensor] = None,
+                        cutoffs: Optional[torch.Tensor] = None):
     """Neighbour lists of a batch of small frames in one pass on the device (ab2_nl_frames_count / fill), straight into the
     kernels' format -> (EdgeCSR over all atoms of the batch, shift_vec [E,3] in the positions' dtype).
 
@@ -626,7 +702,8 @@ def neighbor_csr_frames(pos: torch.Tensor, frame_ptr, cell: Optional[torch.Tenso
     are those of ``neighbor_list(frame, method="brute")`` in the same order (by neighbour, then by image), with the frame's
     atom offset added;  r = pos[nbr] + shift - pos[ctr]  holds for the raw positions.  Refused with ValueError before any
     search (``frames_geometry``): frames above FRAMES_MAX_ATOMS atoms (the search is all-pairs per frame), periodic frames
-    with a non-finite, singular or near-coplanar cell, and frames needing more than FRAMES_MAX_IMAGES images per pair."""
+    with a non-finite, singular or near-coplanar cell, and frames needing more than FRAMES_MAX_IMAGES images per pair.
+    ``cutoffs`` [T,T] with ``types`` [n]: the list is pruned to per-type-pair radii, as in ``neighbor_csr``."""
     from . import _lib
 
     dev = pos.device
@@ -641,13 +718,13 @@ def neighbor_csr_frames(pos: torch.Tensor, frame_ptr, cell: Optional[torch.Tenso
                          "use neighbor_csr or neighbor_list for large frames")
     pbc_t = _frames_pbc(pbc, B, "cpu")
     rows, _ = frames_geometry(cell, pbc_t, r_max, pos.dtype)  # refuses before any device work; _lib.nl_frames derives nimg
+    prune = _prune_args(types, cutoffs, n, r_max, dev)
     rows = rows.to(dev)
     periodic = pbc_t.any(dim=1).view(B, 1, 1).to(dev)
     eye = torch.eye(3, dtype=torch.float64, device=dev).expand(B, 3, 3)
     inv = torch.where(periodic, torch.linalg.inv(torch.where(periodic, rows, eye)), torch.zeros_like(rows))
     row_ptr, nbr, shift = _lib.nl_frames(pos.contiguous(), fp.to(device=dev, dtype=torch.int32), rows.to(pos.dtype).contiguous(),
                                          inv.to(pos.dtype).contiguous(), pbc_t.to(device=dev, dtype=torch.int32), float(r_max))
-    counts = row_ptr[1:] - row_ptr[:-1]
-    ctr = torch.repeat_interleave(torch.arange(n, device=dev, dtype=torch.int32), counts.long())
-    maxdeg = int(counts.max()) if n > 0 else 0
-    return EdgeCSR(n, ctr.contiguous(), nbr, row_ptr, None, maxdeg), shift
+    if prune is not None:
+        return _prune(pos, row_ptr, nbr, shift, *prune)
+    return _csr_of(row_ptr, nbr, r_max), shift

@@ -28,6 +28,7 @@ import torch
 import torch.distributed as dist
 
 from . import data as D
+from .calculator import prune_table
 
 
 class SlabGeometry:
@@ -731,16 +732,24 @@ class _SlabPlan(SlabDecomposition):
         self.csr = self.shift_vec = self.edge_index = self.edge_cell_shift = None
         self.n_edges = 0
 
-    def build_list(self, pos_local: torch.Tensor, r_list: float):
-        """neighbour list of the owned centres over owned + ghost atoms, row 0 open, rows 1 and 2 periodic"""
+    def build_list(self, pos_local: torch.Tensor, r_list: float, cutoffs: Optional[torch.Tensor] = None):
+        """neighbour list of the owned centres over owned + ghost atoms, row 0 open, rows 1 and 2 periodic; ``cutoffs``
+        [T,T]: pruned to those per-type-pair radii (data.prune_csr)"""
         if pos_local.is_cuda:
-            self.csr, self.shift_vec = D.neighbor_csr(pos_local, r_list, self.cell, self.pbc, n_centres=self.n_owned)
+            prune = {} if cutoffs is None else dict(types=self.types_local, cutoffs=cutoffs)
+            self.csr, self.shift_vec = D.neighbor_csr(pos_local, r_list, self.cell, self.pbc, n_centres=self.n_owned, **prune)
             self.n_edges = self.csr.num_edges
         else:  # CPU (the gloo tests): the pair search, rows of owned centres only
             ei, sh = D.neighbor_list(pos_local, r_list, self.cell, self.pbc)
             keep = ei[0] < self.n_owned
             self.edge_index, self.edge_cell_shift = ei[:, keep].contiguous(), sh[keep].contiguous()
             self.n_edges = int(self.edge_index.shape[1])
+            if cutoffs is not None:
+                shift_vec = (self.edge_cell_shift @ self.cell.view(3, 3).to(pos_local.dtype)).contiguous()
+                self.csr, self.shift_vec = D.prune_csr(D.build_csr(self.edge_index, self.n_owned), shift_vec, pos_local, self.types_local,
+                                                       cutoffs, r_list)
+                self.edge_index = self.edge_cell_shift = None
+                self.n_edges = self.csr.num_edges
 
 
 class LocalAtoms:
@@ -795,10 +804,15 @@ class DistributedCalculator:
     periodic face shifted by the row).  Set-up refuses (ValueError, on every rank, since every rank checks the same
     arguments) a cell that is singular, not finite or near-coplanar, slabs thinner than ``r_max + skin`` (ghosts then
     come from adjacent slabs only; the thickness of a triclinic slab is the height H_0 / world), and a model without
-    ``energy_and_forces`` (NotImplementedError)."""
+    ``energy_and_forces`` (NotImplementedError).
+
+    ``prune_edges=True`` with a model built with ``per_edge_type_cutoff``: ``r_list = max(rmax_table) + skin`` (the ghost
+    shells and the slab-thickness check use it) and every rank's list is pruned to ``rmax_table + skin`` pair type by
+    pair type (``data.prune_csr``), as in ``AllegroCalculator``.  Without a per-type table the flag changes nothing."""
 
     def __init__(self, model, cell: torch.Tensor, r_max: float, skin: float = 0.5, rank: int = 0, world: int = 1, device=None,
-                 transport: str = "p2p", stress: bool = False, heat_current: bool = False, use_graph: bool = True, warmup: int = 2):
+                 transport: str = "p2p", stress: bool = False, heat_current: bool = False, use_graph: bool = True, warmup: int = 2,
+                 prune_edges: bool = False):
         inner = getattr(model, "model", model)
         if not hasattr(inner, "energy_and_forces"):
             raise NotImplementedError("DistributedCalculator needs a model with energy_and_forces (the fused CUDA model)")
@@ -815,7 +829,8 @@ class DistributedCalculator:
             raise ValueError(f"DistributedCalculator: {e}") from None
         self.box = [float(v) for v in torch.diagonal(c)] if self.geom.diagonal else None
         self.r_max, self.skin = float(r_max), float(skin)
-        self.r_list = self.r_max + self.skin
+        self._cutoffs = prune_table(inner, self.skin) if prune_edges else None
+        self.r_list = float(self._cutoffs.max()) if self._cutoffs is not None else self.r_max + self.skin
         self.width = self.geom.thickness
         if self.width < self.r_list:
             if self.geom.diagonal:
@@ -1027,7 +1042,7 @@ class DistributedCalculator:
         t3 = time.perf_counter()
         self.rebuild_seconds["ghosts"] += t3 - t2
         # 5. neighbour list on owned + ghosts with r_max + skin, rows for the owned centres
-        plan.build_list(torch.cat([local.pos, pos_ghost]).contiguous(), self.r_list)
+        plan.build_list(torch.cat([local.pos, pos_ghost]).contiguous(), self.r_list, self._cutoffs)
         self.plan = plan
         self.runner = DistributedAllegro(self.model, plan, p2p=self.p2p, stress=self.stress, atomic_virial=self.heat_current,
                                          heat_current=self.heat_current)

@@ -386,6 +386,29 @@ int ab2_nl_frames_fill(int pos_dtype, int64_t n, int64_t n_frames, const int32_t
                        const void* cell, const void* inv_cell, const int32_t* pbc, const int32_t* nimg, double r_max,
                        const int32_t* row_ptr, int32_t* nbr, void* shift, void* stream);
 
+/* Pruning of any centre-sorted list above (or a slab's local list) to per-edge-type list radii (the reference's
+ * per_edge_type_cutoff, allegro_models.py:42,122,156).  Edge z of row i (neighbour j = nbr[z], shift s = shift[z]) is
+ * kept iff
+ *   d2 < cut2[types[i] * num_types + types[j]],   d2 = ((dx * dx + dy * dy) + dz * dz),   d_x = (pos[j][x] + s[x]) - pos[i][x]
+ * every operation in fp64 with round-to-nearest and no contraction (fp32 positions and shifts convert exactly), so a
+ * restatement in any language gets the same bits.  cut2 [num_types][num_types] fp64 device table of SQUARED radii,
+ * directed: row = centre type, column = neighbour type.  An edge beyond its own cutoff r_ab contributes an exact zero to
+ * the model (x = r / r_ab >= 1), so with cut2 = (rmax_table + skin)^2 the pruned list gives the same energies, forces and
+ * virials as the list it came from.  Rows i in [0, n_centres) (row_ptr [n_centres + 1] int32, n_edges = row_ptr[n_centres]
+ * < 2^31 - 1); neighbours index the n >= n_centres atoms of pos [n][3] (fp64 or fp32; shift [n_edges][3] in the same
+ * dtype) and types [n] int32 in [0, num_types) (not checked here: the Python wrapper data.prune_csr checks them).
+ *   ab2_nl_prune_count: counts[i] = kept edges of row i                                         (one warp per row)
+ *   ab2_nl_prune_fill : the kept edges of row i at out_row_ptr[i], in their input order; out_nbr and out_shift are bitwise
+ *                       copies of nbr and shift
+ * Call order: ab2_nl_prune_count -> (host: out_row_ptr = prefix sum of counts) -> ab2_nl_prune_fill.  n_centres = 0 or
+ * n_edges = 0 launches nothing and writes nothing (every count is 0). */
+int ab2_nl_prune_count(int pos_dtype, int64_t n_centres, int64_t n_edges, int num_types, const void* pos, const int32_t* types,
+                       const double* cut2, const int32_t* row_ptr, const int32_t* nbr, const void* shift, int32_t* counts,
+                       void* stream);
+int ab2_nl_prune_fill(int pos_dtype, int64_t n_centres, int64_t n_edges, int num_types, const void* pos, const int32_t* types,
+                      const double* cut2, const int32_t* row_ptr, const int32_t* nbr, const void* shift,
+                      const int32_t* out_row_ptr, int32_t* out_nbr, void* out_shift, void* stream);
+
 /* Per-frame reductions (nequip's per-graph sums of a batch):
  *   ab2_frame_sum     out[b] = sum_{a in [frame_ptr[b], frame_ptr[b+1])} x[a]                 x [n], out [n_frames]
  *   ab2_frame_virial  W[b] = sum_{z in frame b} vec[z] (x) gvec[z]                 vec, gvec [E][3], W [n_frames][3][3]
