@@ -99,6 +99,11 @@ _SIGNATURES = {
     "ab2_frame_sum": ([_i32, _i64, _i64, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_frame_virial": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_frame_heat_current": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
+    "ab2_slots_check": ([_i32, _i64, _i64, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
+    "ab2_slots_count": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp], C.c_int),
+    "ab2_slots_place": ([_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_slots_fill": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_slots_transpose": ([_i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
 }
 
 
@@ -940,3 +945,62 @@ def frame_heat_current(e_atom: torch.Tensor, vel: torch.Tensor, W: torch.Tensor,
         _check(load().ab2_frame_heat_current(DTYPE_ENUM[W.dtype], n, B, _ptr(_contig(frame_ptr, "frame_ptr")), _ptr(e_atom), _ptr(vel),
                                              _ptr(_contig(W, "W")), _ptr(scratch), m, _ptr(J), _stream()))
     return J
+
+
+# --------------------------------------------------------------------------- #
+# Verlet lists of a batch of frames in fixed edge slots (ab2_slots_*): every output is a preallocated buffer written in
+# place, so the five launches of one rebuild can be captured into a graph.  Arguments as in include/allegro_b200.h; the
+# caller (calculator.BatchedCalculator) checks shapes and frame sizes once, when it builds the buffers.
+# --------------------------------------------------------------------------- #
+def slots_check(pos: torch.Tensor, pos_ref: torch.Tensor, frame_ptr: torch.Tensor, half_skin: float, frame_flag: torch.Tensor):
+    """frame_flag[b] = 1 when an atom of frame b moved more than ``half_skin`` from pos_ref (ab2_slots_check)."""
+    n, B = pos.shape[0], frame_ptr.shape[0] - 1
+    with _timed("slots_check"):
+        _check(load().ab2_slots_check(DTYPE_ENUM[pos.dtype], n, B, _ptr(_contig(frame_ptr, "frame_ptr")), _ptr(_contig(pos, "pos")),
+                                      _ptr(_contig(pos_ref, "pos_ref")), float(half_skin), _ptr(_contig(frame_flag, "frame_flag")), _stream()))
+
+
+def _slots_geom(frame_ptr, cell, inv_cell, pbc, nimg, r_list):
+    return (_ptr(_contig(frame_ptr, "frame_ptr")), _ptr(_contig(cell, "cell")), _ptr(_contig(inv_cell, "inv_cell")), _ptr(_contig(pbc, "pbc")),
+            _ptr(_contig(nimg, "nimg")), float(r_list))
+
+
+def slots_count(pos: torch.Tensor, frame_ptr, cell, inv_cell, pbc, nimg, r_list: float, frame_flag: torch.Tensor, counts: torch.Tensor):
+    """counts[i] = neighbours of centre i within r_list, for the atoms of flagged frames (ab2_slots_count)."""
+    n, B = pos.shape[0], frame_ptr.shape[0] - 1
+    fp, c, iv, pb, ni, r = _slots_geom(frame_ptr, cell, inv_cell, pbc, nimg, r_list)
+    with _timed("slots_count"):
+        _check(load().ab2_slots_count(DTYPE_ENUM[pos.dtype], n, B, fp, _ptr(_contig(pos, "pos")), c, iv, pb, ni, r,
+                                      _ptr(_contig(frame_flag, "frame_flag")), _ptr(_contig(counts, "counts")), _stream()))
+
+
+def slots_place(frame_ptr: torch.Tensor, slot_ptr: torch.Tensor, counts: torch.Tensor, frame_flag: torch.Tensor, row_ptr: torch.Tensor,
+                overflow: torch.Tensor, rebuilds: torch.Tensor):
+    """row_ptr of every flagged frame over its slot, or overflow (ab2_slots_place)."""
+    B = frame_ptr.shape[0] - 1
+    with _timed("slots_place"):
+        _check(load().ab2_slots_place(B, _ptr(_contig(frame_ptr, "frame_ptr")), _ptr(_contig(slot_ptr, "slot_ptr")), _ptr(_contig(counts, "counts")),
+                                      _ptr(_contig(frame_flag, "frame_flag")), _ptr(_contig(row_ptr, "row_ptr")), _ptr(_contig(overflow, "overflow")),
+                                      _ptr(_contig(rebuilds, "rebuilds")), _stream()))
+
+
+def slots_fill(pos: torch.Tensor, frame_ptr, cell, inv_cell, pbc, nimg, r_list: float, frame_flag: torch.Tensor, row_ptr: torch.Tensor,
+               pad: float, ctr: torch.Tensor, nbr: torch.Tensor, shift: torch.Tensor, pos_ref: torch.Tensor):
+    """Rows of the flagged frames (real edges, then padding) and pos_ref of their atoms (ab2_slots_fill)."""
+    n, B = pos.shape[0], frame_ptr.shape[0] - 1
+    fp, c, iv, pb, ni, r = _slots_geom(frame_ptr, cell, inv_cell, pbc, nimg, r_list)
+    with _timed("slots_fill"):
+        _check(load().ab2_slots_fill(DTYPE_ENUM[pos.dtype], n, B, fp, _ptr(_contig(pos, "pos")), c, iv, pb, ni, r,
+                                     _ptr(_contig(frame_flag, "frame_flag")), _ptr(_contig(row_ptr, "row_ptr")), float(pad),
+                                     _ptr(_contig(ctr, "ctr")), _ptr(_contig(nbr, "nbr")), _ptr(_contig(shift, "shift")),
+                                     _ptr(_contig(pos_ref, "pos_ref")), _stream()))
+
+
+def slots_transpose(frame_ptr: torch.Tensor, slot_ptr: torch.Tensor, nbr: torch.Tensor, frame_flag: torch.Tensor, col_ptr: torch.Tensor,
+                    col_perm: torch.Tensor, max_frame_atoms: int):
+    """col_ptr / col_perm of the flagged frames' slots; clears frame_flag (ab2_slots_transpose)."""
+    B = frame_ptr.shape[0] - 1
+    with _timed("slots_transpose"):
+        _check(load().ab2_slots_transpose(B, int(max_frame_atoms), _ptr(_contig(frame_ptr, "frame_ptr")), _ptr(_contig(slot_ptr, "slot_ptr")),
+                                          _ptr(_contig(nbr, "nbr")), _ptr(_contig(frame_flag, "frame_flag")), _ptr(_contig(col_ptr, "col_ptr")),
+                                          _ptr(_contig(col_perm, "col_perm")), _stream()))

@@ -432,6 +432,48 @@ int ab2_frame_virial(int acc_dtype, int64_t E, int64_t n_frames, const int32_t* 
 int ab2_frame_heat_current(int acc_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* e_atom,
                            const void* vel, const void* W, double* scratch, int64_t scratch_elems, void* J, void* stream);
 
+/* ---- Verlet lists of a batch of frames in fixed edge slots (molecular dynamics of many small frames) ---------------- */
+
+/* Largest frame of the slot kernels (and of data.FRAMES_MAX_ATOMS): ab2_slots_place covers a frame with one CTA. */
+#define AB2_FRAMES_MAX_ATOMS 4096
+
+/* Frame b owns the edges [slot_ptr[b], slot_ptr[b+1]) of one centre-sorted list (slot_ptr [n_frames+1] int32, rising from
+ * 0 to E, contiguous in frame order; an empty frame has an empty slot), so E never changes and a CUDA graph captured on
+ * the list stays valid while frames rebuild their rows inside it.  The rows of frame b partition its slot:
+ * row_ptr[frame_ptr[b]] = slot_ptr[b], row_ptr[frame_ptr[b+1]] = slot_ptr[b+1] (set once by the caller, never written
+ * here; row_ptr [n+1] int32).  Row i holds its real edges first, exactly the row of ab2_nl_frames_fill at r_max (by
+ * neighbour, then image), then padding self-edges (nbr = ctr = i, shift = (pad, 0, 0) with pad >= 2 r_max), which are
+ * longer than every cutoff and contribute exactly zero.  A frame's slack k = capacity - count is spread over its n_b
+ * atoms: atom l gets k / n_b + (l < k % n_b) padding edges.  Every launch takes the current stream, has a grid fixed by
+ * n and n_frames and is graph-capturable; the frames with frame_flag[b] != 1 leave at once.  frame_flag [n_frames] int32
+ * is 0 between rebuilds.  Frames hold at most AB2_FRAMES_MAX_ATOMS atoms (checked by the Python wrapper).
+ *   ab2_slots_check    : frame_flag[b] = 1 when an atom a of frame b has |pos[a] - pos_ref[a]| > half_skin, in the
+ *                        positions' dtype: d2 = (dx * dx + dy * dy) + dz * dz without contraction, then sqrt  (n threads)
+ *   ab2_slots_count    : counts[i] of ab2_nl_frames_count for the atoms of flagged frames              (one warp per centre)
+ *   ab2_slots_place    : one CTA per flagged frame.  count_b = sum of its counts; if count_b > capacity, *overflow += 1,
+ *                        frame_flag[b] = 2 and nothing else is written for the frame (its old rows stay, the caller
+ *                        must rebuild every slot); else row_ptr of its atoms over the slot and rebuilds[b] += 1
+ *   ab2_slots_fill     : nbr / shift of ab2_nl_frames_fill at row_ptr for flagged frames, ctr over each whole row, the
+ *                        padding edges, and pos_ref[a] = pos[a] for the frame's atoms                (one warp per centre)
+ *   ab2_slots_transpose: one CTA per flagged frame: col_ptr [n+1] / col_perm [E] of its slot (edge ids grouped by
+ *                        neighbour, ascending inside a group: bitwise EdgeCSR.transposed of the whole list; col_ptr[n] = E
+ *                        is the caller's); then frame_flag[b] = 0 for every frame.  max_frame_atoms >= every n_b sizes
+ *                        its shared memory, (8 + 1) * 4 * max_frame_atoms bytes.
+ * Call order of one rebuild: check -> count -> place -> fill -> transpose.  pos, pos_ref, cell, inv_cell and shift in one
+ * dtype (fp64 or fp32); cell, inv_cell, pbc, nimg as for ab2_nl_frames_count. */
+int ab2_slots_check(int pos_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* pos, const void* pos_ref,
+                    double half_skin, int32_t* frame_flag, void* stream);
+int ab2_slots_count(int pos_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* pos, const void* cell,
+                    const void* inv_cell, const int32_t* pbc, const int32_t* nimg, double r_max, const int32_t* frame_flag,
+                    int32_t* counts, void* stream);
+int ab2_slots_place(int64_t n_frames, const int32_t* frame_ptr, const int32_t* slot_ptr, const int32_t* counts,
+                    int32_t* frame_flag, int32_t* row_ptr, int32_t* overflow, int32_t* rebuilds, void* stream);
+int ab2_slots_fill(int pos_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* pos, const void* cell,
+                   const void* inv_cell, const int32_t* pbc, const int32_t* nimg, double r_max, const int32_t* frame_flag,
+                   const int32_t* row_ptr, double pad, int32_t* ctr, int32_t* nbr, void* shift, void* pos_ref, void* stream);
+int ab2_slots_transpose(int64_t n_frames, int max_frame_atoms, const int32_t* frame_ptr, const int32_t* slot_ptr,
+                        const int32_t* nbr, int32_t* frame_flag, int32_t* col_ptr, int32_t* col_perm, void* stream);
+
 /* Radial embedding with per-type-pair matrices: out[z][c] = sum_n B_n(x_z) PQ[t_c * T + t_n][n][c], B_n as above
  * (num_bessels must be 8, S <= 128).  PQ: [T*T][8][S] in the accumulate dtype.  The product embedding above is
  * PQ = typeemb(t_c,t_n)[c] * Wb[n][c]; because everything up to the first nonlinearity is linear
