@@ -3,13 +3,17 @@ replayed graph, and the energies, forces and stresses evaluated on them.
 
 1. Layout, bitwise: after the first build and after chosen frames move past skin / 2, row_ptr / ctr / nbr / shift /
    col_ptr / col_perm equal the restated layout (tests/slot_spec.py) of ``data.neighbor_csr_frames`` at r_list, and the
-   slots of frames that did not move are byte-identical to before.
+   slots of frames that did not move are byte-identical to before; on the mixed small frames, and on a dense 4096-atom
+   frame (rows and columns over 256 edges) next to one-atom, empty, 64-atom and triclinic 1176-atom frames.
 2. Outputs: frame by frame those of ``collate`` + ``energy_and_forces_frames`` on the exact-r_max list; a frame alone in
    a one-frame calculator gives its in-batch results (bitwise in fp32).
 3. A hot velocity-Verlet trajectory: forces at every step match a fresh exact-list evaluation, every frame rebuilds
    exactly when an AllegroCalculator of that frame alone rebuilds, and the graph is captured once.
-4. A frame compressed past its slot: right forces, one re-capture, the other frames unchanged.
+4. A frame compressed past its slot (a small cluster, or the 4096-atom frame): right forces, one re-capture, the other
+   frames unchanged.
 5. Launches per replay: the model's plus the rebuild's five."""
+import math
+
 import pytest
 import torch
 
@@ -76,10 +80,20 @@ def _kind(kind, g, r_max, ntypes):
         return _f(torch.zeros(1, 3, dtype=torch.float64), None, None, ntypes, g)
     if kind == "empty":
         return _f(torch.zeros(0, 3, dtype=torch.float64), None, None, ntypes, g)
+    if kind == "dense4096":  # the largest frame, ~340 neighbours per atom: rows and columns longer than 256 edges
+        side = (4096 / (340.0 / (4.0 / 3.0 * math.pi * (r_max + SKIN) ** 3))) ** (1.0 / 3.0)
+        cell = torch.diag(torch.tensor([side, side, side], dtype=torch.float64))
+        return _f(torch.rand(4096, 3, generator=g, dtype=torch.float64) @ cell, cell, None, ntypes, g)
+    if kind == "tri1176":  # triclinic, more than 1024 atoms: every thread of the place CTA holds atoms
+        pos, cell = systems._lattice(systems._FCC, 3.615, (7, 7, 6), 0.05, g)
+        shear = torch.tensor([[1.0, 0.0, 0.0], [0.21, 1.0, 0.0], [-0.15, 0.12, 1.0]], dtype=torch.float64)
+        return _f(pos @ shear, cell @ shear, None, ntypes, g)
     raise KeyError(kind)
 
 
 MIXED = ("si", "fcc_sheared", "hcp", "short_axis", "zero_row_sheet", "cluster", "one_atom", "empty")
+# the frame-size limit next to the smallest frames
+LARGE = ("dense4096", "one_atom", "empty", "si", "tri1176")
 
 
 def _frames(kinds, dtype, r_max, ntypes, seed):
@@ -92,7 +106,8 @@ def _frames(kinds, dtype, r_max, ntypes, seed):
 
 
 def _bytes(t):
-    return t.detach().contiguous().view(torch.uint8).cpu()
+    """the bytes of a tensor, flat: a slice [lo * w, hi * w) is entries [lo, hi) of its first dimension, w bytes each"""
+    return t.detach().contiguous().view(torch.uint8).reshape(-1).cpu()
 
 
 def _state(calc):
@@ -116,33 +131,40 @@ def _check_layout(calc, pos):
     assert calc.real_edges() == csr.num_edges
 
 
-@pytest.mark.parametrize("dtype", DTYPES, ids=DTYPE_IDS)
-def test_slots_equal_the_spec_and_untouched_frames_keep_their_bytes(dtype):
+# (dtype, frames, frames moved together at each step); the large batch moves its 4096-atom frame alone, then a small one
+LAYOUT_CASES = ([pytest.param(dt, MIXED, ([0, 3, 5],), id=i) for dt, i in zip(DTYPES, DTYPE_IDS)]
+                + [pytest.param(dt, LARGE, ([0], [3]), id="large-" + i) for dt, i in zip(DTYPES, DTYPE_IDS)])
+
+
+@pytest.mark.parametrize("dtype,kinds,moves", LAYOUT_CASES)
+def test_slots_equal_the_spec_and_untouched_frames_keep_their_bytes(dtype, kinds, moves):
     model, r_max, nt = _model(dtype)
-    frames = _frames(MIXED, dtype, r_max, nt, seed=1)
+    frames = _frames(kinds, dtype, r_max, nt, seed=1)
     calc = C.BatchedCalculator(model, frames, r_max, skin=SKIN)
     pos = torch.cat([f[D.POSITIONS_KEY] for f in frames]).clone()
     _check_layout(calc, pos)
     assert calc.frame_rebuilds() == [1] * len(frames)
     calc.compute(pos)
-    before = [_bytes(t) for t in _state(calc)]
     fp, sp = calc._fp_host, calc.slot_ptr.cpu().tolist()
-    moved = [0, 3, 5]  # si, short axis, cluster: one atom each past skin / 2
-    for b in moved:
-        pos[fp[b]] += torch.tensor([0.3, -0.1, 0.05], dtype=dtype, device=DEV)
-    calc.compute(pos)
-    torch.cuda.synchronize()
-    _check_layout(calc, pos)
-    assert calc.frame_rebuilds() == [2 if b in moved else 1 for b in range(len(frames))]
-    after = [_bytes(t) for t in _state(calc)]
-    for b in range(len(frames)):
-        if b in moved:
-            continue
-        for k, (x, y) in enumerate(zip(before, after)):
-            per_atom = k in (0, 4)
-            lo, hi = (fp[b], fp[b + 1]) if per_atom else (sp[b], sp[b + 1])
-            w = x.numel() // ((fp[-1] + 1) if per_atom else sp[-1])
-            assert torch.equal(x[lo * w:hi * w], y[lo * w:hi * w]), (b, k)
+    want = [1] * len(frames)
+    for moved in moves:  # one atom of each frame past skin / 2
+        before = [_bytes(t) for t in _state(calc)]
+        for b in moved:
+            pos[fp[b]] += torch.tensor([0.3, -0.1, 0.05], dtype=dtype, device=DEV)
+            want[b] += 1
+        calc.compute(pos)
+        torch.cuda.synchronize()
+        _check_layout(calc, pos)
+        assert calc.frame_rebuilds() == want
+        after = [_bytes(t) for t in _state(calc)]
+        for b in range(len(frames)):
+            if b in moved:
+                continue
+            for k, (x, y) in enumerate(zip(before, after)):
+                per_atom = k in (0, 4)
+                lo, hi = (fp[b], fp[b + 1]) if per_atom else (sp[b], sp[b + 1])
+                w = x.numel() // ((fp[-1] + 1) if per_atom else sp[-1])
+                assert torch.equal(x[lo * w:hi * w], y[lo * w:hi * w]), (b, k)
     assert calc.n_captures == 1
 
 
@@ -243,18 +265,24 @@ def test_hot_trajectory_rebuilds_like_single_frame_calculators():
     assert calc.n_captures == 1 and calc.n_overflows == 0
 
 
-@pytest.mark.parametrize("dtype", DTYPES, ids=DTYPE_IDS)
-def test_overflow_recaptures_once_and_never_returns_a_stale_force(dtype):
+# (dtype, frames, the frame compressed, by how much): the cluster to 0.3 of its size, or the periodic 4096-atom frame to
+# 0.7 (the gap the compression opens at the cell's faces leaves its list less than 0.7^-3 times longer)
+OVERFLOW_CASES = ([pytest.param(dt, MIXED, "cluster", 0.3, id=i) for dt, i in zip(DTYPES, DTYPE_IDS)]
+                  + [pytest.param(torch.float32, LARGE, "dense4096", 0.7, id="large-fp32")])
+
+
+@pytest.mark.parametrize("dtype,kinds,squeezed,factor", OVERFLOW_CASES)
+def test_overflow_recaptures_once_and_never_returns_a_stale_force(dtype, kinds, squeezed, factor):
     model, r_max, nt = _model(dtype)
-    frames = _frames(MIXED, dtype, r_max, nt, seed=6)
+    frames = _frames(kinds, dtype, r_max, nt, seed=6)
     calc = C.BatchedCalculator(model, frames, r_max, skin=SKIN)
     fp, B = calc._fp_host, len(frames)
     pos = torch.cat([f[D.POSITIONS_KEY] for f in frames]).clone()
     first = {k: v.clone() for k, v in calc.compute(pos).items()}
     cap0 = list(calc.capacity)
-    c = MIXED.index("cluster")
+    c = kinds.index(squeezed)
     p = pos[fp[c]:fp[c + 1]]
-    pos[fp[c]:fp[c + 1]] = p.mean(0) + 0.3 * (p - p.mean(0))
+    pos[fp[c]:fp[c + 1]] = p.mean(0) + factor * (p - p.mean(0))
     res = calc.compute(pos)
     assert calc.n_overflows == 1 and calc.n_captures == 2 and calc.capacity[c] > cap0[c]
     tol = 1e-9 if dtype == torch.float64 else 1e-4

@@ -8,6 +8,7 @@ rebuild kernels swapped for their torch restatement (tests/slot_spec.py), and it
   frame rebuilds), after small moves (nothing rebuilds), and after a frame outgrows its slot (every slot is re-sized once).
 * Every refusal is raised before any kernel is reached.
 The kernels themselves are held to the same layout on the GPU (tests/test_gpu_batched_md.py)."""
+import bisect
 import math
 
 import pytest
@@ -15,6 +16,7 @@ import torch
 
 import nlist_cases
 import nlist_lattice_cases
+import slot_cases
 import slot_spec
 from golden_util import unpack_state_dict
 from test_host_frames import MODELS, _models, _mixed_frames, spec_kernels  # noqa: F401  (spec_kernels is a fixture)
@@ -160,6 +162,78 @@ def test_slack_is_spread_over_the_atoms():
     assert slot_spec.pad_counts([5, 0, 2], 3, 7 + 8) == [5 + 3, 0 + 3, 2 + 2]
     assert slot_spec.pad_counts([1], 1, 17) == [17]
     assert slot_spec.pad_counts([0, 0, 0, 0], 4, 2) == [1, 1, 0, 0]
+
+
+# --------------------------------------------------------------------------- #
+# the restated place / transpose / check on the synthetic branch cases (tests/slot_cases.py) the GPU kernels are held to
+# bitwise: here the restatement itself is held to the contract, written out a second way
+# --------------------------------------------------------------------------- #
+@pytest.mark.parametrize("mode", list(slot_cases.PLACE_SLACK))
+def test_spec_place_follows_the_contract(mode):
+    c = slot_cases.place_case(mode)
+    flag0, rebuilds0 = c["frame_flag"].clone(), c["rebuilds"].clone()
+    slot_spec.slots_place(c["frame_ptr"], c["slot_ptr"], c["counts"], c["frame_flag"], c["row_ptr"], c["overflow"], c["rebuilds"])
+    fp, sp, counts, row_ptr = c["frame_ptr"].tolist(), c["slot_ptr"].tolist(), c["counts"].tolist(), c["row_ptr"].tolist()
+    over = 0
+    for b, nb in enumerate(c["sizes"]):
+        a0, a1, cap = fp[b], fp[b + 1], sp[b + 1] - sp[b]
+        count = sum(counts[a0:a1])
+        if int(flag0[b]) != 1:
+            assert int(c["frame_flag"][b]) == int(flag0[b]) and int(c["rebuilds"][b]) == int(rebuilds0[b])
+            assert row_ptr[a0:a1] == [slot_cases.SENTINEL] * nb, b
+            continue
+        if count > cap:
+            over += 1
+            assert int(c["frame_flag"][b]) == 2 and int(c["rebuilds"][b]) == int(rebuilds0[b])
+            assert row_ptr[a0:a1] == [slot_cases.SENTINEL] * nb, b
+            continue
+        assert int(c["frame_flag"][b]) == 1 and int(c["rebuilds"][b]) == int(rebuilds0[b]) + 1
+        if nb == 0:
+            continue
+        # row l holds counts[l] real edges and k // n_b (+ 1 for the first k % n_b atoms) padding edges
+        k = cap - count
+        ends = row_ptr[a0 + 1:a1] + [sp[b + 1]]
+        lens = [e - s for s, e in zip(row_ptr[a0:a1], ends)]
+        assert row_ptr[a0] == sp[b] and sum(lens) == cap
+        assert lens == [counts[a0 + l] + k // nb + (1 if l < k % nb else 0) for l in range(nb)], b
+    assert int(c["overflow"][0]) == over
+    assert (over > 0) == (mode == "one_over")
+
+
+@pytest.mark.parametrize("pattern", slot_cases.TRANSPOSE_PATTERNS)
+def test_spec_transpose_is_the_stable_column_sort(pattern):
+    c = slot_cases.transpose_case(pattern)
+    flag0 = c["frame_flag"].clone()
+    slot_spec.slots_transpose(c["frame_ptr"], c["slot_ptr"], c["nbr"], c["frame_flag"], c["col_ptr"], c["col_perm"], c["max_frame_atoms"])
+    assert c["frame_flag"].tolist() == [0] * len(c["sizes"])
+    fp, sp = c["frame_ptr"].tolist(), c["slot_ptr"].tolist()
+    nbr = c["nbr"].tolist()
+    for b, nb in enumerate(c["sizes"]):
+        s0, s1 = sp[b], sp[b + 1]
+        perm, cp = c["col_perm"][s0:s1].tolist(), c["col_ptr"][fp[b]:fp[b + 1]].tolist()
+        if int(flag0[b]) != 1:
+            assert perm == [slot_cases.SENTINEL] * (s1 - s0) and cp == [slot_cases.SENTINEL] * nb, b
+            continue
+        # edge ids grouped by neighbour, ascending inside a group; col_ptr[j] = s0 + edges on columns before j
+        want = sorted(range(s0, s1), key=lambda z: (nbr[z], z))
+        assert perm == want, b
+        cols = [nbr[z] for z in want]
+        assert cp == [s0 + bisect.bisect_left(cols, fp[b] + j) for j in range(nb)], b
+
+
+@pytest.mark.parametrize("skin", [0.5, 0.3, 1.0 / 3.0])
+@pytest.mark.parametrize("dtype", DTYPES, ids=DTYPE_IDS)
+def test_spec_check_flags_only_beyond_half_the_skin(dtype, skin):
+    pos, pos_ref, fp, half, want = slot_cases.check_case(dtype, skin)
+    # the cases are what they claim: exact single-axis displacements, h and the next value above it
+    h = torch.tensor(half, dtype=torch.float64).to(dtype)
+    d = (pos - pos_ref).abs().max(dim=1).values
+    assert torch.equal(((pos - pos_ref).abs() > 0).sum(1), torch.ones(pos.shape[0], dtype=torch.int64))
+    assert torch.equal(d > h, torch.tensor(want[:-1], dtype=torch.bool))
+    assert bool((d[torch.tensor(want[:-1]) == 0] <= h).all())
+    flag = torch.zeros(fp.shape[0] - 1, dtype=torch.int32)
+    slot_spec.slots_check(pos, pos_ref, fp, half, flag)
+    assert flag.tolist() == want
 
 
 # --------------------------------------------------------------------------- #
