@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Tuple
 
 import torch
 
@@ -99,6 +99,8 @@ _SIGNATURES = {
     "ab2_frame_sum": ([_i32, _i64, _i64, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_frame_virial": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_frame_heat_current": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
+    "ab2_frame_extrema": ([_i32, _i64, _i64, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
+    "ab2_committee_moments": ([_i32, _i32, _i64, _i32, C.POINTER(C.c_void_p), _vp, _vp, _vp], C.c_int),
     "ab2_slots_check": ([_i32, _i64, _i64, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_slots_count": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp], C.c_int),
     "ab2_slots_place": ([_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
@@ -945,6 +947,52 @@ def frame_heat_current(e_atom: torch.Tensor, vel: torch.Tensor, W: torch.Tensor,
         _check(load().ab2_frame_heat_current(DTYPE_ENUM[W.dtype], n, B, _ptr(_contig(frame_ptr, "frame_ptr")), _ptr(e_atom), _ptr(vel),
                                              _ptr(_contig(W, "W")), _ptr(scratch), m, _ptr(J), _stream()))
     return J
+
+
+def frame_extrema(x: torch.Tensor, frame_ptr: torch.Tensor) -> torch.Tensor:
+    """out[b] = (max, min, mean) of x over the atoms [frame_ptr[b], frame_ptr[b+1]) -> [B,3] in x's dtype, (0, 0, 0) for
+    an empty frame  (ab2_frame_extrema; fixed order, no atomics)."""
+    B = frame_ptr.shape[0] - 1
+    n = x.numel()
+    if x.dtype not in (torch.float64, torch.float32):
+        raise RuntimeError(f"allegro_b200: frame_extrema takes fp64 or fp32 values, got {x.dtype}")
+    if frame_ptr.dtype != torch.int32 or frame_ptr.device != x.device:
+        raise RuntimeError("allegro_b200: frame_ptr must be int32 on the values' device")
+    out = torch.empty(B, 3, dtype=x.dtype, device=x.device)
+    scratch, m = _frame_scratch(n, B, 3, x.device)
+    with _timed("frame_extrema", 2):
+        _check(load().ab2_frame_extrema(DTYPE_ENUM[x.dtype], n, B, _ptr(_contig(frame_ptr, "frame_ptr")), _ptr(_contig(x, "x")), _ptr(scratch), m,
+                                        _ptr(out), _stream()))
+    return out
+
+
+COMMITTEE_MAX_MEMBERS = 16  # AB2_COMMITTEE_MAX_MEMBERS
+
+
+def committee_moments(xs: Sequence[torch.Tensor], G: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Mean over the members ``xs`` (K tensors of one dtype, device and size, each read as [m][G]) and the population
+    deviation of every element's G-vector -> (mean in the shape of xs[0], dev [m])  (ab2_committee_moments; fixed member
+    order, fp64, bitwise reproducible).  K outside [1, COMMITTEE_MAX_MEMBERS] is refused by the kernel's entry point."""
+    xs = list(xs)
+    if not xs:
+        raise ValueError("committee_moments needs at least one member")
+    x0 = xs[0]
+    if x0.dtype not in (torch.float64, torch.float32):
+        raise RuntimeError(f"allegro_b200: committee_moments takes fp64 or fp32 values, got {x0.dtype}")
+    for k, x in enumerate(xs):
+        if x.dtype != x0.dtype or x.device != x0.device or x.numel() != x0.numel():
+            raise RuntimeError(f"allegro_b200: member {k} differs from member 0 in dtype, device or size")
+        _contig(x, f"member {k}")
+    G = int(G)
+    if G < 1 or x0.numel() % G:
+        raise RuntimeError(f"allegro_b200: {x0.numel()} values do not form rows of G = {G}")
+    m = x0.numel() // G
+    mean = torch.empty_like(x0)
+    dev = torch.empty(m, dtype=x0.dtype, device=x0.device)
+    ptrs = (C.c_void_p * len(xs))(*[_ptr(x).value for x in xs])
+    with _timed("committee_moments"):
+        _check(load().ab2_committee_moments(DTYPE_ENUM[x0.dtype], len(xs), m, G, ptrs, _ptr(mean), _ptr(dev), _stream()))
+    return mean, dev
 
 
 # --------------------------------------------------------------------------- #

@@ -33,12 +33,31 @@ from . import data as D
 
 
 def prune_table(model, skin: float) -> Optional[torch.Tensor]:
-    """``rmax_table + skin`` [T,T] fp64 on the CPU of a model built with per-edge-type cutoffs, else None."""
+    """``rmax_table + skin`` [T,T] fp64 on the CPU of a model built with per-edge-type cutoffs, else None.  For a
+    ``committee.Committee``, the elementwise max over its members, a member without per-edge-type cutoffs counting as
+    ``r_max + skin`` everywhere; None when no member has per-edge-type cutoffs."""
+    from .committee import Committee
+
     inner = getattr(model, "model", model)
+    if isinstance(inner, Committee):
+        tables = [prune_table(m, skin) for m in inner.members]
+        if all(t is None for t in tables):
+            return None
+        T = len(inner.type_names)
+        full = [t if t is not None else torch.full((T, T), float(getattr(m, "model", m).r_max) + float(skin), dtype=torch.float64)
+                for m, t in zip(inner.members, tables)]
+        return torch.stack(full).amax(dim=0)
     norm = getattr(inner, "edge_norm", None)
     if norm is None or not getattr(norm, "per_type", False):
         return None
     return norm.rmax_table.detach().to(device="cpu", dtype=torch.float64) + float(skin)
+
+
+def _committee_keys(out: D.Type, res: Dict[str, torch.Tensor]):
+    """The statistics of a ``committee.Committee`` model (data.COMMITTEE_KEYS), where the model wrote them."""
+    for k in D.COMMITTEE_KEYS:
+        if k in out:
+            res[k] = out[k]
 
 
 class AllegroCalculator:
@@ -139,8 +158,8 @@ class AllegroCalculator:
         is given: with ``cell=None`` no stress is returned, a singular cell (``data.is_regular_cell``) raises ValueError, and
         any other cell, however thin an open axis, divides the virial by its own volume;
         "atomic_virial" [N,3,3] with compute_atomic_virial; "heat_current" [1,3] with compute_heat_current, which needs
-        ``velocities`` [N,3]).  The returned tensors are the model's output buffers: with graph replay they are
-        overwritten by the next call."""
+        ``velocities`` [N,3]; with a ``committee.Committee`` as the model, also its statistics, data.COMMITTEE_KEYS).  The
+        returned tensors are the model's output buffers: with graph replay they are overwritten by the next call."""
         if self.compute_heat_current and (velocities is None or tuple(velocities.shape) != (pos.shape[0], 3)):
             raise ValueError(f"compute_heat_current needs velocities [{pos.shape[0]},3]")
         if self._needs_rebuild(pos, cell, atom_types):
@@ -165,6 +184,7 @@ class AllegroCalculator:
             res["atomic_virial"] = out[D.ATOMIC_VIRIAL_KEY]
         if self.compute_heat_current:
             res["heat_current"] = out[D.HEAT_CURRENT_KEY]
+        _committee_keys(out, res)
         return res
 
     @property
@@ -352,7 +372,8 @@ class BatchedCalculator:
     # ---- evaluation ----------------------------------------------------------------------------
     def compute(self, pos: torch.Tensor) -> Dict[str, torch.Tensor]:
         """-> {"energy" [B,1], "forces" [N,3], "atomic_energy" [N,1]} (+ "stress", "virial" [B,3,3] with compute_stress)
-        for the positions ``pos`` [N,3] of every frame, back to back in the frames' order.  The returned tensors are the
+        for the positions ``pos`` [N,3] of every frame, back to back in the frames' order (with a ``committee.Committee``
+        as the model, also its statistics, data.COMMITTEE_KEYS).  The returned tensors are the
         graph's output buffers: the next call overwrites them.  Costs one device-to-host read (the overflow count)."""
         if not isinstance(pos, torch.Tensor) or tuple(pos.shape) != (self.num_atoms, 3):
             raise ValueError(f"pos must be [{self.num_atoms},3] (the atoms of every frame back to back), got "
@@ -371,6 +392,7 @@ class BatchedCalculator:
         res = {"energy": out[D.TOTAL_ENERGY_KEY], "forces": out[D.FORCE_KEY], "atomic_energy": out[D.PER_ATOM_ENERGY_KEY]}
         if self.compute_stress:
             res["stress"], res["virial"] = out[D.STRESS_KEY], out[D.VIRIAL_KEY]
+        _committee_keys(out, res)
         return res
 
     # ---- state, for tests and timing -------------------------------------------------------

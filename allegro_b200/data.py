@@ -49,6 +49,19 @@ EDGE_SHIFT_VEC_KEY = "edge_shift_vec"
 VELOCITY_KEY = "velocities"
 ATOMIC_VIRIAL_KEY = "atomic_virial"
 HEAT_CURRENT_KEY = "heat_current"
+# committee statistics (committee.Committee; DP-GEN's model deviation): each member's total energy [K,B], the deviation
+# over the members of the total energy [B,1], of every per-atom energy [N,1] and of every virial component [B,3,3], the
+# per-atom force deviation sigma_F [N], and its max / min / mean over each frame's atoms [B]
+COMMITTEE_ENERGY_KEY = "committee_energy"
+ENERGY_STD_KEY = "energy_std"
+ATOMIC_ENERGY_STD_KEY = "atomic_energy_std"
+FORCE_DEVIATION_KEY = "force_deviation"
+MAX_FORCE_DEVIATION_KEY = "max_force_deviation"
+MIN_FORCE_DEVIATION_KEY = "min_force_deviation"
+MEAN_FORCE_DEVIATION_KEY = "mean_force_deviation"
+VIRIAL_STD_KEY = "virial_std"
+COMMITTEE_KEYS = (COMMITTEE_ENERGY_KEY, ENERGY_STD_KEY, ATOMIC_ENERGY_STD_KEY, FORCE_DEVIATION_KEY, MAX_FORCE_DEVIATION_KEY,
+                  MIN_FORCE_DEVIATION_KEY, MEAN_FORCE_DEVIATION_KEY, VIRIAL_STD_KEY)
 
 Type = Dict[str, torch.Tensor]
 

@@ -431,6 +431,31 @@ int ab2_frame_virial(int acc_dtype, int64_t E, int64_t n_frames, const int32_t* 
  * the caller's. */
 int ab2_frame_heat_current(int acc_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* e_atom,
                            const void* vel, const void* W, double* scratch, int64_t scratch_elems, void* J, void* stream);
+/* Extrema and mean of a per-atom value over every frame:
+ *   out[b][0] = max, out[b][1] = min, out[b][2] = (sum) / n_b   of x[a], a in [frame_ptr[b], frame_ptr[b+1])
+ * x [n], out [n_frames][3], in the accumulate dtype (fp64 or fp32; compared and summed in fp64, each output rounded once),
+ * with the chunking of the reductions above (a frame's result does not depend on the launch or on the other frames); an
+ * empty frame gives (0, 0, 0).  scratch: at least ab2_frame_scratch_elems(n, n_frames) * 3 elements.  With the committee's
+ * per-atom force deviation this is DP-GEN's max_devi_f / min_devi_f / avg_devi_f. */
+int ab2_frame_extrema(int acc_dtype, int64_t n, int64_t n_frames, const int32_t* frame_ptr, const void* x, double* scratch,
+                      int64_t scratch_elems, void* out, void* stream);
+
+/* ---- committees of models: statistics over the members' outputs ---------------------------------------------------- */
+
+#define AB2_COMMITTEE_MAX_MEMBERS 16
+
+/* Mean and population deviation over K members of a field laid out [m][G] in every member (x: K host-held device
+ * pointers, read by value at the launch, so the call is graph-capturable as it is):
+ *   mean[i][g] = mu[i][g] = (1/K) sum_k x_k[i][g]
+ *   dev[i]     = sqrt( sum_g (1/K) sum_k (x_k[i][g] - mu[i][g])^2 )          (np.std's population form)
+ * In fp64, members summed in member order in two passes (the deviations use the unrounded fp64 mu), every step an explicit
+ * round-to-nearest add / sub / mul / div / sqrt (no FMA contraction): sum and square-sum start from member 0, mu = sum / K,
+ * each g's square-sum is divided by K, the g terms are added in g order.  Each output is rounded once to dtype (AB2_F64 /
+ * AB2_F32, the dtype of every x_k, mean [m][G] and dev [m]).  K = 1 gives mean = x_0 and dev = 0 exactly.  G = 3 of
+ * per-atom forces is the per-atom force deviation; G = 1 the deviation of each energy or virial component.  Refuses
+ * K outside [1, AB2_COMMITTEE_MAX_MEMBERS], G < 1, m < 0, a null x and (for m > 0) null data pointers; launches nothing
+ * for m = 0. */
+int ab2_committee_moments(int dtype, int K, int64_t m, int G, const void* const* x, void* mean, void* dev, void* stream);
 
 /* ---- Verlet lists of a batch of frames in fixed edge slots (molecular dynamics of many small frames) ---------------- */
 
