@@ -171,6 +171,8 @@ class TwoBodySphericalHarmonicTensorEmbed(torch.nn.Module):
         super().__init__()
         irreps = Irreps.spherical_harmonics(irreps_edge_sh) if isinstance(irreps_edge_sh, int) else Irreps(irreps_edge_sh)
         lmax = irreps.lmax
+        if lmax > 4:  # AB2_MAX_LMAX (include/allegro_b200.h): the kernels are instantiated for l_max 0..4
+            raise NotImplementedError(f"l_max = {lmax}: the kernels support l_max <= 4")
         if repr(irreps) != repr(Irreps.spherical_harmonics(lmax)):
             raise NotImplementedError(f"irreps_edge_sh must be the full SH set 0..l_max with parity (-1)^l, got {irreps}")
         if edge_sh_normalization != "component" or not edge_sh_normalize:

@@ -35,11 +35,12 @@ def sh_fwd(vec, lmax):
 
 
 def sh_bwd(vec, gY, lmax, out=None, accumulate=False):
-    if vec.shape[0] == 0:
-        return torch.zeros_like(vec) if out is None else out
-    v = vec.detach().clone().requires_grad_(True)
-    with torch.enable_grad():
-        (g,) = torch.autograd.grad(sh_fwd(v, lmax), v, gY)
+    if vec.shape[0] == 0 or lmax == 0:  # Y_0 is a constant: no gradient reaches the edge vectors
+        g = torch.zeros_like(vec)
+    else:
+        v = vec.detach().clone().requires_grad_(True)
+        with torch.enable_grad():
+            (g,) = torch.autograd.grad(sh_fwd(v, lmax), v, gY)
     if out is None:
         return g
     out.copy_(out + g if accumulate else g)

@@ -19,26 +19,30 @@ def spec_kernels(monkeypatch):
         monkeypatch.setattr(_lib, name, getattr(kernel_spec, name))
 
 
+# l_max 2; l_max 4 with the parity-doubled output of an inner Allegro layer (25 x 25 -> 49: 2052 table entries)
+IRREPS = [("0e + 1o + 2e",) * 3, ("0e + 1o + 2e + 3o + 4e", "0e + 1o + 2e + 3o + 4e", "0e + 1e + 1o + 2e + 2o + 3e + 3o + 4e + 4o")]
+
+
+@pytest.mark.parametrize("irreps", IRREPS, ids=["lmax2", "lmax4"])
 @pytest.mark.parametrize("sorted_idx", [False, True], ids=["generic", "sorted"])
 @pytest.mark.parametrize("coupling", [True, False])
-def test_operator_first_and_second_order_on_cpu(spec_kernels, coupling, sorted_idx):
+def test_operator_first_and_second_order_on_cpu(spec_kernels, coupling, sorted_idx, irreps):
     from allegro_b200.nn import B200Contracter
 
     prev = torch.get_default_dtype()
     torch.set_default_dtype(torch.float64)
     try:
         torch.manual_seed(5)
-        sh = "0e + 1o + 2e"
-        ir = o3_ref.Irreps(sh)
+        i1, i2, io = (o3_ref.Irreps(x) for x in irreps)
         mul, E, N = 3, 19, 5
-        c_base = R.Contracter(ir, ir, ir, mul=mul, path_channel_coupling=coupling, scatter_factor=0.41)
-        c_k = B200Contracter(sh, sh, sh, mul=mul, instructions=c_base.instructions, path_channel_coupling=coupling, scatter_factor=0.41)
+        c_base = R.Contracter(i1, i2, io, mul=mul, path_channel_coupling=coupling, scatter_factor=0.41)
+        c_k = B200Contracter(*irreps, mul=mul, instructions=c_base.instructions, path_channel_coupling=coupling, scatter_factor=0.41)
         c_k.load_state_dict(c_base.state_dict())
         idx = torch.randint(0, N, (E,))
         if sorted_idx:
             idx = torch.sort(idx).values
-        x1, x2 = torch.randn(E, mul, ir.dim), torch.randn(E, mul, ir.dim)
-        go, v1, v2 = torch.randn(E, mul, ir.dim), torch.randn(E, mul, ir.dim), torch.randn(E, mul, ir.dim)
+        x1, x2 = torch.randn(E, mul, i1.dim), torch.randn(E, mul, i2.dim)
+        go, v1, v2 = torch.randn(E, mul, io.dim), torch.randn(E, mul, i1.dim), torch.randn(E, mul, i2.dim)
 
         def losses(fwd, weights):
             a, b = x1.clone().requires_grad_(True), x2.clone().requires_grad_(True)

@@ -25,7 +25,12 @@ TOL = 1e-4
 # l_max = 3 in fp32 runs the shape-generic tensor-product kernels (tp.cu) on a 353-entry layer-0 table, with fp32
 # atomics; the same templates meet 1e-9 in fp64 (test_gpu_model.test_c5_lmax3_three_layers_fp64).  Measured force
 # errors on an H100: 1.25e-4 (3^3 cell) and 1.13e-4 (5^3 cell) of max |F|; energies meet 1e-4.
-TOL_F = {"lmax3": 2e-4}
+# l_max 4 runs the same generic kernels on tables of 1158 (L = 2) and 2052 entries (L = 3); measured on an H100 (700 W) at
+# 3^3 in two runs: forces 2.55e-5 / 2.60e-5 (L = 2) and 7.68e-5 / 8.11e-5 (L = 3) of max |F|, energies 3.1e-5 / 2.4e-5.
+# The bars are 1.5x the larger measurement.  The same fp32 models
+# through the host pipeline with the kernels' torch restatement in fp32 on the CPU (tests/kernel_spec.py) land at 5.7e-6 /
+# 1.3e-5: the CUDA error is 5-9x that at every l_max (lmax0, lmax1 and lmax3 alike), so it is not the l_max 4 tables.
+TOL_F = {"lmax3": 2e-4, "lmax4": 4e-5, "lmax4_L3": 1.2e-4}
 
 # c2 widths (S = H = readout hidden width = 64, U = 32, l_max = 2, L = 2), then per case the overrides, and whether the
 # opt-in plain-GEMM backward is switched on
@@ -51,6 +56,9 @@ CASES = {
     "three_species": dict(C3_AT_C2_WIDTHS, per_type_energy_scales=[2.5, 0.5, 1.25], per_type_energy_shifts=[-1.25, 0.5, 2.0],
                           per_edge_type_cutoff={"Li": 4.0, "P": {"Li": 5.0, "P": 4.5, "S": 6.0}, "S": 5.5}),
     "plain_bwd_L3": dict(num_layers=3),
+    "lmax0": dict(l_max=0),
+    "lmax4": dict(l_max=4),
+    "lmax4_L3": dict(l_max=4, num_layers=3),
 }
 PLAIN_BWD = {"plain_bwd_L3"}
 
@@ -127,6 +135,18 @@ DISPATCH = {
     "three_species": C2,
     # the plain-GEMM backward runs no fused MLP kernel; its forward is that of L3_U32
     "plain_bwd_L3": {"fwd.L0": "mlp2+", "fwd.L1": "mlp2+", "fwd.L2": "ro- mlp2+", "fwd.readout": "mlp2+"},
+    # l_max 0 and 4: no composed tensor products either; the env weights are (l_max + 1) U wide, so the first latent MLP is
+    # 96 x 64 -> 96 and 96 x 64 -> 224 (S + 5U, under the four-chunk limit) and its backward 96 / 224 x 64 -> 96; the fused
+    # readout depends on (L, U) only: taken at (2, 32), declined at (3, 32) as in L3_U32
+    "lmax0": {"fwd.L0": "mlp2+", "fwd.L1": "ro+", "bwd.readout": "ro+", "bwd.L0": "mlp2+"},
+    "lmax4": {"fwd.L0": "mlp2+", "fwd.L1": "ro+", "bwd.readout": "ro+", "bwd.L0": "mlp2+"},
+    "lmax4_L3": {
+        "fwd.L0": "mlp2+", "fwd.L1": "mlp2+",  # both write S + 5U = 224 columns
+        "fwd.L2": "ro- mlp2+",         # ro: 260 224 bytes; 224 x 64 -> 64
+        "fwd.readout": "mlp2+",
+        "bwd.readout": "ro- mlp2+",    # ro: 259 200 bytes
+        "bwd.L2": "mlp2+", "bwd.L1": "mlp2+", "bwd.L0": "mlp2+",
+    },
 }
 # A frame without edges: the direct path, and the torch.autograd path (use_autograd), return zeros before any kernel
 NO_EDGES_AUTOGRAD = {"L2_U32": {}, "L1_U32": {}}
@@ -137,7 +157,7 @@ SPIED = {"mlp2": "mlp2", "mlp2_readout": "ro", "tp_chain_fwd": "chain", "tp_chai
 def _frames(case):
     if case == "three_species":
         return ["c3_4", "c3_6"]
-    frames = ["c2_3", "c2_5"]
+    frames = ["c2_3", "c2_5"] if not case.startswith("lmax4") else ["c2_3"]  # the fp64 oracle at l_max 4 takes ~20 s at 3^3
     if case in NO_EDGES_AUTOGRAD:
         frames += ["isolated_atoms_ragged_rows", "no_edges_at_all"]
     return frames

@@ -31,7 +31,7 @@ def _csr_random(N, E, seed=0):
     return D.build_csr(ei.to(DEV), N), ctr
 
 
-@pytest.mark.parametrize("lmax", [1, 2, 3, 4])
+@pytest.mark.parametrize("lmax", [1, 2, 3, 4, 0])
 @pytest.mark.parametrize("dtype", [torch.float64, torch.float32])
 def test_sh_fwd_bwd(lmax, dtype):
     g = torch.Generator().manual_seed(lmax)
@@ -40,8 +40,11 @@ def test_sh_fwd_bwd(lmax, dtype):
     Y = _lib.sh_fwd(vec.to(DEV, dtype), lmax)
     assert _rel(Y, Yr) < TOL[dtype]
     gY = torch.randn(1000, (lmax + 1) ** 2, generator=g, dtype=torch.float64)
-    v = vec.clone().requires_grad_(True)
-    (gr,) = torch.autograd.grad((o3_ref.spherical_harmonics(lmax, v) * gY).sum(), v)
+    if lmax == 0:  # Y_0 is a constant
+        gr = torch.zeros_like(vec)
+    else:
+        v = vec.clone().requires_grad_(True)
+        (gr,) = torch.autograd.grad((o3_ref.spherical_harmonics(lmax, v) * gY).sum(), v)
     gv = _lib.sh_bwd(vec.to(DEV, dtype), gY.to(DEV, dtype), lmax)
     assert _rel(gv, gr) < TOL[dtype] * 10
     # accumulate mode
@@ -174,13 +177,14 @@ def test_linear_prologue_mul_dsilu(dtype, shape):
         assert _rel(out, ref) < tol
 
 
-@pytest.mark.parametrize("lmax", [1, 2, 3])
+@pytest.mark.parametrize("lmax", [1, 2, 3, 0, 4])
 @pytest.mark.parametrize("U", [4, 32, 48, 64])
 @pytest.mark.parametrize("dtype", [torch.float64, torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("fastpath", [True, False, "dense"])
 def test_env_sum_and_bwd(lmax, U, dtype, fastpath):
     """fastpath "dense": contiguous w / gw rows, what the pipeline passes -- the TMA-staged streaming adjoint
-    (env_stream.cu) takes these; the strided views exercise the round-1 kernels."""
+    (env_stream.cu) takes these; the strided views exercise the round-1 kernels.  l_max 0 runs env_bwd_fast_kernel with
+    one value per warp reduction; l_max 4 is past both fast adjoints and runs env_bwd_kernel<..., 4> whatever the options."""
     dense = fastpath == "dense"
     fastpath = bool(fastpath)
     N, E = 37, 600
@@ -263,7 +267,10 @@ def tp_fast(request):
     _lib.set_option("tp_stream_gytile", 1)
 
 
-@pytest.mark.parametrize("case", [(1, 0, 1), (2, 0, 2), (2, 1, 2), (3, 0, 3), (3, 1, 3), (3, 2, 3), (1, 0, 2), (1, 1, 3)])
+# (l_max, layer, L); the l_max 4 cases are the tables 25 -> 25 (1158 entries), 25 -> 49, 49 -> 25 (2052 each) and 25 -> 1,
+# which no fast family takes: every option set must land on the shape-generic kernels; l_max 0 is the 1 x 1 x 1 table
+@pytest.mark.parametrize("case", [(1, 0, 1), (2, 0, 2), (2, 1, 2), (3, 0, 3), (3, 1, 3), (3, 2, 3), (1, 0, 2), (1, 1, 3),
+                                  (4, 0, 2), (4, 0, 3), (4, 1, 3), (4, 2, 3), (0, 0, 2), (0, 1, 2)])
 @pytest.mark.parametrize("coupling", [True, False])
 @pytest.mark.parametrize("dtype", [torch.float64, torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("U", [8, 32, 40])
@@ -299,7 +306,7 @@ def test_tp_fwd_bwd_explicit(case, coupling, dtype, U, tp_fast):
     assert _rel(ggam.transpose(1, 2), ggam_ref) < (tol if dtype != torch.bfloat16 else 1e-5)
 
 
-@pytest.mark.parametrize("lmax", [1, 2, 3])
+@pytest.mark.parametrize("lmax", [1, 2, 3, 0, 4])
 @pytest.mark.parametrize("dtype", [torch.float64, torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("U", [8, 32, 40])
 def test_tp_fwd_bwd_implicit_v0(lmax, dtype, U, tp_fast):
@@ -335,6 +342,82 @@ def test_tp_fwd_bwd_implicit_v0(lmax, dtype, U, tp_fast):
     assert _rel(gw0, gw_ref) < tol
     assert _rel(gY, gY_ref) < (tol if dtype != torch.bfloat16 else 1e-5)
     assert _rel(ggam.transpose(1, 2), ggam_ref) < (tol if dtype != torch.bfloat16 else 1e-5)
+
+
+@pytest.mark.parametrize("dtype", [torch.float64, torch.float32])
+@pytest.mark.parametrize("layer", [0, 1, 2])
+def test_tp_lmax4_ragged_generic(layer, dtype):
+    """l_max 4, L = 3 (25 -> 49, 49 -> 25, 25 -> 1; layer 0 with implicit input features) on a ragged CSR: empty centres
+    (the first, the last and one run in the middle) and one centre of 300 edges, U = 64 (two channel chunks).  Held to the
+    oracle's autograd.  Which kernels serve these tables is checked with torch.profiler in
+    test_gpu_tp_ragged.test_lmax4_tables_run_the_generic_kernels."""
+    lmax, L, U, N = 4, 3, 64, 29
+    c, b = _tp_case(lmax, layer, L, U, True, dtype)
+    g = torch.Generator().manual_seed(40 + layer)
+    deg = torch.randint(0, 12, (N,), generator=g)
+    deg[0] = deg[-1] = 0
+    deg[9:12] = 0
+    deg[17] = 300
+    ctr = torch.repeat_interleave(torch.arange(N), deg)
+    E = int(ctr.numel())
+    csr = D.build_csr(torch.stack([ctr, torch.randint(0, N, (E,), generator=g)]).to(DEV), N)
+    acc = _lib.ACC_DTYPE[dtype]
+    implicit = layer == 0
+    d_in, d_out, Dd, n_ir = c.base_dim1, c.base_dim_out, (lmax + 1) ** 2, lmax + 1
+    dd = dict(dtype=torch.float64, generator=g)
+    Y = torch.randn(E, Dd, **dd).to(acc).double()
+    w0 = torch.randn(E, n_ir * U, **dd).to(dtype).double()
+    V = torch.randn(E, U, d_in, **dd).to(dtype).double()
+    gam = torch.randn(N, U, Dd, **dd).to(acc).double()
+    gout = torch.randn(E, U, d_out, **dd).to(dtype).double()
+    leaves = [t.clone().requires_grad_(True) for t in ((Y, w0) if implicit else (V,))] + [gam.clone().requires_grad_(True)]
+    if implicit:
+        m = R.MakeWeightedChannels(o3_ref.Irreps.spherical_harmonics(lmax), U)
+        Vin_ref = m(leaves[0], leaves[1].view(E, n_ir, U).transpose(1, 2).reshape(E, -1))
+    else:
+        Vin_ref = leaves[0]
+    out_ref = c._contract(Vin_ref, leaves[-1][ctr])
+    grads_ref = torch.autograd.grad((out_ref * gout).sum(), leaves)
+    ijk, _, _ = b.sparse_table()
+    tab, cgw = ijk.to(DEV), b.cgw(acc, DEV)
+    gi = gam.transpose(1, 2).contiguous().to(DEV, acc)
+    Yd, wd = Y.to(DEV, acc), w0.to(DEV, dtype)
+    Vi = None if implicit else V.transpose(1, 2).contiguous().to(DEV, dtype)
+    go = gout.transpose(1, 2).contiguous().to(DEV, dtype)
+    Vout = torch.empty(E, d_out, U, device=DEV, dtype=dtype)
+    _lib.tp_fwd(dtype, lmax, N, E, U, d_in, d_out, tab, cgw, csr.row_ptr, csr.ctr, gi, Vi, Yd if implicit else None,
+                wd if implicit else None, Vout)
+    gVin = None if implicit else torch.empty(E, d_in, U, device=DEV, dtype=dtype)
+    gw0 = torch.empty(E, n_ir * U, device=DEV, dtype=dtype) if implicit else None
+    gY = torch.zeros(E, Dd, device=DEV, dtype=acc) if implicit else None
+    ggam = torch.full((N, Dd, U), float("nan"), device=DEV, dtype=acc)
+    _lib.tp_bwd(dtype, lmax, N, E, U, d_in, d_out, tab, cgw, csr.row_ptr, csr.ctr, gi, Vi, Yd if implicit else None,
+                wd if implicit else None, go, gVin, gw0, gY, ggam)
+    grads = [t for t in (gY, gw0, gVin) if t is not None] + [ggam]
+    tol = {torch.float64: 1e-12, torch.float32: 2e-5}[dtype]
+    assert _rel(Vout.transpose(1, 2), out_ref.detach()) < tol
+    if implicit:
+        got = [grads[0], grads[1], grads[2].transpose(1, 2)]
+    else:
+        got = [grads[0].transpose(1, 2), grads[1].transpose(1, 2)]
+    for name, a, r in zip(("gY", "gw0", "ggamma") if implicit else ("gVin", "ggamma"), got, grads_ref):
+        assert _rel(a, r) < tol, (name, _rel(a, r))
+    # empty centres own no edges: their gamma gradient is exactly zero
+    assert (grads[-1][deg.to(DEV) == 0] == 0).all()
+
+
+def test_lmax_above_4_is_refused_by_the_library():
+    """l_max 5 has no kernel instantiation: the argument checks refuse it with the library's message before any launch."""
+    vec = torch.randn(10, 3, device=DEV, dtype=torch.float64)
+    with pytest.raises(RuntimeError, match="lmax 5 not supported"):
+        _lib.sh_fwd(vec, 5)
+    N, E, U, Dd = 2, 4, 8, 36
+    csr = D.build_csr(torch.tensor([[0, 0, 1, 1], [1, 1, 0, 0]], device=DEV), N)
+    f64 = dict(device=DEV, dtype=torch.float64)
+    tab = torch.zeros(1, 3, device=DEV, dtype=torch.int32)
+    with pytest.raises(RuntimeError, match="bad argument: lmax"):
+        _lib.tp_fwd(torch.float64, 5, N, E, U, 1, 1, tab, torch.ones(1, U, **f64), csr.row_ptr, csr.ctr, torch.zeros(N, Dd, U, **f64),
+                    torch.zeros(E, 1, U, **f64), None, None, torch.empty(E, 1, U, **f64))
 
 
 @pytest.mark.parametrize("layer", [0, 1, 2])
@@ -455,7 +538,8 @@ def test_contract_kernel_vs_base(irreps_in1, irreps_in2, irreps_out, coupling, m
 
 @pytest.mark.parametrize("sorted_idx", [False, True], ids=["generic", "sorted"])
 @pytest.mark.parametrize("coupling", [True, False])
-@pytest.mark.parametrize("irreps", [("0e + 1o + 2e", "0e + 1o + 2e", "0e + 1o + 2e"), ("2o + 1e + 0e", "0e + 0o + 1e + 1o", "1o + 2e")])
+@pytest.mark.parametrize("irreps", [("0e + 1o + 2e", "0e + 1o + 2e", "0e + 1o + 2e"), ("2o + 1e + 0e", "0e + 0o + 1e + 1o", "1o + 2e"),
+                                    ("0e + 1o + 2e + 3o + 4e", "0e + 1o + 2e + 3o + 4e", "0e + 1e + 1o + 2e + 2o + 3e + 3o + 4e + 4o")])
 def test_contracter_weight_grad_and_double_backward(irreps, coupling, sorted_idx):
     """Training support (SURVEY row f4): the reference's ``weights`` are Parameters and its einsum path is differentiable
     to any order through autograd (_contract.py:170-177, 213-251).  The B200 operator builds every derivative from four
@@ -490,7 +574,7 @@ def test_contracter_weight_grad_and_double_backward(irreps, coupling, sorted_idx
 
         ref, got = losses(c_base, "cpu"), losses(c_k, DEV)
         route = c_k._tab_cache.get("route")
-        assert (route is not None and route[3] is not None) == (sorted_idx and i2.dim == 9)
+        assert (route is not None and route[3] is not None) == (sorted_idx and i2.dim in (9, 25))
         for name, r, g in zip(("out", "dL/dw", "dL/dx1", "dL/dx2", "d2/dw", "d2/dx1", "d2/dx2"), ref, got):
             assert g.shape == r.shape, name
             assert _rel(g, r) < 1e-10, (name, float(_rel(g, r)))

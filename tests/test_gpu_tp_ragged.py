@@ -333,7 +333,7 @@ def _check_kernels(names, fwd, bwd):
         for fam, args in want.items():
             got = [_template_args(n, fam) for n in names if _template_args(n, fam) is not None]
             exp = [str(a) for a in args]
-            assert any(g[-len(exp):] == exp for g in got), (fam, exp, got)
+            assert any(g[len(g) - len(exp):] == exp for g in got), (fam, exp, got)  # exp may be empty (generic kernels)
 
 
 # --------------------------------------------------------------------------------------------------------------------
@@ -711,3 +711,95 @@ def test_c3_widths_bf16():
     assert core.U == 64 and core.chain is None
     ee, ef = _check(oracle, model, d, 2e-2, 5e-2)
     print(f"c3 widths bf16: E {ee:.2e} F {ef:.2e}")
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# GPU: which kernels serve the l_max 4 tables (values: test_gpu_kernels.test_tp_lmax4_ragged_generic and the explicit /
+# implicit grids there)
+# --------------------------------------------------------------------------------------------------------------------
+LMAX4_TABLES = {"25to25": (2, 0), "25to49": (3, 0), "49to25": (3, 1), "25to1": (3, 2)}  # (L, layer) of an l_max 4 model
+LMAX4_DTYPES = {"float64": torch.float64, "float32": torch.float32, "bfloat16": torch.bfloat16}
+
+
+def _lmax4_trace(table, dtype):
+    """(d_in, d_out, D, implicit, nnz, names of the kernels ab2_tp_fwd + ab2_tp_bwd launch under the default options) of one
+    l_max 4 table on a small ragged CSR with empty centres."""
+    from test_gpu_kernels import _tp_case
+
+    L, layer = LMAX4_TABLES[table]
+    lmax, U, N = 4, 32, 9
+    _, b = _tp_case(lmax, layer, L, U, True, dtype)
+    implicit = layer == 0
+    d_in, d_out, Dd = b.base_dim1, b.base_dim_out, (lmax + 1) ** 2
+    ijk, _, _ = b.sparse_table()
+    acc = _lib.ACC_DTYPE[dtype]
+    tab, cgw = ijk.to(DEV), b.cgw(acc, DEV)
+    g = torch.Generator().manual_seed(L * 10 + layer)
+    deg = torch.tensor([0, 5, 1, 0, 12, 3, 0, 7, 0])
+    ctr = torch.repeat_interleave(torch.arange(N), deg)
+    E = int(ctr.numel())
+    csr = D.build_csr(torch.stack([ctr, torch.randint(0, N, (E,), generator=g)]).to(DEV), N)
+    dd = dict(dtype=torch.float64, generator=g)
+    yw = (torch.randn(E, Dd, **dd).to(DEV, acc), torch.randn(E, (lmax + 1) * U, **dd).to(DEV, dtype)) if implicit else (None, None)
+    Vin = None if implicit else torch.randn(E, d_in, U, **dd).to(DEV, dtype)
+    gam, gout = torch.randn(N, Dd, U, **dd).to(DEV, acc), torch.randn(E, d_out, U, **dd).to(DEV, dtype)
+
+    def run():
+        Vout = torch.empty(E, d_out, U, device=DEV, dtype=dtype)
+        gVin = None if implicit else torch.empty(E, d_in, U, device=DEV, dtype=dtype)
+        gw0 = torch.empty(E, (lmax + 1) * U, device=DEV, dtype=dtype) if implicit else None
+        gY = torch.zeros(E, Dd, device=DEV, dtype=acc) if implicit else None
+        ggam = torch.empty(N, Dd, U, device=DEV, dtype=acc)
+        _lib.tp_fwd(dtype, lmax, N, E, U, d_in, d_out, tab, cgw, csr.row_ptr, csr.ctr, gam, Vin, *yw, Vout)
+        _lib.tp_bwd(dtype, lmax, N, E, U, d_in, d_out, tab, cgw, csr.row_ptr, csr.ctr, gam, Vin, *yw, gout, gVin, gw0, gY, ggam)
+        torch.cuda.synchronize()
+        return bool(torch.isfinite(Vout).all())
+
+    _set(DEFAULTS)
+    finite, names = _kernels_launched(run)
+    assert finite
+    return d_in, d_out, Dd, implicit, int(tab.shape[0]), names
+
+
+_LMAX4_FRESH_PROCESS = r"""
+import json, sys
+sys.path[:0] = [{root!r}, {tests!r}]
+import test_gpu_tp_ragged as T
+out = {{}}
+for table in T.LMAX4_TABLES:
+    for dname, dtype in T.LMAX4_DTYPES.items():
+        out[table + "-" + dname] = T._lmax4_trace(table, dtype)
+print("TRACES " + json.dumps(out))
+"""
+
+
+@pytest.fixture(scope="module")
+def lmax4_traces():
+    """The traces of every l_max 4 table and dtype, taken in a fresh process: in one long pytest process, traces taken after
+    many earlier profiler sessions have lacked kernel records (the forward kernel's, while the values were right), so these
+    tables are traced where no earlier session runs and add no sessions to the process of the other trace checks."""
+    import json
+    import subprocess
+    import sys
+
+    here = os.path.dirname(os.path.abspath(__file__))
+    code = _LMAX4_FRESH_PROCESS.format(root=os.path.dirname(here), tests=here)
+    r = subprocess.run([sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code], capture_output=True, text=True,
+                       timeout=900)
+    line = [ln for ln in r.stdout.splitlines() if ln.startswith("TRACES ")]
+    assert r.returncode == 0 and line, r.stdout[-2000:] + r.stderr[-4000:]
+    return json.loads(line[-1][len("TRACES "):])
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("dtype", list(LMAX4_DTYPES))
+@pytest.mark.parametrize("table", list(LMAX4_TABLES))
+def test_lmax4_tables_run_the_generic_kernels(table, dtype, lmax4_traces):
+    """No fast family takes an l_max 4 table (25 -> 25, 25 -> 49, 49 -> 25, 25 -> 1): under the default options ab2_tp_fwd /
+    ab2_tp_bwd run tp_fwd_generic_kernel / tp_bwd_generic_kernel and no other tensor-product kernel.  A later fast kernel
+    for these tables changes this expectation and comes with its own test."""
+    d_in, d_out, Dd, implicit, nnz, names = lmax4_traces[f"{table}-{dtype}"]
+    if names is None:
+        pytest.skip("torch.profiler recorded no CUDA kernel events on this machine")
+    print(f"  l_max 4 {d_in} -> {d_out} ({nnz} entries) {dtype}: " + " ".join(_families(names)))
+    _check_kernels(names, *_expected_for(d_in, d_out, Dd, implicit, nnz, LMAX4_DTYPES[dtype], 32, DEFAULTS))
