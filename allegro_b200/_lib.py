@@ -230,6 +230,18 @@ def _contig(t: torch.Tensor, name: str):
     return t
 
 
+def _edge_index(idxs: torch.Tensor, device, rows: int) -> torch.Tensor:
+    """The scatter indices of the operator kernels: a contiguous 1-D int64 tensor on the operands' device with one entry
+    per edge row.  The kernels read them as int64_t, so another integer type would be misread."""
+    if idxs.dtype != torch.int64 or idxs.dim() != 1:
+        raise RuntimeError(f"allegro_b200: idxs must be a 1-D int64 tensor (got {idxs.dtype}, {idxs.dim()}-D)")
+    if idxs.device != device:
+        raise RuntimeError(f"allegro_b200: idxs is on {idxs.device}, the operands on {device}")
+    if idxs.shape[0] != rows:
+        raise RuntimeError(f"allegro_b200: idxs has {idxs.shape[0]} entries for {rows} edge rows")
+    return _contig(idxs, "idxs")
+
+
 def _row_strided(t: torch.Tensor, name: str):
     """2-D view with unit inner stride -> (tensor, leading dimension)."""
     if t.dim() != 2 or t.stride(1) != 1:
@@ -623,29 +635,36 @@ def transpose_ui(x: torch.Tensor, to_internal: bool) -> torch.Tensor:
 
 def op_scatter_env(x2: torch.Tensor, idxs: torch.Tensor, n: int, sf: float) -> torch.Tensor:
     E = x2.shape[0]
+    idxs = _edge_index(idxs, x2.device, E)
     row = x2[0].numel() if E else 0
     gamma = torch.zeros((n,) + tuple(x2.shape[1:]), dtype=x2.dtype, device=x2.device)
     with _timed("op_scatter_env"):
-        _check(load().ab2_op_scatter_env(DTYPE_ENUM[x2.dtype], E, row, float(sf), _ptr(_contig(x2, "x2")), _ptr(_contig(idxs, "idxs")), _ptr(gamma), _stream()))
+        _check(load().ab2_op_scatter_env(DTYPE_ENUM[x2.dtype], E, row, float(sf), _ptr(_contig(x2, "x2")), _ptr(idxs), _ptr(gamma), _stream()))
     return gamma
 
 
 def op_gather_rows(src: torch.Tensor, idxs: torch.Tensor, sf: float) -> torch.Tensor:
     E = idxs.shape[0]
+    idxs = _edge_index(idxs, src.device, E)
     row = src[0].numel()
     out = torch.empty((E,) + tuple(src.shape[1:]), dtype=src.dtype, device=src.device)
     with _timed("op_gather_rows"):
-        _check(load().ab2_op_gather_rows(DTYPE_ENUM[src.dtype], E, row, float(sf), _ptr(_contig(src, "src")), _ptr(_contig(idxs, "idxs")), _ptr(out), _stream()))
+        _check(load().ab2_op_gather_rows(DTYPE_ENUM[src.dtype], E, row, float(sf), _ptr(_contig(src, "src")), _ptr(idxs), _ptr(out), _stream()))
     return out
 
 
 def op_contract(mode: int, U, d1, d2, dout, tab, cgw, a, b, idxs, out):
-    E = idxs.shape[0]
+    """mode 0: out[E] from a = x1, b = gamma; mode 1: out[E] from a = gout, b = gamma; mode 2: out[N] += from a = x1, b = gout."""
+    E = a.shape[0]
+    idxs = _edge_index(idxs, a.device, E)
+    for t, name in ((b, "b"),) if mode == 2 else ((out, "out"),):
+        if t.shape[0] != E:
+            raise RuntimeError(f"allegro_b200: op_contract mode {mode}: {name} has {t.shape[0]} rows for {E} edges")
     with _timed("op_contract", 1):
         _check(
             load().ab2_op_contract(
                 DTYPE_ENUM[a.dtype], mode, E, U, d1, d2, dout, tab.shape[0], _ptr(tab), _ptr(cgw), _ptr(_contig(a, "a")), _ptr(_contig(b, "b")),
-                _ptr(_contig(idxs, "idxs")), _ptr(out), _stream(),
+                _ptr(idxs), _ptr(out), _stream(),
             )
         )
     return out
@@ -663,11 +682,14 @@ def zbl(p_cut: float, qq: float, vec, ctr, nbr, types, Z, rmax_table, gvec: Opti
 
 def op_contract_wgrad(U, d1, d2, dout, tab, x1, gamma, gout, idxs) -> torch.Tensor:
     """gcgw[nnz][U] = sum_z x1 (x) gamma[idxs] (x) gout over the coupling table (training)."""
-    E = idxs.shape[0]
+    E = x1.shape[0]
+    idxs = _edge_index(idxs, x1.device, E)
+    if gout.shape[0] != E:
+        raise RuntimeError(f"allegro_b200: op_contract_wgrad: gout has {gout.shape[0]} rows for {E} edges")
     out = torch.zeros(tab.shape[0], U, dtype=x1.dtype, device=x1.device)
     with _timed("op_contract_wgrad", 1):
         _check(load().ab2_op_contract_wgrad(DTYPE_ENUM[x1.dtype], E, U, d1, d2, dout, tab.shape[0], _ptr(tab), _ptr(_contig(x1, "x1")),
-                                            _ptr(_contig(gamma, "gamma")), _ptr(_contig(gout, "gout")), _ptr(_contig(idxs, "idxs")), _ptr(out), _stream()))
+                                            _ptr(_contig(gamma, "gamma")), _ptr(_contig(gout, "gout")), _ptr(idxs), _ptr(out), _stream()))
     return out
 
 

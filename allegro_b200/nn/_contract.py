@@ -251,35 +251,68 @@ class Contracter(torch.nn.Module):
 
     def _forward_impl(self, x1: torch.Tensor, x2: torch.Tensor, idxs: torch.Tensor, n: int) -> torch.Tensor:
         U, d1, d2, dout = self.mul, self.base_dim1, self.base_dim2, self.base_dim_out
+        idxs, checked = self._checked_indices(x1, x2, idxs, n)
         tab, cgw = self.device_tables(x1.dtype, x1.device)
         if torch.is_grad_enabled() and self.weights.requires_grad:
             cgw = self.cgw_live(x1.dtype, x1.device)
-        idxs = idxs.contiguous()
         sf = 1.0 if self.scatter_factor is None else float(self.scatter_factor)
         gamma = _ScatterRows.apply(x2.to(x1.dtype).reshape(-1, U, d2), idxs, n, sf)
-        csr, lmax = self._fast_route(idxs, n, d2)
+        csr, lmax = self._fast_route(checked, n, d2)
         return _Tri.apply("g", _Meta(U, d1, d2, dout, tab, idxs, n, csr, lmax), cgw, x1.reshape(-1, U, d1).contiguous(), gamma, None)
 
-    def _fast_route(self, idxs: torch.Tensor, n: int, d2: int):
+    def _checked_indices(self, x1: torch.Tensor, x2: torch.Tensor, idxs: torch.Tensor, n: int):
+        """(idxs as a contiguous int64 tensor, the cached check of this index tensor or None).
+
+        x1 and x2 must hold one row of mul * dim values per entry of the 1-D ``idxs``; other integer index types are
+        converted to int64, as torch's index ops accept them.  Every index must lie in [0, n): the kernels scatter into
+        and gather from n rows of the environment sum without a bounds test.  That check and the sortedness test of
+        ``_fast_route`` are one reduction with one host synchronisation, made once per index tensor (cached on the
+        tensor object, its version and n).  While a CUDA graph is being captured no synchronisation is possible: an
+        index tensor not checked before the capture is then used unchecked, and takes the generic route."""
+        if idxs.dim() != 1:
+            raise ValueError(f"Contracter: idxs must be 1-D (got shape {tuple(idxs.shape)})")
+        if idxs.dtype == torch.bool or idxs.is_floating_point() or idxs.is_complex():
+            raise TypeError(f"Contracter: idxs must be an integer tensor (got {idxs.dtype})")
+        E = idxs.shape[0]
+        for x, dim, name in ((x1, self.base_dim1, "x1"), (x2, self.base_dim2, "x2")):
+            if x.dim() < 1 or x.shape[0] != E or math.prod(x.shape[1:]) != self.mul * dim:
+                raise ValueError(f"Contracter: {name} of shape {tuple(x.shape)} does not match {E} edges of {self.mul} x {dim}")
+            if x.device != idxs.device:
+                raise ValueError(f"Contracter: {name} is on {x.device}, idxs on {idxs.device}")
+        hit = self._tab_cache.get("route")
+        if hit is not None and hit[0] is idxs and hit[1] == idxs._version and hit[2] == n:
+            return hit[4], hit
+        prepared = idxs.to(torch.int64).contiguous()
+        if idxs.is_cuda and torch.cuda.is_current_stream_capturing():
+            return prepared, None
+        is_sorted = False
+        if E:
+            lo, hi, is_sorted = torch.stack([prepared.min(), prepared.max(), (prepared[1:] >= prepared[:-1]).all().long()]).tolist()
+            if lo < 0 or hi >= n:
+                raise ValueError(f"Contracter: scatter index out of range: indices span [{lo}, {hi}], scatter_dim_size is {n}")
+        # (index tensor, version, n, CSR of the fast route: built on first use, prepared int64 indices, sorted by centre)
+        hit = (idxs, idxs._version, n, None, prepared, bool(is_sorted))
+        self._tab_cache["route"] = hit
+        return prepared, hit
+
+    def _fast_route(self, checked, n: int, d2: int):
         """(EdgeCSR, l_max) when the call can use the fused pipeline's tensor-product kernels: scatter indices sorted by
-        centre (what a centre-sorted neighbour list gives; checked once per index tensor) and a second operand that is a full
-        spherical-harmonic basis (d2 = (l+1)^2).  ALLEGRO_B200_OP_FAST=0 keeps the generic operator kernels."""
+        centre (what a centre-sorted neighbour list gives; ``checked`` by ``_checked_indices``) and a second operand that is
+        a full spherical-harmonic basis (d2 = (l+1)^2).  ALLEGRO_B200_OP_FAST=0 keeps the generic operator kernels."""
         import os
 
         from ..data import build_csr
 
         lmax = int(round(d2 ** 0.5)) - 1
-        if os.environ.get("ALLEGRO_B200_OP_FAST", "1") != "1" or (lmax + 1) ** 2 != d2 or lmax > 4 or idxs.numel() == 0:
+        if os.environ.get("ALLEGRO_B200_OP_FAST", "1") != "1" or (lmax + 1) ** 2 != d2 or lmax > 4 or checked is None or not checked[5]:
             return None, -1
-        hit = self._tab_cache.get("route")
-        if hit is None or hit[0] is not idxs or hit[1] != idxs._version or hit[2] != n:
+        if checked[3] is None:
+            idxs = checked[4]
             if idxs.is_cuda and torch.cuda.is_current_stream_capturing():
-                return None, -1  # the sortedness test synchronises: not while a CUDA graph is being captured
-            is_sorted = bool((idxs[1:] >= idxs[:-1]).all())
-            csr = build_csr(torch.stack([idxs, idxs]), n) if is_sorted else None
-            hit = (idxs, idxs._version, n, csr)
-            self._tab_cache["route"] = hit
-        return hit[3], (lmax if hit[3] is not None else -1)
+                return None, -1  # building the CSR synchronises
+            checked = checked[:3] + (build_csr(torch.stack([idxs, idxs]), n),) + checked[4:]
+            self._tab_cache["route"] = checked
+        return checked[3], lmax
 
     def extra_repr(self):
         return f"{self.irreps_in1} x {self.irreps_in2} -> {self.irreps_out} | {self.mul} channels | {self.num_paths} paths"

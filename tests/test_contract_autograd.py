@@ -62,3 +62,78 @@ def test_operator_first_and_second_order_on_cpu(spec_kernels, coupling, sorted_i
             assert err < 1e-10, (name, err)
     finally:
         torch.set_default_dtype(prev)
+
+
+def _small_operator(sorted_idx=True):
+    from allegro_b200.nn import B200Contracter
+
+    torch.manual_seed(7)
+    irr = "0e + 1o + 2e"
+    c = B200Contracter(irr, irr, irr, mul=3, scatter_factor=0.3).double()
+    E, N = 11, 4
+    idx = torch.randint(0, N, (E,))
+    if sorted_idx:
+        idx = torch.sort(idx).values
+    return c, torch.randn(E, 3, 9, dtype=torch.float64), torch.randn(E, 3, 9, dtype=torch.float64), idx, N
+
+
+@pytest.mark.parametrize("sorted_idx", [False, True], ids=["generic", "sorted"])
+def test_operator_refuses_bad_indices_before_any_kernel(spec_kernels, sorted_idx):
+    """Scatter indices outside [0, scatter_dim_size), negative ones and edge counts that differ between x1, x2 and idxs
+    are refused by the Contracter before a kernel sees them; another integer index type gives the int64 result."""
+    c, x1, x2, idx, N = _small_operator(sorted_idx)
+    ref = c._forward_impl(x1, x2, idx, N)
+    with pytest.raises(ValueError, match="out of range"):
+        c._forward_impl(x1, x2, torch.where(idx == idx.max(), N, idx), N)
+    with pytest.raises(ValueError, match="out of range"):
+        c._forward_impl(x1, x2, idx, int(idx.max()))  # scatter_dim_size too small for the same indices
+    neg = idx.clone()
+    neg[3] = -1
+    with pytest.raises(ValueError, match="out of range"):
+        c._forward_impl(x1, x2, neg, N)
+    for a, b, i in ((x1[:-1], x2, idx), (x1, x2[:-1], idx), (x1, x2, idx[:-1]), (x1[:, :2], x2, idx)):
+        with pytest.raises(ValueError, match="does not match"):
+            c._forward_impl(a, b, i, N)
+    with pytest.raises(TypeError):
+        c._forward_impl(x1, x2, idx.double(), N)
+    for dt in (torch.int32, torch.int16):
+        assert torch.equal(c._forward_impl(x1, x2, idx.to(dt), N), ref)
+
+
+@pytest.fixture()
+def no_library(monkeypatch):
+    """Any call into liballegro_b200 fails the test: a refusal must come before the kernel launch."""
+    from allegro_b200 import _lib
+
+    def reached(*a, **k):
+        raise AssertionError("the library was reached with arguments that must be refused")
+
+    monkeypatch.setattr(_lib, "load", reached)
+    return _lib
+
+
+def test_operator_wrappers_refuse_bad_index_tensors(no_library):
+    """The ctypes wrappers of the operator kernels pass idxs to an int64_t* parameter: an index tensor of another type,
+    of another length than the operands' rows, or not 1-D is refused before the library is reached."""
+    _lib = no_library
+    E, N, U, d = 6, 3, 2, 4
+    x = torch.zeros(E, U, d)
+    tab = torch.zeros(1, 3, dtype=torch.int32)
+    cgw = torch.zeros(1, U)
+    good = torch.zeros(E, dtype=torch.int64)
+    bad = [good.int(), good[:-1], good.view(2, 3), torch.zeros(2 * E, dtype=torch.int64)[::2]]
+    for idxs in bad:
+        with pytest.raises(RuntimeError, match="idxs"):
+            _lib.op_scatter_env(x, idxs, N, 1.0)
+        with pytest.raises(RuntimeError, match="idxs"):
+            _lib.op_contract(0, U, d, d, d, tab, cgw, x, torch.zeros(N, U, d), idxs, torch.zeros(E, U, d))
+        with pytest.raises(RuntimeError, match="idxs"):
+            _lib.op_contract_wgrad(U, d, d, d, tab, x, torch.zeros(N, U, d), x, idxs)
+    with pytest.raises(RuntimeError, match="idxs"):
+        _lib.op_gather_rows(torch.zeros(N, U, d), good.int(), 1.0)
+    with pytest.raises(RuntimeError, match="rows"):
+        _lib.op_contract(2, U, d, d, d, tab, cgw, x, x[:-1], good, torch.zeros(N, U, d))
+    with pytest.raises(RuntimeError, match="rows"):
+        _lib.op_contract(1, U, d, d, d, tab, cgw, x, torch.zeros(N, U, d), good, torch.zeros(E - 1, U, d))
+    with pytest.raises(RuntimeError, match="rows"):
+        _lib.op_contract_wgrad(U, d, d, d, tab, x, torch.zeros(N, U, d), x[:-1], good)
