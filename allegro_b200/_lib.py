@@ -101,6 +101,11 @@ _SIGNATURES = {
     "ab2_frame_heat_current": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_frame_extrema": ([_i32, _i64, _i64, _vp, _vp, _vp, _i64, _vp, _vp], C.c_int),
     "ab2_committee_moments": ([_i32, _i32, _i64, _i32, C.POINTER(C.c_void_p), _vp, _vp, _vp], C.c_int),
+    "ab2_fc_centres_count": ([_i64, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_fc_centres_fill": ([_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_fc_columns": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_fc_gather": ([_i32, _i32, _i64, _i64, _i64, _dbl] + [_vp] * 17, C.c_int),
+    "ab2_fc_fold": ([_i32, _i64, _i64, _dbl] + [_vp] * 14, C.c_int),
     "ab2_slots_check": ([_i32, _i64, _i64, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_slots_count": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp], C.c_int),
     "ab2_slots_place": ([_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
@@ -1015,6 +1020,86 @@ def committee_moments(xs: Sequence[torch.Tensor], G: int) -> Tuple[torch.Tensor,
     with _timed("committee_moments"):
         _check(load().ab2_committee_moments(DTYPE_ENUM[x0.dtype], len(xs), m, G, ptrs, _ptr(mean), _ptr(dev), _stream()))
     return mean, dev
+
+
+# --------------------------------------------------------------------------- #
+# Force constants from local displacement clusters (ab2_fc_*, phonons.force_constants).  ``atoms`` [A] int64 on the
+# device; the list is centre-sorted with a row per atom, its transpose from ``csr.transposed(n)``.
+# --------------------------------------------------------------------------- #
+FC_MAX_ATOMS = 1 << 20  # AB2_FC_MAX_ATOMS
+
+
+def _prefix(counts: torch.Tensor) -> torch.Tensor:
+    out = torch.zeros(counts.shape[0] + 1, dtype=torch.int64, device=counts.device)
+    torch.cumsum(counts, 0, out=out[1:])
+    return out
+
+
+def fc_centres(atoms: torch.Tensor, csr, n: int):
+    """C_j of every displaced atom -> (cptr [A+1] int64, cen [M] int32 ascending per atom, coff [M] int32 edge offset of
+    each centre's row inside its atom's cluster, ea [A] int64 edges of each cluster)  (ab2_fc_centres_count / fill)."""
+    A = atoms.shape[0]
+    dev = atoms.device
+    col_ptr, col_perm = csr.transposed(n)
+    counts = torch.empty(A, dtype=torch.int64, device=dev)
+    lib = load()
+    with _timed("fc_centres_count"):
+        _check(lib.ab2_fc_centres_count(A, _ptr(_contig(atoms, "atoms")), _ptr(col_ptr), _ptr(col_perm), _ptr(csr.ctr), _ptr(counts), _stream()))
+    cptr = _prefix(counts)
+    M = int(cptr[-1])
+    cen = torch.empty(M, dtype=torch.int32, device=dev)
+    coff = torch.empty(M, dtype=torch.int32, device=dev)
+    ea = torch.empty(A, dtype=torch.int64, device=dev)
+    with _timed("fc_centres_fill"):
+        _check(lib.ab2_fc_centres_fill(A, _ptr(atoms), _ptr(col_ptr), _ptr(col_perm), _ptr(csr.ctr), _ptr(csr.row_ptr), _ptr(cptr), _ptr(cen),
+                                       _ptr(coff), _ptr(ea), _stream()))
+    return cptr, cen, coff, ea
+
+
+def fc_columns(cptr: torch.Tensor, cen: torch.Tensor, csr, n: int):
+    """Columns of every displaced atom -> (fptr [A+1] int64, col [nnzb] int32 ascending per atom)  (ab2_fc_columns)."""
+    A = cptr.shape[0] - 1
+    dev = cptr.device
+    counts = torch.empty(A, dtype=torch.int64, device=dev)
+    lib = load()
+    with _timed("fc_columns_count"):
+        _check(lib.ab2_fc_columns(0, A, int(n), _ptr(cptr), _ptr(cen), _ptr(csr.row_ptr), _ptr(csr.nbr), None, _ptr(counts), None, _stream()))
+    fptr = _prefix(counts)
+    col = torch.empty(int(fptr[-1]), dtype=torch.int32, device=dev)
+    with _timed("fc_columns_fill"):
+        _check(lib.ab2_fc_columns(1, A, int(n), _ptr(cptr), _ptr(cen), _ptr(csr.row_ptr), _ptr(csr.nbr), _ptr(fptr), None, _ptr(col), _stream()))
+    return fptr, col
+
+
+def fc_gather(pos: torch.Tensor, shift: Optional[torch.Tensor], h: float, acc_dtype, atoms, cptr, cen, coff, ea, csr, Cp, Ep,
+              u0: int, u1: int, Cb: int, Eb: int):
+    """The jobs of units [u0, u1) as one batched CSR -> (row_ptr_b [Cb+1], cen_b [Cb], ctr_b [Eb], nbr_b [Eb] int32,
+    vec_b [Eb,3] acc dtype)  (ab2_fc_gather; Cb, Eb the chunk's totals from Cp, Ep)."""
+    dev = pos.device
+    row_ptr_b = torch.empty(Cb + 1, dtype=torch.int32, device=dev)
+    cen_b = torch.empty(Cb, dtype=torch.int32, device=dev)
+    ctr_b = torch.empty(Eb, dtype=torch.int32, device=dev)
+    nbr_b = torch.empty(Eb, dtype=torch.int32, device=dev)
+    vec_b = torch.empty(Eb, 3, dtype=acc_dtype, device=dev)
+    if shift is not None:
+        assert shift.dtype == pos.dtype
+    with _timed("fc_gather"):
+        _check(load().ab2_fc_gather(DTYPE_ENUM[pos.dtype], DTYPE_ENUM[acc_dtype], int(u0), int(u1 - u0), int(Cb), float(h), _ptr(_contig(pos, "pos")),
+                                    _ptr(_contig(shift, "shift")) if shift is not None else None, _ptr(atoms), _ptr(cptr), _ptr(cen), _ptr(coff),
+                                    _ptr(ea), _ptr(csr.row_ptr), _ptr(csr.nbr), _ptr(Cp), _ptr(Ep), _ptr(row_ptr_b), _ptr(cen_b), _ptr(ctr_b),
+                                    _ptr(nbr_b), _ptr(vec_b), _stream()))
+    return row_ptr_b, cen_b, ctr_b, nbr_b, vec_b
+
+
+def fc_fold(gvec: torch.Tensor, h: float, cptr, cen, coff, ea, csr, n: int, fptr, col, Ep, u0: int, u1: int, blocks: torch.Tensor):
+    """Rows alpha of the blocks of units [u0, u1) into ``blocks`` [nnzb,3,3] fp64 from the chunk's per-edge gradients
+    (ab2_fc_fold)."""
+    col_ptr, col_perm = csr.transposed(n)
+    assert blocks.dtype == torch.float64
+    with _timed("fc_fold"):
+        _check(load().ab2_fc_fold(DTYPE_ENUM[gvec.dtype], int(u0), int(u1 - u0), float(h), _ptr(cptr), _ptr(cen), _ptr(coff), _ptr(ea),
+                                  _ptr(csr.row_ptr), _ptr(csr.ctr), _ptr(col_ptr), _ptr(col_perm), _ptr(fptr), _ptr(col), _ptr(Ep),
+                                  _ptr(_contig(gvec, "gvec")) if gvec.numel() else None, _ptr(_contig(blocks, "blocks")), _stream()))
 
 
 # --------------------------------------------------------------------------- #

@@ -461,6 +461,33 @@ class UpstreamPack:
             _lib.radial_bwd(dt, self.S_rc, self.p, vec, csr.ctr, csr.nbr, types_i32, self.rmax_table, self.bessel_w, self.Wb, self.cemb, self.nemb, g_e0, gvec)
 
 
+def edge_energy_grad(core: "AllegroCore", up: UpstreamPack, csr: EdgeCSR, vec: torch.Tensor, types_i32: torch.Tensor,
+                     gEi_scale: Optional[torch.Tensor], pair=None):
+    """The per-edge part of ``energy_forces``: edge vectors ``vec`` [E,3] (acc dtype, CSR order, E > 0) -> (Ei [n_centres],
+    X, Ez, gvec [E,3] = d E_total / d vec (acc dtype), Ei_pair or None).  ``types_i32`` is indexed by both ``csr.ctr`` and
+    ``csr.nbr``; ``gEi_scale`` and ``pair`` as in ``energy_forces``.  Positions never enter: the caller may hand in edge
+    vectors of any geometry (phonons.force_constants passes displaced copies of the rows of a cluster)."""
+    dt = core.dtype
+    E = csr.num_edges
+    if up.fold:
+        box = []
+        Ei, X, Ez, sv = core.forward(csr, vec, None, fill_embed=lambda w0, x0, om0: box.append(up.forward(vec, csr, types_i32, [w0, x0, om0])))
+        up_saved = box[0]
+    else:
+        x_emb = torch.empty(E, core.S_in, dtype=dt, device=vec.device)
+        up_saved = up.forward(vec, csr, types_i32, [x_emb])
+        Ei, X, Ez, sv = core.forward(csr, vec, x_emb)
+    gEi = gEi_scale if gEi_scale is not None else torch.ones_like(Ei)
+    gvec, gx_emb = core.backward(sv, gEi)
+    _lib.set_tag("bwd.radial")
+    up.backward(up_saved, gx_emb if up.fold else [gx_emb], vec, csr, types_i32, gvec)
+    Ei_pair = None
+    if pair is not None:
+        Ez_pair = pair[0].edge_energy_and_grad(vec, csr, types_i32, pair[1], gvec)
+        Ei_pair = _lib.edge_sum(Ez_pair, csr.row_ptr, 1.0)
+    return Ei, X, Ez, gvec, Ei_pair
+
+
 def energy_forces(core: "AllegroCore", up: UpstreamPack, csr: EdgeCSR, pos: torch.Tensor, types_i32: torch.Tensor,
                   shift_vec: Optional[torch.Tensor], gEi_scale: Optional[torch.Tensor], want_virial: bool = False, pair=None,
                   frame_ptr: Optional[torch.Tensor] = None, want_atomic_virial: bool = False):
@@ -487,22 +514,7 @@ def energy_forces(core: "AllegroCore", up: UpstreamPack, csr: EdgeCSR, pos: torc
                 torch.zeros(pos.shape[0], 3, 3, dtype=acc, device=dev) if want_atomic_virial else None)
     _lib.set_tag("fwd.radial")
     vec = _lib.edge_vec(pos, csr.ctr, csr.nbr, shift_vec, acc)
-    if up.fold:
-        box = []
-        Ei, X, Ez, sv = core.forward(csr, vec, None, fill_embed=lambda w0, x0, om0: box.append(up.forward(vec, csr, types_i32, [w0, x0, om0])))
-        up_saved = box[0]
-    else:
-        x_emb = torch.empty(E, core.S_in, dtype=dt, device=pos.device)
-        up_saved = up.forward(vec, csr, types_i32, [x_emb])
-        Ei, X, Ez, sv = core.forward(csr, vec, x_emb)
-    gEi = gEi_scale if gEi_scale is not None else torch.ones_like(Ei)
-    gvec, gx_emb = core.backward(sv, gEi)
-    _lib.set_tag("bwd.radial")
-    up.backward(up_saved, gx_emb if up.fold else [gx_emb], vec, csr, types_i32, gvec)
-    Ei_pair = None
-    if pair is not None:
-        Ez_pair = pair[0].edge_energy_and_grad(vec, csr, types_i32, pair[1], gvec)
-        Ei_pair = _lib.edge_sum(Ez_pair, csr.row_ptr, 1.0)
+    Ei, X, Ez, gvec, Ei_pair = edge_energy_grad(core, up, csr, vec, types_i32, gEi_scale, pair)
     virial = None
     if want_virial:
         virial = (vec.T @ gvec.to(vec.dtype)) if frame_ptr is None else _lib.frame_virial(vec, gvec.to(vec.dtype), frame_ptr, csr.row_ptr)

@@ -1,0 +1,174 @@
+"""Harmonic force constants by finite displacements, as phonopy forms them, from local displacement clusters.
+
+    fc = force_constants(model, pos, cell, atom_types, pbc=True, atoms=None, displacement=0.01, max_edges=None)
+    fc.blocks[k][alpha][beta] = -(F+_{col[k],beta} - F-_{col[k],beta}) / (2h)  ~  d2E / dr_{atoms[a],alpha} dr_{col[k],beta}
+
+Displacing atom j by +-h along alpha moves only the edges of the rows in C_j = {j} u {k : an edge of row k has neighbour
+j}, each by s h e_alpha ([nbr = j] - [ctr = j]) (an edge from j to its own image does not move), and Allegro's energy is
+a sum of per-centre terms that see only their own row.  So F(r + h e) - F(r - h e) is exactly the difference of the forces
+of those rows alone: each displacement costs |C_j| rows instead of the whole frame (DESIGN.md section 4.9).  The list is
+built at r_max + h, so every pair that comes within r_max under a displacement is in it, and the edges beyond r_max add
+exact zeros.
+
+The plan (C_j, the non-zero columns of each row, the batched jobs) and the fold of per-edge gradients into blocks are the
+ab2_fc_* kernels (csrc/fc.cu); each chunk of jobs runs through the same per-edge pipeline as ``energy_and_forces``
+(nn._pipeline.edge_energy_grad).  A displaced atom's blocks do not depend on the chunking or on the other displaced atoms:
+bitwise for fp32 models, to rounding for fp64 models (their tensor-product adjoint adds with atomics).
+"""
+from __future__ import annotations
+
+import math
+from typing import Optional
+
+import torch
+
+from . import _lib
+from . import data as D
+
+# the kernels index edges with int32 (AB2 lists): one chunk holds at most this many edges
+MAX_CHUNK_EDGES = (1 << 31) - 2
+
+
+class ForceConstants:
+    """Block-sparse force constants: row a (displaced atom ``atoms[a]``) holds the blocks ``blocks[row_ptr[a]:row_ptr[a+1]]``
+    of the atoms ``col[row_ptr[a]:row_ptr[a+1]]`` (ascending).  Blocks are fp64 in the model's energy unit per length^2;
+    the first index is the displaced atom (phonopy's convention)."""
+
+    def __init__(self, atoms: torch.Tensor, row_ptr: torch.Tensor, col: torch.Tensor, blocks: torch.Tensor, num_atoms: int):
+        self.atoms, self.row_ptr, self.col, self.blocks = atoms, row_ptr, col, blocks
+        self.num_atoms = int(num_atoms)
+
+    def dense(self) -> torch.Tensor:
+        """[A,N,3,3] fp64: phonopy's force-constant array (its compact form when ``atoms`` lists the primitive atoms)."""
+        A = self.atoms.shape[0]
+        out = torch.zeros(A, self.num_atoms, 3, 3, dtype=torch.float64, device=self.blocks.device)
+        rows = torch.repeat_interleave(torch.arange(A, device=self.blocks.device), self.row_ptr[1:] - self.row_ptr[:-1])
+        out[rows, self.col] = self.blocks
+        return out
+
+
+def _fused(model):
+    from .committee import Committee
+    from .model.allegro_models import FusedAllegroEnergy
+
+    inner = getattr(model, "model", model)
+    if isinstance(inner, Committee) or not isinstance(inner, FusedAllegroEnergy):
+        raise TypeError(f"force_constants takes an AllegroModel or a FusedAllegroEnergy, got {type(model).__name__}")
+    return inner
+
+
+def _pbc3(pbc):
+    return tuple(bool(p) for p in (pbc if not isinstance(pbc, bool) else (pbc,) * 3))
+
+
+def _atoms(atoms, n: int) -> torch.Tensor:
+    """-> the displaced atoms as a CPU int64 tensor, checked."""
+    if atoms is None:
+        return torch.arange(n, dtype=torch.int64)
+    a = torch.as_tensor(atoms).detach().cpu()
+    if a.dim() != 1 or a.dtype.is_floating_point or a.dtype.is_complex or a.dtype == torch.bool:
+        raise ValueError(f"atoms must be a 1-D integer tensor, got {a.dtype} of shape {tuple(a.shape)}")
+    a = a.to(torch.int64)
+    if a.numel() and (int(a.min()) < 0 or int(a.max()) >= n):
+        raise ValueError(f"atoms must lie in [0, {n})")
+    if torch.unique(a).numel() != a.numel():
+        raise ValueError("atoms must not repeat")
+    return a
+
+
+def edge_bytes(core) -> int:
+    """Device bytes the per-edge pipeline allocates per edge of a chunk, counted from the model's widths (activations,
+    their gradients, the batched list and edge vectors), with 50 % headroom for the per-centre tensors and the allocator."""
+    es = torch.empty(0, dtype=core.dtype).element_size()
+    ac = torch.empty(0, dtype=core.acc).element_size()
+    hid = max([core.readout.dims[1]] + [ly["mlp"].dims[1] for ly in core.layers] + [core.S])
+    tp = sum(ly["d_out"] * core.U for ly in core.layers)
+    act = 2 * core.S * (core.L + 1) + 3 * core.nw * (core.L + 1) + 2 * tp + 4 * hid * (core.L + 2) + core.S_in
+    return int(1.5 * (es * act + ac * (2 * core.D + 9) + 12))
+
+
+def _default_max_edges(core, device) -> int:
+    free, _ = torch.cuda.mem_get_info(device)
+    return int(max(1, min(MAX_CHUNK_EDGES, free // 2 // edge_bytes(core))))
+
+
+def force_constants(model, pos: torch.Tensor, cell: Optional[torch.Tensor], atom_types: torch.Tensor, pbc=True, atoms=None,
+                    displacement: float = 0.01, max_edges: Optional[int] = None) -> ForceConstants:
+    """Force constants of the displaced ``atoms`` (default: every atom) by central differences with step ``displacement``,
+    equal to the full-frame finite difference up to rounding.  ``model``: an ``AllegroModel`` or ``FusedAllegroEnergy`` on a
+    CUDA device (TypeError otherwise, a committee included).  ``pos`` [N,3] fp32 / fp64 and ``atom_types`` [N] on the
+    device; ``cell`` [3,3] (needed, and regular, on every periodic axis) or None.  Displacements run in chunks of at most
+    ``max_edges`` batched edges (default: half the free device memory over ``edge_bytes``)."""
+    inner = _fused(model)
+    if not torch.is_tensor(pos) or not pos.is_cuda or not torch.is_tensor(atom_types) or not atom_types.is_cuda:
+        raise RuntimeError("allegro_b200: inputs must be CUDA tensors (no CPU fallback on the hot path)")
+    h = float(displacement)
+    if not math.isfinite(h) or h <= 0.0:
+        raise ValueError(f"displacement must be finite and > 0, got {displacement!r}")
+    if pos.dim() != 2 or pos.shape[1] != 3 or pos.dtype not in (torch.float32, torch.float64):
+        raise ValueError(f"pos must be fp32 or fp64 [N,3], got {pos.dtype} of shape {tuple(pos.shape)}")
+    n = pos.shape[0]
+    if atom_types.dim() != 1 or atom_types.shape[0] != n or atom_types.dtype.is_floating_point or atom_types.dtype == torch.bool:
+        raise ValueError(f"atom_types must be [N] = [{n}] integers, got {atom_types.dtype} of shape {tuple(atom_types.shape)}")
+    if n < 1 or n > _lib.FC_MAX_ATOMS:
+        raise ValueError(f"force_constants takes frames of 1 .. {_lib.FC_MAX_ATOMS} atoms, got {n}")
+    pbc = _pbc3(pbc)
+    if any(pbc) and (cell is None or not D.is_regular_cell(cell)):
+        raise ValueError("a periodic axis needs a regular cell (data.is_regular_cell)")
+    atoms_h = _atoms(atoms, n)
+    if max_edges is not None and not (1 <= int(max_edges) <= MAX_CHUNK_EDGES):
+        raise ValueError(f"max_edges must lie in [1, {MAX_CHUNK_EDGES}], got {max_edges!r}")
+    core = inner.core()
+    dev = pos.device
+    pos = pos.detach().contiguous()
+    types_i32 = atom_types.to(torch.int32).contiguous()
+    if cell is not None:
+        cell = cell.detach().reshape(3, 3).to(device=dev, dtype=pos.dtype)
+    from .calculator import prune_table
+
+    cutoffs = prune_table(inner, h)
+    prune = {} if cutoffs is None else dict(types=types_i32, cutoffs=cutoffs)
+    csr, shift = D.neighbor_csr(pos, inner.r_max + h, cell, pbc, **prune)
+    A = atoms_h.shape[0]
+    atoms_d = atoms_h.to(dev)
+    # the plan: C_j and its edge offsets, then the non-zero columns of every row
+    cptr, cen, coff, ea = _lib.fc_centres(atoms_d, csr, n)
+    fptr, col = _lib.fc_columns(cptr, cen, csr, n)
+    blocks = torch.empty(col.shape[0], 3, 3, dtype=torch.float64, device=dev)
+    # units u = 3 a + alpha, each two jobs (+h, -h) of m_a centres and E_a edges
+    Cp = _lib._prefix((cptr[1:] - cptr[:-1]).repeat_interleave(3))
+    Ep = _lib._prefix(ea.repeat_interleave(3))
+    Cp_h, Ep_h = Cp.cpu(), Ep.cpu()
+    cap = int(max_edges) if max_edges is not None else _default_max_edges(core, dev)
+    unit_edges = 2 * (Ep_h[1:] - Ep_h[:-1])
+    if unit_edges.numel() and int(unit_edges.max()) > cap:
+        raise ValueError(f"max_edges = {cap} is below the {int(unit_edges.max())} edges of one displacement pair")
+    hp = float(torch.tensor(h, dtype=pos.dtype))  # the step as the positions hold it
+    ss = inner.per_type_energy_scale_shift
+    gscale = ss.scales[atom_types.long()].to(core.acc)
+    pair = None
+    if inner.pair_potential is not None:
+        pair = (inner.pair_potential, inner.edge_norm.rmax_table.to(device=dev, dtype=core.acc))
+    from .nn._pipeline import edge_energy_grad
+
+    U = 3 * A
+    u0 = 0
+    while u0 < U:
+        # the largest run of units whose jobs fit in cap edges
+        u1 = int(torch.searchsorted(Ep_h, Ep_h[u0] + cap // 2, right=True)) - 1
+        u1 = max(u0 + 1, min(u1, U))
+        while u1 > u0 + 1 and int(2 * (Cp_h[u1] - Cp_h[u0])) + n > MAX_CHUNK_EDGES:  # batched centres and atoms index int32 too
+            u1 = u0 + (u1 - u0) // 2
+        Cb, Eb = int(2 * (Cp_h[u1] - Cp_h[u0])), int(2 * (Ep_h[u1] - Ep_h[u0]))
+        if Eb == 0:
+            # every cluster of the chunk is an isolated atom: zero gradients (energy_forces' E == 0 path)
+            gvec = torch.zeros(0, 3, dtype=core.acc, device=dev)
+        else:
+            row_ptr_b, cen_b, ctr_b, nbr_b, vec_b = _lib.fc_gather(pos, shift, hp, core.acc, atoms_d, cptr, cen, coff, ea, csr, Cp, Ep,
+                                                                   u0, u1, Cb, Eb)
+            csr_b = D.EdgeCSR(Cb, ctr_b, nbr_b, row_ptr_b, None, csr.max_degree)
+            types_b = torch.cat([types_i32[cen_b.long()], types_i32])
+            _, _, _, gvec, _ = edge_energy_grad(core, inner._upstream, csr_b, vec_b, types_b, gscale[cen_b.long()], pair)
+        _lib.fc_fold(gvec, hp, cptr, cen, coff, ea, csr, n, fptr, col, Ep, u0, u1, blocks)
+        u0 = u1
+    return ForceConstants(atoms_d, fptr, col.long(), blocks, n)

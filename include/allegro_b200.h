@@ -457,6 +457,47 @@ int ab2_frame_extrema(int acc_dtype, int64_t n, int64_t n_frames, const int32_t*
  * for m = 0. */
 int ab2_committee_moments(int dtype, int K, int64_t m, int G, const void* const* x, void* mean, void* dev, void* stream);
 
+/* ---- harmonic force constants from local displacement clusters (phonons.force_constants) ------------------------- */
+
+/* Largest frame of ab2_fc_columns: one CTA holds a bitmap of every atom in shared memory (128 KiB). */
+#define AB2_FC_MAX_ATOMS (1 << 20)
+
+/* Centres of each displaced atom j = atoms[a] (a in [0, A)) on a centre-sorted CSR with its transpose (col_ptr, col_perm
+ * of EdgeCSR.transposed):  C_j = {j} u {ctr[z] : nbr[z] = j}, ascending, without repeats.
+ *   count: counts[a] = |C_j| (int64).
+ *   fill:  cen[cptr[a] + c] = c-th centre k of C_j; coff[...] = sum of the row lengths of the centres before it (the row's
+ *          edge offset inside the atom's cluster); ea[a] = sum of the row lengths of all of C_j. */
+int ab2_fc_centres_count(int64_t A, const int64_t* atoms, const int32_t* col_ptr, const int32_t* col_perm, const int32_t* ctr,
+                         int64_t* counts, void* stream);
+int ab2_fc_centres_fill(int64_t A, const int64_t* atoms, const int32_t* col_ptr, const int32_t* col_perm, const int32_t* ctr,
+                        const int32_t* row_ptr, const int64_t* cptr, int32_t* cen, int32_t* coff, int64_t* ea, void* stream);
+/* Columns of each displaced atom: the ascending atoms that are a centre of C_j or a neighbour of an edge of a row of C_j.
+ * fill = 0: counts[a] (int64); fill = 1: col[fptr[a] ...].  n: atoms of the frame, 1 .. AB2_FC_MAX_ATOMS. */
+int ab2_fc_columns(int fill, int64_t A, int64_t n, const int64_t* cptr, const int32_t* cen, const int32_t* row_ptr, const int32_t* nbr,
+                   const int64_t* fptr, int64_t* counts, int32_t* col, void* stream);
+/* One chunk of displacement jobs as a batched CSR.  Units u in [u0, u0 + U) are (a = u / 3, alpha = u % 3); each gives
+ * two jobs, s = +1 then s = -1, of m_a = cptr[a+1] - cptr[a] centres and E_a = ea[a] edges.  Cp, Ep [3A+1] int64 are
+ * the exclusive prefix sums of m and E over units; Cb = 2 (Cp[u0+U] - Cp[u0]) batched centres.  Job sigma of unit u
+ * takes centres from q0 = 2 (Cp[u] - Cp[u0]) + sigma m_a and edges from 2 (Ep[u] - Ep[u0]) + sigma E_a.  For centre c
+ * (k = cen[cptr[a] + c]) and its row edge z = row_ptr[k] + e, the batched edge zb = row_ptr_b[q0 + c] + e holds
+ *   ctr_b[zb] = q0 + c,  nbr_b[zb] = Cb + nbr[z],  cen_b[q0 + c] = k,
+ *   vec_b[zb] = (acc) ((pos[nbr[z]] - pos[k] + shift[z]) + s h e_alpha ([nbr[z] = j] - [k = j]))
+ * in the positions' dtype (the operations of ab2_edge_vec, then one add of +-h on axis alpha), rounded once to the
+ * accumulate dtype; row_ptr_b [Cb+1] int32.  shift may be null. */
+int ab2_fc_gather(int pos_dtype, int acc_dtype, int64_t u0, int64_t U, int64_t Cb, double h, const void* pos, const void* shift,
+                  const int64_t* atoms, const int64_t* cptr, const int32_t* cen, const int32_t* coff, const int64_t* ea,
+                  const int32_t* row_ptr, const int32_t* nbr, const int64_t* Cp, const int64_t* Ep, int32_t* row_ptr_b,
+                  int32_t* cen_b, int32_t* ctr_b, int32_t* nbr_b, void* vec_b, void* stream);
+/* Force-constant rows of the units [u0, u0 + U) from the per-edge gradients gvec [Eb][3] (acc dtype) of the chunk
+ * ab2_fc_gather laid out:  blocks[p][alpha][beta] = -(F+_{i,beta} - F-_{i,beta}) * (1 / (2h)), i = col[p], p in
+ * [fptr[a], fptr[a+1]), fp64, where F_i = sum of gvec over the job's edges centred on i - sum over the job's edges with
+ * neighbour i (every image of i).  One warp per column: each lane sums (g+ - g-) in fp64 over the row of i (lane-strided)
+ * and then over column i of the transposed list (lane-strided, edges whose centre is in C_j), the warp reduces with a
+ * fixed butterfly; no atomics, so a row depends on its own jobs only. */
+int ab2_fc_fold(int acc_dtype, int64_t u0, int64_t U, double h, const int64_t* cptr, const int32_t* cen, const int32_t* coff,
+                const int64_t* ea, const int32_t* row_ptr, const int32_t* ctr, const int32_t* col_ptr, const int32_t* col_perm,
+                const int64_t* fptr, const int32_t* col, const int64_t* Ep, const void* gvec, double* blocks, void* stream);
+
 /* ---- Verlet lists of a batch of frames in fixed edge slots (molecular dynamics of many small frames) ---------------- */
 
 /* Largest frame of the slot kernels (and of data.FRAMES_MAX_ATOMS): ab2_slots_place covers a frame with one CTA. */
