@@ -106,6 +106,10 @@ _SIGNATURES = {
     "ab2_fc_columns": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_fc_gather": ([_i32, _i32, _i64, _i64, _i64, _dbl] + [_vp] * 17, C.c_int),
     "ab2_fc_fold": ([_i32, _i64, _i64, _dbl] + [_vp] * 14, C.c_int),
+    "ab2_fc3_pairs_count": ([_i64] + [_vp] * 6, C.c_int),
+    "ab2_fc3_pairs_fill": ([_i64] + [_vp] * 10, C.c_int),
+    "ab2_fc3_gather": ([_i32, _i32, _i64, _i64, _i64, _dbl] + [_vp] * 16, C.c_int),
+    "ab2_fc3_fold": ([_i32, _i64, _i64, _dbl] + [_vp] * 13, C.c_int),
     "ab2_slots_check": ([_i32, _i64, _i64, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_slots_count": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp], C.c_int),
     "ab2_slots_place": ([_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
@@ -1100,6 +1104,58 @@ def fc_fold(gvec: torch.Tensor, h: float, cptr, cen, coff, ea, csr, n: int, fptr
         _check(load().ab2_fc_fold(DTYPE_ENUM[gvec.dtype], int(u0), int(u1 - u0), float(h), _ptr(cptr), _ptr(cen), _ptr(coff), _ptr(ea),
                                   _ptr(csr.row_ptr), _ptr(csr.ctr), _ptr(col_ptr), _ptr(col_perm), _ptr(fptr), _ptr(col), _ptr(Ep),
                                   _ptr(_contig(gvec, "gvec")) if gvec.numel() else None, _ptr(_contig(blocks, "blocks")), _stream()))
+
+
+def fc3_pairs(pj: torch.Tensor, pk: torch.Tensor, Kptr: torch.Tensor, Ken: torch.Tensor, csr):
+    """C_j n C_k of every pair (pj, pk [P] int32 atom ids) from the centre sets of every atom (Kptr, Ken of
+    ``fc_centres(arange(n))``) -> (iptr [P+1] int64, icen [M] int32 ascending per pair, ioff [M] int32 edge offset of each
+    centre's row inside its pair's cluster, pe [P] int64 edges of each cluster)  (ab2_fc3_pairs_count / fill)."""
+    P = pj.shape[0]
+    dev = pj.device
+    counts = torch.empty(P, dtype=torch.int64, device=dev)
+    lib = load()
+    with _timed("fc3_pairs_count"):
+        _check(lib.ab2_fc3_pairs_count(P, _ptr(_contig(pj, "pj")), _ptr(_contig(pk, "pk")), _ptr(Kptr), _ptr(Ken), _ptr(counts), _stream()))
+    iptr = _prefix(counts)
+    M = int(iptr[-1])
+    icen = torch.empty(M, dtype=torch.int32, device=dev)
+    ioff = torch.empty(M, dtype=torch.int32, device=dev)
+    pe = torch.empty(P, dtype=torch.int64, device=dev)
+    with _timed("fc3_pairs_fill"):
+        _check(lib.ab2_fc3_pairs_fill(P, _ptr(pj), _ptr(pk), _ptr(Kptr), _ptr(Ken), _ptr(csr.row_ptr), _ptr(iptr), _ptr(icen), _ptr(ioff), _ptr(pe),
+                                      _stream()))
+    return iptr, icen, ioff, pe
+
+
+def fc3_gather(pos: torch.Tensor, shift: Optional[torch.Tensor], h: float, acc_dtype, pj, pk, iptr, icen, ioff, Pe, csr, u0: int, u1: int,
+               Cb: int, Eb: int):
+    """The four jobs of each unit of [u0, u1) as one batched CSR -> (row_ptr_b [Cb+1], cen_b [Cb], ctr_b [Eb], nbr_b [Eb]
+    int32, vec_b [Eb,3] acc dtype)  (ab2_fc3_gather; Pe [P+1] the prefix of the pairs' edge counts)."""
+    dev = pos.device
+    row_ptr_b = torch.empty(Cb + 1, dtype=torch.int32, device=dev)
+    cen_b = torch.empty(Cb, dtype=torch.int32, device=dev)
+    ctr_b = torch.empty(Eb, dtype=torch.int32, device=dev)
+    nbr_b = torch.empty(Eb, dtype=torch.int32, device=dev)
+    vec_b = torch.empty(Eb, 3, dtype=acc_dtype, device=dev)
+    if shift is not None:
+        assert shift.dtype == pos.dtype
+    with _timed("fc3_gather"):
+        _check(load().ab2_fc3_gather(DTYPE_ENUM[pos.dtype], DTYPE_ENUM[acc_dtype], int(u0), int(u1 - u0), int(Cb), float(h), _ptr(_contig(pos, "pos")),
+                                     _ptr(_contig(shift, "shift")) if shift is not None else None, _ptr(pj), _ptr(pk), _ptr(iptr), _ptr(icen),
+                                     _ptr(ioff), _ptr(Pe), _ptr(csr.row_ptr), _ptr(csr.nbr), _ptr(row_ptr_b), _ptr(cen_b), _ptr(ctr_b), _ptr(nbr_b),
+                                     _ptr(vec_b), _stream()))
+    return row_ptr_b, cen_b, ctr_b, nbr_b, vec_b
+
+
+def fc3_fold(gvec: torch.Tensor, h: float, iptr, icen, ioff, Pe, csr, n: int, rptr, col, u0: int, u1: int, blocks: torch.Tensor):
+    """Blocks [alpha][beta] of the units [u0, u1) into ``blocks`` [T,3,3,3] fp64 from the chunk's per-edge gradients
+    (ab2_fc3_fold)."""
+    col_ptr, col_perm = csr.transposed(n)
+    assert blocks.dtype == torch.float64
+    with _timed("fc3_fold"):
+        _check(load().ab2_fc3_fold(DTYPE_ENUM[gvec.dtype], int(u0), int(u1 - u0), float(h), _ptr(iptr), _ptr(icen), _ptr(ioff), _ptr(Pe),
+                                   _ptr(csr.row_ptr), _ptr(csr.ctr), _ptr(col_ptr), _ptr(col_perm), _ptr(rptr), _ptr(col),
+                                   _ptr(_contig(gvec, "gvec")) if gvec.numel() else None, _ptr(_contig(blocks, "blocks")), _stream()))
 
 
 # --------------------------------------------------------------------------- #

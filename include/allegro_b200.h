@@ -498,6 +498,42 @@ int ab2_fc_fold(int acc_dtype, int64_t u0, int64_t U, double h, const int64_t* c
                 const int64_t* ea, const int32_t* row_ptr, const int32_t* ctr, const int32_t* col_ptr, const int32_t* col_perm,
                 const int64_t* fptr, const int32_t* col, const int64_t* Ep, const void* gvec, double* blocks, void* stream);
 
+/* ---- third-order force constants from pair displacement clusters (phonons.third_order_force_constants) ------------ */
+
+/* Clusters of the pairs p in [0, P) of displaced atoms j = pj[p], k = pk[p] (int32 atom ids): C_j n C_k, from the
+ * centre sets of every atom (Kptr [n+1], Ken: ab2_fc_centres_* with atoms = 0 .. n-1), ascending.
+ *   count: counts[p] = |C_j n C_k| (int64).
+ *   fill:  icen[iptr[p] + c] = c-th centre of the intersection; ioff[...] = its row's edge offset inside the pair's
+ *          cluster (sum of the row lengths of the centres before it); pe[p] = the cluster's edge count. */
+int ab2_fc3_pairs_count(int64_t P, const int32_t* pj, const int32_t* pk, const int64_t* Kptr, const int32_t* Ken, int64_t* counts,
+                        void* stream);
+int ab2_fc3_pairs_fill(int64_t P, const int32_t* pj, const int32_t* pk, const int64_t* Kptr, const int32_t* Ken, const int32_t* row_ptr,
+                       const int64_t* iptr, int32_t* icen, int32_t* ioff, int64_t* pe, void* stream);
+/* One chunk of pair jobs as a batched CSR.  Units u in [u0, u0 + U) are (p = u / 9, alpha = u / 3 % 3, beta = u % 3);
+ * each gives four jobs sigma = 0..3 with (s1, s2) = (+,+), (+,-), (-,+), (-,-), of m_p = iptr[p+1] - iptr[p] centres and
+ * E_p = Pe[p+1] - Pe[p] edges (Pe [P+1] int64: exclusive prefix of pe).  With C(u) = 9 iptr[p] + (u % 9) m_p and
+ * E(u) = 9 Pe[p] + (u % 9) E_p, Cb = 4 (C(u0 + U) - C(u0)) batched centres; job sigma of unit u takes centres from
+ * q0 = 4 (C(u) - C(u0)) + sigma m_p and edges from 4 (E(u) - E(u0)) + sigma E_p.  For centre c (kc = icen[iptr[p] + c])
+ * and its row edge z = row_ptr[kc] + e, the batched edge zb = row_ptr_b[q0 + c] + e holds
+ *   ctr_b[zb] = q0 + c,  nbr_b[zb] = Cb + nbr[z],  cen_b[q0 + c] = kc,
+ *   vec_b[zb] = (acc) ((pos[nbr[z]] - pos[kc] + shift[z]) + delta),
+ *   delta = s1 h e_alpha ([nbr[z] = j] - [kc = j]) + s2 h e_beta ([nbr[z] = k] - [kc = k])
+ * in the positions' dtype; delta is exact and added once, so the pair (k, j) with (beta, alpha) forms the same vectors.
+ * row_ptr_b [Cb+1] int32.  shift may be null. */
+int ab2_fc3_gather(int pos_dtype, int acc_dtype, int64_t u0, int64_t U, int64_t Cb, double h, const void* pos, const void* shift,
+                   const int32_t* pj, const int32_t* pk, const int64_t* iptr, const int32_t* icen, const int32_t* ioff,
+                   const int64_t* Pe, const int32_t* row_ptr, const int32_t* nbr, int32_t* row_ptr_b, int32_t* cen_b,
+                   int32_t* ctr_b, int32_t* nbr_b, void* vec_b, void* stream);
+/* Third-order blocks of the units [u0, u0 + U) from the per-edge gradients gvec [Eb][3] (acc dtype) of the chunk
+ * ab2_fc3_gather laid out:  blocks[t][alpha][beta][gamma] = -((F++ + F--) - (F+- + F-+))_{i,gamma} * (1 / (4 h^2)),
+ * i = col[t], t in [rptr[p], rptr[p+1]) (ab2_fc_columns of the pair clusters), fp64.  F_i as in ab2_fc_fold over the
+ * edges of C_j n C_k.  One warp per column, lane-strided over the row of i and then column i of the transposed list, a
+ * fixed butterfly; no atomics, so a pair's blocks depend on its own jobs only.  gvec may be null when the chunk has no
+ * edges. */
+int ab2_fc3_fold(int acc_dtype, int64_t u0, int64_t U, double h, const int64_t* iptr, const int32_t* icen, const int32_t* ioff,
+                 const int64_t* Pe, const int32_t* row_ptr, const int32_t* ctr, const int32_t* col_ptr, const int32_t* col_perm,
+                 const int64_t* rptr, const int32_t* col, const void* gvec, double* blocks, void* stream);
+
 /* ---- Verlet lists of a batch of frames in fixed edge slots (molecular dynamics of many small frames) ---------------- */
 
 /* Largest frame of the slot kernels (and of data.FRAMES_MAX_ATOMS): ab2_slots_place covers a frame with one CTA. */
