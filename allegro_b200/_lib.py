@@ -110,6 +110,16 @@ _SIGNATURES = {
     "ab2_fc3_pairs_fill": ([_i64] + [_vp] * 10, C.c_int),
     "ab2_fc3_gather": ([_i32, _i32, _i64, _i64, _i64, _dbl] + [_vp] * 16, C.c_int),
     "ab2_fc3_fold": ([_i32, _i64, _i64, _dbl] + [_vp] * 13, C.c_int),
+    "ab2_sh_jvp": ([_i32, _i32, _i64, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_sh_hvp": ([_i32, _i32, _i64, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_act_bwd_jvp": ([_i32, _i64, _vp, _vp, _vp, _vp, _vp, _i32, _vp], C.c_int),
+    "ab2_radial_pq_jvp": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_radial_jvp": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_radial_pq_hvp": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp], C.c_int),
+    "ab2_radial_hvp": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_zbl_hvp": ([_i32, _i64, _i32, _dbl, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
+    "ab2_fc_gather_tangent": ([_i32, _i32, _i64, _i64, _i64] + [_vp] * 18, C.c_int),
+    "ab2_fc_fold_tangent": ([_i32, _i64, _i64] + [_vp] * 14, C.c_int),
     "ab2_slots_check": ([_i32, _i64, _i64, _vp, _vp, _vp, _dbl, _vp, _vp], C.c_int),
     "ab2_slots_count": ([_i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp], C.c_int),
     "ab2_slots_place": ([_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
@@ -730,6 +740,90 @@ def radial_bwd(dtype, S_rc: int, p_cut: float, vec, ctr, nbr, types, rmax_table,
                                      _ptr(_contig(g_e0, "g_e0")), _ptr(gvec), _stream()))
 
 
+# --------------------------------------------------------------------------- #
+# Tangents of the nonlinear steps of the per-edge path (ab2_*_jvp / ab2_*_hvp, nn._hessian)
+# --------------------------------------------------------------------------- #
+def sh_jvp(vec: torch.Tensor, vdot: torch.Tensor, lmax: int) -> torch.Tensor:
+    """Yd [E,(lmax+1)^2] = dY/dvec . vdot (ab2_sh_jvp)."""
+    E = vec.shape[0]
+    Yd = torch.empty(E, (lmax + 1) ** 2, dtype=vec.dtype, device=vec.device)
+    assert vdot.dtype == vec.dtype and vdot.shape == vec.shape
+    with _timed("sh_jvp"):
+        _check(load().ab2_sh_jvp(DTYPE_ENUM[vec.dtype], lmax, E, _ptr(_contig(vec, "vec")), _ptr(_contig(vdot, "vdot")), _ptr(Yd), _stream()))
+    return Yd
+
+
+def sh_hvp(vec: torch.Tensor, vdot: torch.Tensor, gY: torch.Tensor, lmax: int, gvec_dot: torch.Tensor):
+    """gvec_dot += (d2 sum_k gY_k Y_k / dvec2) . vdot (ab2_sh_hvp)."""
+    E = vec.shape[0]
+    assert vdot.dtype == vec.dtype == gY.dtype == gvec_dot.dtype
+    with _timed("sh_hvp"):
+        _check(load().ab2_sh_hvp(DTYPE_ENUM[vec.dtype], lmax, E, _ptr(_contig(vec, "vec")), _ptr(_contig(vdot, "vdot")), _ptr(_contig(gY, "gY")),
+                                 _ptr(_contig(gvec_dot, "gvec_dot")), _stream()))
+
+
+def act_bwd_jvp(ga_dot: Optional[torch.Tensor], ga: torch.Tensor, pre: torch.Tensor, pre_dot: torch.Tensor, nonlin: int = NL_SILU) -> torch.Tensor:
+    """ga_dot * phi'(pre) + ga * phi''(pre) * pre_dot (ab2_act_bwd_jvp; ga_dot None = 0), all of one shape and dtype."""
+    for t in (ga_dot, pre, pre_dot):
+        assert t is None or (t.shape == ga.shape and t.dtype == ga.dtype)
+    out = torch.empty_like(ga)
+    with _timed("act_bwd_jvp"):
+        _check(load().ab2_act_bwd_jvp(DTYPE_ENUM[ga.dtype], ga.numel(), _ptr(_contig(ga_dot, "ga_dot")) if ga_dot is not None else None,
+                                      _ptr(_contig(ga, "ga")), _ptr(_contig(pre, "pre")), _ptr(_contig(pre_dot, "pre_dot")), _ptr(out), int(nonlin),
+                                      _stream()))
+    return out
+
+
+def radial_pq_jvp(dtype, S: int, p_cut: float, vec, vdot, ctr, nbr, types, rmax_table, bessel_w, PQ) -> torch.Tensor:
+    """d radial_pq_fwd / dvec . vdot (ab2_radial_pq_jvp)."""
+    E = ctr.shape[0]
+    out = torch.empty(E, S, dtype=dtype, device=vec.device)
+    with _timed("radial_jvp"):
+        _check(load().ab2_radial_pq_jvp(DTYPE_ENUM[dtype], E, S, bessel_w.numel(), float(p_cut), _ptr(_contig(vec, "vec")), _ptr(_contig(vdot, "vdot")),
+                                        _ptr(ctr), _ptr(nbr), _ptr(types), _ptr(rmax_table), rmax_table.shape[0], _ptr(bessel_w),
+                                        _ptr(_contig(PQ, "PQ")), _ptr(out), _stream()))
+    return out
+
+
+def radial_jvp(dtype, S_rc: int, p_cut: float, vec, vdot, ctr, nbr, types, rmax_table, bessel_w, Wb, cemb, nemb) -> torch.Tensor:
+    """d radial_fwd / dvec . vdot (ab2_radial_jvp)."""
+    E = ctr.shape[0]
+    out = torch.empty(E, S_rc, dtype=dtype, device=vec.device)
+    with _timed("radial_jvp"):
+        _check(load().ab2_radial_jvp(DTYPE_ENUM[dtype], E, S_rc, bessel_w.numel(), float(p_cut), _ptr(_contig(vec, "vec")), _ptr(_contig(vdot, "vdot")),
+                                     _ptr(ctr), _ptr(nbr), _ptr(types), _ptr(rmax_table), rmax_table.shape[0], _ptr(bessel_w), _ptr(Wb), _ptr(cemb),
+                                     _ptr(nemb), _ptr(out), _stream()))
+    return out
+
+
+def radial_pq_hvp(dtype, S: int, p_cut: float, vec, vdot, ctr, nbr, types, rmax_table, bessel_w, PQ, g_out, aux, gvec_dot, nonlin: int = NL_SILU):
+    """gvec_dot += (d2 sum_c g_c out_c / dvec2) . vdot, g = g_out * phi'(aux) (aux None: g_out)  (ab2_radial_pq_hvp)."""
+    E = ctr.shape[0]
+    with _timed("radial_hvp"):
+        _check(load().ab2_radial_pq_hvp(DTYPE_ENUM[dtype], E, S, bessel_w.numel(), float(p_cut), _ptr(_contig(vec, "vec")), _ptr(_contig(vdot, "vdot")),
+                                        _ptr(ctr), _ptr(nbr), _ptr(types), _ptr(rmax_table), rmax_table.shape[0], _ptr(bessel_w),
+                                        _ptr(_contig(PQ, "PQ")), _ptr(_contig(g_out, "g_out")), _ptr(_contig(aux, "aux")) if aux is not None else None,
+                                        _ptr(_contig(gvec_dot, "gvec_dot")), int(nonlin), _stream()))
+
+
+def radial_hvp(dtype, S_rc: int, p_cut: float, vec, vdot, ctr, nbr, types, rmax_table, bessel_w, Wb, cemb, nemb, g_e0, gvec_dot):
+    """gvec_dot += (d2 sum_c g_e0_c e0_c / dvec2) . vdot of radial_fwd (ab2_radial_hvp)."""
+    E = ctr.shape[0]
+    with _timed("radial_hvp"):
+        _check(load().ab2_radial_hvp(DTYPE_ENUM[dtype], E, S_rc, bessel_w.numel(), float(p_cut), _ptr(_contig(vec, "vec")), _ptr(_contig(vdot, "vdot")),
+                                     _ptr(ctr), _ptr(nbr), _ptr(types), _ptr(rmax_table), rmax_table.shape[0], _ptr(bessel_w), _ptr(Wb), _ptr(cemb),
+                                     _ptr(nemb), _ptr(_contig(g_e0, "g_e0")), _ptr(_contig(gvec_dot, "gvec_dot")), _stream()))
+
+
+def zbl_hvp(p_cut: float, qq: float, vec, vdot, ctr, nbr, types, Z, rmax_table, gvec_dot: torch.Tensor):
+    """gvec_dot += (d2 Ez / dvec2) . vdot per edge of ``zbl`` (ab2_zbl_hvp)."""
+    E = ctr.shape[0]
+    with _timed("zbl_hvp"):
+        _check(load().ab2_zbl_hvp(DTYPE_ENUM[vec.dtype], E, Z.shape[0], float(p_cut), float(qq), _ptr(_contig(vec, "vec")), _ptr(_contig(vdot, "vdot")),
+                                  _ptr(ctr), _ptr(nbr), _ptr(types), _ptr(_contig(Z, "Z")), _ptr(_contig(rmax_table, "rmax_table")),
+                                  _ptr(_contig(gvec_dot, "gvec_dot")), _stream()))
+
+
 def neighbor_csr(pos: torch.Tensor, r_max: float, box, ncell, pbc=(True, True, True), origin=None, n_centres: Optional[int] = None):
     """Cell-list neighbour search on the device -> (row_ptr [n_centres+1] int32, nbr [E] int32, shift_vec [E,3] pos dtype).
     Orthorhombic ``box`` (3 lengths) cut into ``ncell`` (3 counts, from ``data.cell_grid``); centres are atoms
@@ -1104,6 +1198,38 @@ def fc_fold(gvec: torch.Tensor, h: float, cptr, cen, coff, ea, csr, n: int, fptr
         _check(load().ab2_fc_fold(DTYPE_ENUM[gvec.dtype], int(u0), int(u1 - u0), float(h), _ptr(cptr), _ptr(cen), _ptr(coff), _ptr(ea),
                                   _ptr(csr.row_ptr), _ptr(csr.ctr), _ptr(col_ptr), _ptr(col_perm), _ptr(fptr), _ptr(col), _ptr(Ep),
                                   _ptr(_contig(gvec, "gvec")) if gvec.numel() else None, _ptr(_contig(blocks, "blocks")), _stream()))
+
+
+def fc_gather_tangent(pos: torch.Tensor, shift: Optional[torch.Tensor], acc_dtype, atoms, cptr, cen, coff, ea, csr, Cp, Ep, u0: int, u1: int,
+                      Cb: int, Eb: int):
+    """Tangent mode of ``fc_gather``: units [u0, u1) one job each, undisplaced -> (row_ptr_b, cen_b, ctr_b, nbr_b, vec_b,
+    vdot_b [Eb,3] acc dtype = e_alpha ([nbr = j] - [ctr = j]))  (ab2_fc_gather_tangent; Cb, Eb the chunk's totals)."""
+    dev = pos.device
+    row_ptr_b = torch.empty(Cb + 1, dtype=torch.int32, device=dev)
+    cen_b = torch.empty(Cb, dtype=torch.int32, device=dev)
+    ctr_b = torch.empty(Eb, dtype=torch.int32, device=dev)
+    nbr_b = torch.empty(Eb, dtype=torch.int32, device=dev)
+    vec_b = torch.empty(Eb, 3, dtype=acc_dtype, device=dev)
+    vdot_b = torch.empty(Eb, 3, dtype=acc_dtype, device=dev)
+    if shift is not None:
+        assert shift.dtype == pos.dtype
+    with _timed("fc_gather_tangent"):
+        _check(load().ab2_fc_gather_tangent(DTYPE_ENUM[pos.dtype], DTYPE_ENUM[acc_dtype], int(u0), int(u1 - u0), int(Cb), _ptr(_contig(pos, "pos")),
+                                            _ptr(_contig(shift, "shift")) if shift is not None else None, _ptr(atoms), _ptr(cptr), _ptr(cen),
+                                            _ptr(coff), _ptr(ea), _ptr(csr.row_ptr), _ptr(csr.nbr), _ptr(Cp), _ptr(Ep), _ptr(row_ptr_b), _ptr(cen_b),
+                                            _ptr(ctr_b), _ptr(nbr_b), _ptr(vec_b), _ptr(vdot_b), _stream()))
+    return row_ptr_b, cen_b, ctr_b, nbr_b, vec_b, vdot_b
+
+
+def fc_fold_tangent(gvec_dot: torch.Tensor, cptr, cen, coff, ea, csr, n: int, fptr, col, Ep, u0: int, u1: int, blocks: torch.Tensor):
+    """Rows alpha of the blocks of units [u0, u1) = -F_dot from the chunk's gradient tangents (ab2_fc_fold_tangent)."""
+    col_ptr, col_perm = csr.transposed(n)
+    assert blocks.dtype == torch.float64
+    with _timed("fc_fold_tangent"):
+        _check(load().ab2_fc_fold_tangent(DTYPE_ENUM[gvec_dot.dtype], int(u0), int(u1 - u0), _ptr(cptr), _ptr(cen), _ptr(coff), _ptr(ea),
+                                          _ptr(csr.row_ptr), _ptr(csr.ctr), _ptr(col_ptr), _ptr(col_perm), _ptr(fptr), _ptr(col), _ptr(Ep),
+                                          _ptr(_contig(gvec_dot, "gvec_dot")) if gvec_dot.numel() else None, _ptr(_contig(blocks, "blocks")),
+                                          _stream()))
 
 
 def fc3_pairs(pj: torch.Tensor, pk: torch.Tensor, Kptr: torch.Tensor, Ken: torch.Tensor, csr):

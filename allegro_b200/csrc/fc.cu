@@ -163,6 +163,52 @@ __global__ void __launch_bounds__(FC_THREADS) fc_gather_kernel(int64_t u0, int64
     if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) row_ptr_b[Cb] = (int32_t)(eb + 2 * Ea);
 }
 
+// Tangent mode (analytic force constants): one job per unit, from centre Cp[u] - Cp[u0] and edge Ep[u] - Ep[u0], the
+// undisplaced edge vectors (the operations of ab2_edge_vec) and their tangent vdot_b = e_alpha ([nbr = j] - [ctr = j]).
+template <typename TPos, typename TAcc>
+__global__ void __launch_bounds__(FC_THREADS) fc_gather_tangent_kernel(int64_t u0, int64_t Cb, const TPos* __restrict__ pos,
+                                                                       const TPos* __restrict__ shift, const int64_t* __restrict__ atoms,
+                                                                       const int64_t* __restrict__ cptr, const int32_t* __restrict__ cen,
+                                                                       const int32_t* __restrict__ coff, const int64_t* __restrict__ ea,
+                                                                       const int32_t* __restrict__ row_ptr, const int32_t* __restrict__ nbr,
+                                                                       const int64_t* __restrict__ Cp, const int64_t* __restrict__ Ep,
+                                                                       int32_t* __restrict__ row_ptr_b, int32_t* __restrict__ cen_b,
+                                                                       int32_t* __restrict__ ctr_b, int32_t* __restrict__ nbr_b,
+                                                                       TAcc* __restrict__ vec_b, TAcc* __restrict__ vdot_b) {
+    const int64_t u = u0 + blockIdx.x;
+    const int64_t a = u / 3;
+    const int alpha = (int)(u % 3);
+    const int32_t j = (int32_t)atoms[a];
+    const int64_t c0 = cptr[a], m = cptr[a + 1] - c0;
+    const int64_t cb = Cp[u] - Cp[u0], eb = Ep[u] - Ep[u0];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int64_t c = warp; c < m; c += FC_WARPS) {
+        const int32_t k = cen[c0 + c];
+        const int64_t q = cb + c;
+        const int64_t rb = eb + coff[c0 + c];
+        if (lane == 0) {
+            row_ptr_b[q] = (int32_t)rb;
+            cen_b[q] = k;
+        }
+        const int32_t z0 = row_ptr[k], deg = row_ptr[k + 1] - z0;
+        for (int32_t e = lane; e < deg; e += 32) {
+            const int64_t z = z0 + e, zb = rb + e;
+            const int32_t jn = nbr[z];
+            ctr_b[zb] = (int32_t)q;
+            nbr_b[zb] = (int32_t)(Cb + jn);
+            const TAcc del = (TAcc)((jn == j) - (k == j));
+#pragma unroll
+            for (int x = 0; x < 3; ++x) {
+                TPos d = pos[(int64_t)jn * 3 + x] - pos[(int64_t)k * 3 + x];
+                if (shift) d += shift[z * 3 + x];
+                vec_b[zb * 3 + x] = (TAcc)d;
+                vdot_b[zb * 3 + x] = x == alpha ? del : TAcc(0);
+            }
+        }
+    }
+    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) row_ptr_b[Cb] = (int32_t)(eb + ea[a]);
+}
+
 // index of k in the ascending list s[0, m), or -1
 __device__ __forceinline__ int64_t fc_find(const int32_t* __restrict__ s, int64_t m, int32_t k) {
     int64_t lo = 0, hi = m;
@@ -179,8 +225,9 @@ __device__ __forceinline__ int64_t fc_find(const int32_t* __restrict__ s, int64_
 // One block per unit u = (a, alpha), one warp per column i of row a.  F_i of a job = sum of gvec over the job's edges
 // centred on i (row i, when i is in C_j) - sum over its edges with neighbour i (column i of the transposed list, kept
 // when the edge's centre is in C_j).  Each lane sums (g+ - g-) in fp64 over its strided share in that order; the warp
-// reduces with the fixed butterfly of warp_sum.
-template <typename TAcc>
+// reduces with the fixed butterfly of warp_sum.  TANGENT: one job per unit holding the tangents of the per-edge
+// gradients, folded as -F_dot (no difference, no 1/(2h): inv2h = 1).
+template <typename TAcc, bool TANGENT>
 __global__ void __launch_bounds__(FC_THREADS) fc_fold_kernel(int64_t u0, double inv2h, const int64_t* __restrict__ cptr,
                                                              const int32_t* __restrict__ cen, const int32_t* __restrict__ coff,
                                                              const int64_t* __restrict__ ea, const int32_t* __restrict__ row_ptr,
@@ -193,7 +240,7 @@ __global__ void __launch_bounds__(FC_THREADS) fc_fold_kernel(int64_t u0, double 
     const int alpha = (int)(u % 3);
     const int64_t c0 = cptr[a], m = cptr[a + 1] - c0, Ea = ea[a];
     const int32_t* __restrict__ cs = cen + c0;
-    const int64_t ep = 2 * (Ep[u] - Ep[u0]), em = ep + Ea;
+    const int64_t ep = (TANGENT ? 1 : 2) * (Ep[u] - Ep[u0]), em = ep + Ea;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int64_t p = fptr[a] + warp; p < fptr[a + 1]; p += FC_WARPS) {
         const int32_t i = col[p];
@@ -204,9 +251,9 @@ __global__ void __launch_bounds__(FC_THREADS) fc_fold_kernel(int64_t u0, double 
             const int32_t deg = row_ptr[i + 1] - row_ptr[i];
             for (int32_t e = lane; e < deg; e += 32) {
                 const int64_t zp = (ep + off + e) * 3, zm = (em + off + e) * 3;
-                s0 += (double)gvec[zp + 0] - (double)gvec[zm + 0];
-                s1 += (double)gvec[zp + 1] - (double)gvec[zm + 1];
-                s2 += (double)gvec[zp + 2] - (double)gvec[zm + 2];
+                s0 += TANGENT ? (double)gvec[zp + 0] : (double)gvec[zp + 0] - (double)gvec[zm + 0];
+                s1 += TANGENT ? (double)gvec[zp + 1] : (double)gvec[zp + 1] - (double)gvec[zm + 1];
+                s2 += TANGENT ? (double)gvec[zp + 2] : (double)gvec[zp + 2] - (double)gvec[zm + 2];
             }
         }
         for (int32_t t = col_ptr[i] + lane; t < col_ptr[i + 1]; t += 32) {
@@ -216,9 +263,9 @@ __global__ void __launch_bounds__(FC_THREADS) fc_fold_kernel(int64_t u0, double 
             if (ck < 0) continue;
             const int64_t off = coff[c0 + ck] + (z - row_ptr[k]);
             const int64_t zp = (ep + off) * 3, zm = (em + off) * 3;
-            s0 -= (double)gvec[zp + 0] - (double)gvec[zm + 0];
-            s1 -= (double)gvec[zp + 1] - (double)gvec[zm + 1];
-            s2 -= (double)gvec[zp + 2] - (double)gvec[zm + 2];
+            s0 -= TANGENT ? (double)gvec[zp + 0] : (double)gvec[zp + 0] - (double)gvec[zm + 0];
+            s1 -= TANGENT ? (double)gvec[zp + 1] : (double)gvec[zp + 1] - (double)gvec[zm + 1];
+            s2 -= TANGENT ? (double)gvec[zp + 2] : (double)gvec[zp + 2] - (double)gvec[zm + 2];
         }
         s0 = warp_sum(s0);
         s1 = warp_sum(s1);
@@ -475,11 +522,54 @@ extern "C" int ab2_fc_fold(int acc_dtype, int64_t u0, int64_t U, double h, const
     const double inv2h = 1.0 / (2.0 * h);
     cudaStream_t st = (cudaStream_t)stream;
     if (acc_dtype == AB2_F64)
-        fc_fold_kernel<double><<<(unsigned)U, FC_THREADS, 0, st>>>(u0, inv2h, cptr, cen, coff, ea, row_ptr, ctr, col_ptr, col_perm, fptr, col, Ep,
+        fc_fold_kernel<double, false><<<(unsigned)U, FC_THREADS, 0, st>>>(u0, inv2h, cptr, cen, coff, ea, row_ptr, ctr, col_ptr, col_perm, fptr, col, Ep,
                                                                    (const double*)gvec, blocks);
     else
-        fc_fold_kernel<float><<<(unsigned)U, FC_THREADS, 0, st>>>(u0, inv2h, cptr, cen, coff, ea, row_ptr, ctr, col_ptr, col_perm, fptr, col, Ep,
+        fc_fold_kernel<float, false><<<(unsigned)U, FC_THREADS, 0, st>>>(u0, inv2h, cptr, cen, coff, ea, row_ptr, ctr, col_ptr, col_perm, fptr, col, Ep,
                                                                   (const float*)gvec, blocks);
+    AB2_CUDA_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int ab2_fc_gather_tangent(int pos_dtype, int acc_dtype, int64_t u0, int64_t U, int64_t Cb, const void* pos, const void* shift,
+                                     const int64_t* atoms, const int64_t* cptr, const int32_t* cen, const int32_t* coff, const int64_t* ea,
+                                     const int32_t* row_ptr, const int32_t* nbr, const int64_t* Cp, const int64_t* Ep, int32_t* row_ptr_b,
+                                     int32_t* cen_b, int32_t* ctr_b, int32_t* nbr_b, void* vec_b, void* vdot_b, void* stream) {
+    AB2_CHECK_ARG(pos_dtype == AB2_F64 || pos_dtype == AB2_F32, "positions must be fp64 or fp32");
+    AB2_CHECK_ARG(acc_dtype == AB2_F64 || acc_dtype == AB2_F32, "edge vectors must be fp64 or fp32");
+    AB2_CHECK_ARG(u0 >= 0 && U >= 1 && U <= 0x7fffffffLL && Cb >= 1 && Cb <= 0x7fffffffLL, "sizes");
+    AB2_CHECK_ARG(pos && atoms && cptr && cen && coff && ea && row_ptr && Cp && Ep && row_ptr_b && cen_b, "null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    const unsigned g = (unsigned)U;
+#define AB2_FC_GATHER_T(TP, TA)                                                                                                       \
+    fc_gather_tangent_kernel<TP, TA><<<g, FC_THREADS, 0, st>>>(u0, Cb, (const TP*)pos, (const TP*)shift, atoms, cptr, cen, coff, ea, row_ptr, \
+                                                               nbr, Cp, Ep, row_ptr_b, cen_b, ctr_b, nbr_b, (TA*)vec_b, (TA*)vdot_b)
+    if (pos_dtype == AB2_F64 && acc_dtype == AB2_F64)
+        AB2_FC_GATHER_T(double, double);
+    else if (pos_dtype == AB2_F64)
+        AB2_FC_GATHER_T(double, float);
+    else if (acc_dtype == AB2_F64)
+        AB2_FC_GATHER_T(float, double);
+    else
+        AB2_FC_GATHER_T(float, float);
+#undef AB2_FC_GATHER_T
+    AB2_CUDA_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int ab2_fc_fold_tangent(int acc_dtype, int64_t u0, int64_t U, const int64_t* cptr, const int32_t* cen, const int32_t* coff,
+                                   const int64_t* ea, const int32_t* row_ptr, const int32_t* ctr, const int32_t* col_ptr, const int32_t* col_perm,
+                                   const int64_t* fptr, const int32_t* col, const int64_t* Ep, const void* gvec_dot, double* blocks, void* stream) {
+    AB2_CHECK_ARG(acc_dtype == AB2_F64 || acc_dtype == AB2_F32, "gradients must be fp64 or fp32");
+    AB2_CHECK_ARG(u0 >= 0 && U >= 1 && U <= 0x7fffffffLL, "sizes");
+    AB2_CHECK_ARG(cptr && cen && coff && ea && row_ptr && col_ptr && fptr && col && Ep && blocks, "null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (acc_dtype == AB2_F64)
+        fc_fold_kernel<double, true><<<(unsigned)U, FC_THREADS, 0, st>>>(u0, 1.0, cptr, cen, coff, ea, row_ptr, ctr, col_ptr, col_perm, fptr, col, Ep,
+                                                                         (const double*)gvec_dot, blocks);
+    else
+        fc_fold_kernel<float, true><<<(unsigned)U, FC_THREADS, 0, st>>>(u0, 1.0, cptr, cen, coff, ea, row_ptr, ctr, col_ptr, col_perm, fptr, col, Ep,
+                                                                        (const float*)gvec_dot, blocks);
     AB2_CUDA_LAUNCH_CHECK();
     return 0;
 }

@@ -397,3 +397,180 @@ extern "C" int ab2_radial_pq_bwd(int dtype, int64_t E, int S, int num_bessels, d
     return ab2_radial_pq_bwd_nl(dtype, E, S, num_bessels, p_cut, vec, ctr, nbr, types, rmax_table, num_types, bessel_w, PQ, g_out, aux, gvec, stream,
                                 AB2_NL_SILU);
 }
+
+// ---------------------------------------------------------------------------------------
+// Tangents of the radial embedding along edge-vector directions vdot (nn._hessian, DESIGN.md section 4.11).  The
+// embedding depends on vec through x = |r| / r_max only, so with F(x) = sum_c g_c out_c(x):
+//   jvp:  out_dot[z][c] = sum_n B_n'(x) x_dot M[n][c],                 x_dot = (r_hat . vdot) / r_max
+//   hvp:  gvec_dot[z] += F''(x) (r_hat.v) r_hat / r_max^2 + F'(x) / (r_max |r|) (v - (r_hat.v) r_hat)
+// M = PQ[pair] (ab2_radial_pq_*), or typeemb(t_c,t_n)[c] * Wb[n][c] (ab2_radial_*).  Beyond r_max every term is
+// exactly zero, as in the primal kernels.  One thread per edge.
+// ---------------------------------------------------------------------------------------
+// B_n, B_n' and B_n'' in x (zero for x >= 1): B = s f with s = sin(pi w x)/(pi x), s' = (w cos(pi w x) - s)/x,
+// s'' = -(pi w)^2 s - 2 s'/x, f the polynomial cutoff
+template <typename TAcc>
+__device__ __forceinline__ void bessel_basis2(TAcc x, TAcc p, int nb, const TAcc* __restrict__ bw, TAcc* dB, TAcc* d2B) {
+    const TAcc PI = TAcc(3.14159265358979323846);
+    if (x >= TAcc(1)) {
+        for (int n = 0; n < nb; ++n) dB[n] = d2B[n] = TAcc(0);
+        return;
+    }
+    const TAcc xp = ab2_pow(x, p);
+    const TAcc a = (p + 1) * (p + 2) / 2, b = p * (p + 2), c = p * (p + 1) / 2;
+    const TAcc f = TAcc(1) - a * xp + b * xp * x - c * xp * x * x;
+    const TAcc df = -a * p * xp / x + b * (p + 1) * xp - c * (p + 2) * xp * x;
+    const TAcc d2f = -a * p * (p - 1) * xp / (x * x) + b * (p + 1) * p * xp / x - c * (p + 2) * (p + 1) * xp;
+    const TAcc inv = TAcc(1) / (PI * x);
+    for (int n = 0; n < nb; ++n) {
+        const TAcc arg = PI * bw[n] * x;
+        const TAcc s = ab2_sin(arg) * inv;
+        const TAcc ds = (bw[n] * ab2_cos(arg) - s) / x;
+        const TAcc d2s = -(PI * bw[n]) * (PI * bw[n]) * s - TAcc(2) * ds / x;
+        dB[n] = ds * f + s * df;
+        d2B[n] = d2s * f + TAcc(2) * ds * df + s * d2f;
+    }
+}
+
+// the edge's geometry: |r|, r_hat . vdot, type pair
+template <typename TAcc>
+__device__ __forceinline__ void radial_edge(int64_t z, const TAcc* __restrict__ vec, const TAcc* __restrict__ vdot, const int32_t* __restrict__ ctr,
+                                            const int32_t* __restrict__ nbr, const int32_t* __restrict__ types, int num_types, TAcc (&v)[3],
+                                            TAcc (&w)[3], TAcc& r, TAcc& uv, int& tc, int& tn) {
+    for (int a = 0; a < 3; ++a) {
+        v[a] = vec[z * 3 + a];
+        w[a] = vdot[z * 3 + a];
+    }
+    r = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+    uv = (v[0] * w[0] + v[1] * w[1] + v[2] * w[2]) / r;
+    tc = types[ctr[z]];
+    tn = types[nbr[z]];
+}
+
+// M[n][c] of the two routes
+template <typename TAcc, bool PQ_FORM>
+__device__ __forceinline__ TAcc radial_m(int n, int c, int S, int pair, int nb, int tc, int tn, const TAcc* __restrict__ PQ, const TAcc* __restrict__ Wb,
+                                         const TAcc* __restrict__ cemb, const TAcc* __restrict__ nemb) {
+    if (PQ_FORM) return PQ[((int64_t)pair * nb + n) * S + c];
+    const int half = S >> 1;
+    const TAcc te = (c < half) ? cemb[tc * half + c] : nemb[tn * half + (c - half)];
+    return te * Wb[n * S + c];
+}
+
+template <typename TAct, typename TAcc, bool PQ_FORM>
+__global__ void __launch_bounds__(128) radial_jvp_kernel(int64_t E, int S, int nb, TAcc p, const TAcc* __restrict__ vec, const TAcc* __restrict__ vdot,
+                                                         const int32_t* __restrict__ ctr, const int32_t* __restrict__ nbr,
+                                                         const int32_t* __restrict__ types, const TAcc* __restrict__ rmax_table, int num_types,
+                                                         const TAcc* __restrict__ bw, const TAcc* __restrict__ PQ, const TAcc* __restrict__ Wb,
+                                                         const TAcc* __restrict__ cemb, const TAcc* __restrict__ nemb, TAct* __restrict__ out) {
+    const int64_t z = (int64_t)blockIdx.x * 128 + threadIdx.x;
+    if (z >= E) return;
+    TAcc v[3], w[3], r, uv;
+    int tc, tn;
+    radial_edge(z, vec, vdot, ctr, nbr, types, num_types, v, w, r, uv, tc, tn);
+    const int pair = tc * num_types + tn;
+    const TAcc rmax = rmax_table[pair];
+    TAcc dB[AB2_MAX_BESSEL], d2B[AB2_MAX_BESSEL];
+    bessel_basis2(r / rmax, p, nb, bw, dB, d2B);
+    const TAcc xd = uv / rmax;
+    for (int c = 0; c < S; ++c) {
+        TAcc s = TAcc(0);
+        for (int n = 0; n < nb; ++n) s += dB[n] * radial_m<TAcc, PQ_FORM>(n, c, S, pair, nb, tc, tn, PQ, Wb, cemb, nemb);
+        out[z * S + c] = from_acc<TAct>(s * xd);
+    }
+}
+
+template <typename TAct, typename TAcc, bool PQ_FORM, int NL>
+__global__ void __launch_bounds__(128) radial_hvp_kernel(int64_t E, int S, int nb, TAcc p, const TAcc* __restrict__ vec, const TAcc* __restrict__ vdot,
+                                                         const int32_t* __restrict__ ctr, const int32_t* __restrict__ nbr,
+                                                         const int32_t* __restrict__ types, const TAcc* __restrict__ rmax_table, int num_types,
+                                                         const TAcc* __restrict__ bw, const TAcc* __restrict__ PQ, const TAcc* __restrict__ Wb,
+                                                         const TAcc* __restrict__ cemb, const TAcc* __restrict__ nemb, const TAct* __restrict__ g_out,
+                                                         const TAct* __restrict__ aux, TAcc* __restrict__ gvec_dot) {
+    const int64_t z = (int64_t)blockIdx.x * 128 + threadIdx.x;
+    if (z >= E) return;
+    TAcc v[3], w[3], r, uv;
+    int tc, tn;
+    radial_edge(z, vec, vdot, ctr, nbr, types, num_types, v, w, r, uv, tc, tn);
+    const int pair = tc * num_types + tn;
+    const TAcc rmax = rmax_table[pair];
+    TAcc dB[AB2_MAX_BESSEL], d2B[AB2_MAX_BESSEL];
+    bessel_basis2(r / rmax, p, nb, bw, dB, d2B);
+    TAcc F1 = TAcc(0), F2 = TAcc(0);
+    for (int c = 0; c < S; ++c) {
+        TAcc gc = to_acc<TAcc>(g_out[z * S + c]);
+        if (aux) gc *= dact_f<NL>(to_acc<TAcc>(aux[z * S + c]));
+        TAcc s1 = TAcc(0), s2 = TAcc(0);
+        for (int n = 0; n < nb; ++n) {
+            const TAcc m = radial_m<TAcc, PQ_FORM>(n, c, S, pair, nb, tc, tn, PQ, Wb, cemb, nemb);
+            s1 += dB[n] * m;
+            s2 += d2B[n] * m;
+        }
+        F1 += gc * s1;
+        F2 += gc * s2;
+    }
+    const TAcc ir = TAcc(1) / r, a = F2 * uv / (rmax * rmax), b = F1 / (rmax * r);
+    for (int k = 0; k < 3; ++k) gvec_dot[z * 3 + k] += a * v[k] * ir + b * (w[k] - uv * v[k] * ir);
+}
+
+extern "C" int ab2_radial_pq_jvp(int dtype, int64_t E, int S, int num_bessels, double p_cut, const void* vec, const void* vdot,
+                                 const int32_t* ctr, const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types,
+                                 const void* bessel_w, const void* PQ, void* out, void* stream) {
+    if (E == 0) return 0;
+    AB2_CHECK_ARG(vec && vdot && ctr && nbr && types && rmax_table && bessel_w && PQ && out, "null pointer");
+    AB2_CHECK_ARG(num_bessels == 8 && S > 0 && S <= 128, "radial_pq: 8 Bessel functions, at most 128 output columns");
+    cudaStream_t st = (cudaStream_t)stream;
+    AB2_DISPATCH_DTYPE(dtype, radial_jvp_kernel<TAct, TAcc, true><<<ab2_blocks(E, 128), 128, 0, st>>>(
+                                  E, S, num_bessels, (TAcc)p_cut, (const TAcc*)vec, (const TAcc*)vdot, ctr, nbr, types, (const TAcc*)rmax_table,
+                                  num_types, (const TAcc*)bessel_w, (const TAcc*)PQ, nullptr, nullptr, nullptr, (TAct*)out));
+    AB2_CUDA_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int ab2_radial_jvp(int dtype, int64_t E, int S_rc, int num_bessels, double p_cut, const void* vec, const void* vdot, const int32_t* ctr,
+                              const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types, const void* bessel_w,
+                              const void* Wb, const void* center_embed, const void* neighbor_embed, void* e0_dot, void* stream) {
+    if (E == 0) return 0;
+    AB2_CHECK_ARG(vec && vdot && ctr && nbr && types && rmax_table && bessel_w && Wb && center_embed && neighbor_embed && e0_dot, "null pointer");
+    AB2_CHECK_ARG(num_bessels > 0 && num_bessels <= AB2_MAX_BESSEL && S_rc > 0 && S_rc % 2 == 0, "num_bessels / embedding dim");
+    cudaStream_t st = (cudaStream_t)stream;
+    AB2_DISPATCH_DTYPE(dtype, radial_jvp_kernel<TAct, TAcc, false><<<ab2_blocks(E, 128), 128, 0, st>>>(
+                                  E, S_rc, num_bessels, (TAcc)p_cut, (const TAcc*)vec, (const TAcc*)vdot, ctr, nbr, types, (const TAcc*)rmax_table,
+                                  num_types, (const TAcc*)bessel_w, nullptr, (const TAcc*)Wb, (const TAcc*)center_embed,
+                                  (const TAcc*)neighbor_embed, (TAct*)e0_dot));
+    AB2_CUDA_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int ab2_radial_pq_hvp(int dtype, int64_t E, int S, int num_bessels, double p_cut, const void* vec, const void* vdot,
+                                 const int32_t* ctr, const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types,
+                                 const void* bessel_w, const void* PQ, const void* g_out, const void* aux, void* gvec_dot, int nonlin,
+                                 void* stream) {
+    AB2_CHECK_ARG(nonlin == AB2_NL_SILU || nonlin == AB2_NL_MISH || nonlin == AB2_NL_GELU, "nonlinearity");
+    if (E == 0) return 0;
+    AB2_CHECK_ARG(vec && vdot && ctr && nbr && types && rmax_table && bessel_w && PQ && g_out && gvec_dot, "null pointer");
+    AB2_CHECK_ARG(num_bessels == 8 && S > 0 && S <= 128, "radial_pq: 8 Bessel functions, at most 128 output columns");
+    cudaStream_t st = (cudaStream_t)stream;
+    AB2_DISPATCH_NL(nonlin, AB2_DISPATCH_DTYPE(dtype, radial_hvp_kernel<TAct, TAcc, true, NL><<<ab2_blocks(E, 128), 128, 0, st>>>(
+                                  E, S, num_bessels, (TAcc)p_cut, (const TAcc*)vec, (const TAcc*)vdot, ctr, nbr, types, (const TAcc*)rmax_table,
+                                  num_types, (const TAcc*)bessel_w, (const TAcc*)PQ, nullptr, nullptr, nullptr, (const TAct*)g_out,
+                                  (const TAct*)aux, (TAcc*)gvec_dot)));
+    AB2_CUDA_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int ab2_radial_hvp(int dtype, int64_t E, int S_rc, int num_bessels, double p_cut, const void* vec, const void* vdot, const int32_t* ctr,
+                              const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types, const void* bessel_w,
+                              const void* Wb, const void* center_embed, const void* neighbor_embed, const void* g_e0, void* gvec_dot,
+                              void* stream) {
+    if (E == 0) return 0;
+    AB2_CHECK_ARG(vec && vdot && ctr && nbr && types && rmax_table && bessel_w && Wb && center_embed && neighbor_embed && g_e0 && gvec_dot,
+                  "null pointer");
+    AB2_CHECK_ARG(num_bessels > 0 && num_bessels <= AB2_MAX_BESSEL && S_rc > 0 && S_rc % 2 == 0, "num_bessels / embedding dim");
+    cudaStream_t st = (cudaStream_t)stream;
+    AB2_DISPATCH_DTYPE(dtype, radial_hvp_kernel<TAct, TAcc, false, AB2_NL_SILU><<<ab2_blocks(E, 128), 128, 0, st>>>(
+                                  E, S_rc, num_bessels, (TAcc)p_cut, (const TAcc*)vec, (const TAcc*)vdot, ctr, nbr, types, (const TAcc*)rmax_table,
+                                  num_types, (const TAcc*)bessel_w, nullptr, (const TAcc*)Wb, (const TAcc*)center_embed,
+                                  (const TAcc*)neighbor_embed, (const TAct*)g_e0, nullptr, (TAcc*)gvec_dot));
+    AB2_CUDA_LAUNCH_CHECK();
+    return 0;
+}

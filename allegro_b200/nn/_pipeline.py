@@ -154,11 +154,14 @@ class AllegroCore:
             self.chain = _lib.tp_chain_plan(dtype, U, l0["cgw"], l1["cgw"])
 
     # ------------------------------------------------------------------------------------
-    def forward(self, csr: EdgeCSR, vec: torch.Tensor, x_emb: Optional[torch.Tensor], keep: bool = True, fill_embed=None):
+    def forward(self, csr: EdgeCSR, vec: torch.Tensor, x_emb: Optional[torch.Tensor], keep: bool = True, fill_embed=None,
+                stored_v: bool = False):
         """vec [E,3] (acc dtype), x_emb [E,S_in] (act dtype), both in CSR edge order.
         Returns (Ei [N] acc dtype, X [E,S(L+1)], Ez [E,1], saved-for-backward).
         ``fill_embed(w0, x0, omega0)``: instead of x_emb, a callback that fills the three outputs of the embed GEMM
-        (the upstream MLP with the embed linears folded into its last layer, energy_forces)."""
+        (the upstream MLP with the embed linears folded into its last layer, energy_forces).
+        ``stored_v``: take the stored-V path even where the composed tensor products would run, so every V_l is kept
+        (the tangent of nn._hessian reads them)."""
         E, N, U, S, L, D = csr.num_edges, csr.num_atoms, self.U, self.S, self.L, self.D
         dt, dev = self.dtype, self.device
         assert vec.dtype == self.acc and (fill_embed is not None or x_emb.dtype == dt)
@@ -178,7 +181,7 @@ class AllegroCore:
         gammas, pre_lat = [], []
         Ez = torch.empty(E, 1, dtype=dt, device=dev)
         pre_read = None
-        chain = self.chain
+        chain = None if stored_v else self.chain
         for l, ly in enumerate(self.layers):
             _lib.set_tag(f"fwd.L{l}")
             gamma = _lib.env_sum(dt, self.lmax, N, U, csr.row_ptr, Y, omega[l], self.sf)

@@ -20,6 +20,15 @@ bitwise for fp32 models, to rounding for fp64 models (their tensor-product adjoi
 gives phono3py's third-order constants the same way: a pair of displacements (j, alpha), (k, beta) changes the mixed
 difference only through the rows of C_j n C_k, so each unit (j, k, alpha, beta) evaluates those rows alone, in four jobs
 (ab2_fc3_* kernels, DESIGN.md section 4.10).
+
+    hv = hessian_vector_product(model, pos, cell, atom_types, v, pbc=True)
+    fc = analytic_force_constants(model, pos, cell, atom_types, pbc=True, atoms=None, max_edges=None)
+
+are exact second derivatives instead: forward-mode differentiation of the fused force path (nn._hessian, DESIGN.md
+section 4.11).  ``hessian_vector_product`` gives d2E/dr2 . v for the whole frame (no dense Hessian: Lanczos lowest modes,
+dimer searches, Hessian-free normal modes of large cells); ``analytic_force_constants`` gives the blocks of
+``force_constants`` with no step, no step error and Phi(j,i)_{alpha beta} = Phi(i,j)_{beta alpha} to rounding, each unit
+(j, alpha) one job on the undisplaced rows of C_j with the edge tangent e_alpha ([nbr = j] - [ctr = j]).
 """
 from __future__ import annotations
 
@@ -159,22 +168,25 @@ def force_constants(model, pos: torch.Tensor, cell: Optional[torch.Tensor], atom
     return ForceConstants(atoms_d, fptr, col.long(), blocks, n)
 
 
-def _checked(name, model, pos, cell, atom_types, pbc, atoms, displacement, max_edges):
-    """The refusals shared by force_constants and third_order_force_constants, before any kernel runs -> (the fused
-    model, the step h, pbc as three bools, the displaced atoms as a CPU int64 tensor)."""
+def _checked(name, model, pos, cell, atom_types, pbc, atoms, displacement, max_edges, max_atoms: int = _lib.FC_MAX_ATOMS):
+    """The refusals shared by force_constants, third_order_force_constants and the analytic entry points (``displacement``
+    None: no step), before any kernel runs -> (the fused model, the step h or None, pbc as three bools, the displaced
+    atoms as a CPU int64 tensor)."""
     inner = _fused(model, name)
     if not torch.is_tensor(pos) or not pos.is_cuda or not torch.is_tensor(atom_types) or not atom_types.is_cuda:
         raise RuntimeError("allegro_b200: inputs must be CUDA tensors (no CPU fallback on the hot path)")
-    h = float(displacement)
-    if not math.isfinite(h) or h <= 0.0:
-        raise ValueError(f"displacement must be finite and > 0, got {displacement!r}")
+    h = None
+    if displacement is not None:
+        h = float(displacement)
+        if not math.isfinite(h) or h <= 0.0:
+            raise ValueError(f"displacement must be finite and > 0, got {displacement!r}")
     if pos.dim() != 2 or pos.shape[1] != 3 or pos.dtype not in (torch.float32, torch.float64):
         raise ValueError(f"pos must be fp32 or fp64 [N,3], got {pos.dtype} of shape {tuple(pos.shape)}")
     n = pos.shape[0]
     if atom_types.dim() != 1 or atom_types.shape[0] != n or atom_types.dtype.is_floating_point or atom_types.dtype == torch.bool:
         raise ValueError(f"atom_types must be [N] = [{n}] integers, got {atom_types.dtype} of shape {tuple(atom_types.shape)}")
-    if n < 1 or n > _lib.FC_MAX_ATOMS:
-        raise ValueError(f"{name} takes frames of 1 .. {_lib.FC_MAX_ATOMS} atoms, got {n}")
+    if n < 1 or n > max_atoms:
+        raise ValueError(f"{name} takes frames of 1 .. {max_atoms} atoms, got {n}")
     pbc = _pbc3(pbc)
     if any(pbc) and (cell is None or not D.is_regular_cell(cell)):
         raise ValueError("a periodic axis needs a regular cell (data.is_regular_cell)")
@@ -296,3 +308,104 @@ def third_order_force_constants(model, pos: torch.Tensor, cell: Optional[torch.T
         _lib.fc3_fold(gvec, hp, iptr, icen, ioff, Pe, csr, n, rptr, col, u0, u1, blocks)
         u0 = u1
     return ThirdOrderForceConstants(atoms_d, pair_ptr, pair_col.long(), rptr, col.long(), blocks, n)
+
+
+def _frame_list(inner, pos, cell, pbc, types_i32):
+    """The device list at r_max (pruned to the per-edge-type cutoffs where the model has them) -> (csr, shift)."""
+    from .calculator import prune_table
+
+    cutoffs = prune_table(inner, 0.0)
+    prune = {} if cutoffs is None else dict(types=types_i32, cutoffs=cutoffs)
+    return D.neighbor_csr(pos, inner.r_max, cell, pbc, **prune)
+
+
+def hessian_vector_product(model, pos: torch.Tensor, cell: Optional[torch.Tensor], atom_types: torch.Tensor, v: torch.Tensor,
+                           pbc=True) -> torch.Tensor:
+    """d2E/dr2 . v [N,3] for the whole frame, exact to rounding (forward mode over the fused force path, no step), in the
+    model's accumulate dtype.  ``v`` [N,3] floating on the device; the edge tangents are v[nbr] - v[ctr], so an edge from an
+    atom to its own image does not move.  Arguments and refusals as ``force_constants`` (without its atom limit); a ``v``
+    that is not a floating [N,3] device tensor raises ValueError.  A frame without edges gives zeros."""
+    name = "hessian_vector_product"
+    inner, _, pbc, _ = _checked(name, model, pos, cell, atom_types, pbc, None, None, None, max_atoms=(1 << 31) - 1)
+    n = pos.shape[0]
+    if (not torch.is_tensor(v) or not v.is_cuda or v.device != pos.device or not v.dtype.is_floating_point or v.dim() != 2
+            or tuple(v.shape) != (n, 3)):
+        desc = f"{v.dtype} of shape {tuple(v.shape)} on {v.device}" if torch.is_tensor(v) else type(v).__name__
+        raise ValueError(f"v must be a floating [N,3] = [{n},3] tensor on {pos.device}, got {desc}")
+    core = inner.core()
+    dev = pos.device
+    pos = pos.detach().contiguous()
+    types_i32 = atom_types.to(torch.int32).contiguous()
+    if cell is not None:
+        cell = cell.detach().reshape(3, 3).to(device=dev, dtype=pos.dtype)
+    csr, shift = _frame_list(inner, pos, cell, pbc, types_i32)
+    if csr.num_edges == 0:
+        return torch.zeros(n, 3, dtype=core.acc, device=dev)
+    vec = _lib.edge_vec(pos, csr.ctr, csr.nbr, shift, core.acc)
+    vdot = _lib.edge_vec(v.detach().to(core.acc).contiguous(), csr.ctr, csr.nbr, None, core.acc)
+    gscale, pair = _energy_terms(inner, core, atom_types, dev)
+    from .nn._hessian import edge_energy_grad_tangent
+
+    _, gvec_dot = edge_energy_grad_tangent(core, inner._upstream, csr, vec, vdot, types_i32, gscale, pair)
+    return -_lib.force_scatter(gvec_dot, csr, n)
+
+
+def analytic_force_constants(model, pos: torch.Tensor, cell: Optional[torch.Tensor], atom_types: torch.Tensor, pbc=True, atoms=None,
+                             max_edges: Optional[int] = None) -> ForceConstants:
+    """The force constants of ``force_constants`` (same ``ForceConstants`` layout, phonopy's convention) as exact second
+    derivatives: each unit (displaced atom j, axis alpha) is one tangent job on the undisplaced rows of C_j, folded
+    without a step.  The plan is that of ``force_constants`` on a list built at r_max exactly.  Arguments and refusals as
+    ``force_constants`` without ``displacement``; chunks of at most ``max_edges`` batched edges (default: half the free
+    device memory over ``nn._hessian.hvp_edge_bytes``).  A displaced atom's blocks do not depend on the chunking or on the
+    other displaced atoms: bitwise for fp32 models, to rounding for fp64 models."""
+    name = "analytic_force_constants"
+    inner, _, pbc, atoms_h = _checked(name, model, pos, cell, atom_types, pbc, atoms, None, max_edges)
+    n = pos.shape[0]
+    core = inner.core()
+    dev = pos.device
+    pos = pos.detach().contiguous()
+    types_i32 = atom_types.to(torch.int32).contiguous()
+    if cell is not None:
+        cell = cell.detach().reshape(3, 3).to(device=dev, dtype=pos.dtype)
+    csr, shift = _frame_list(inner, pos, cell, pbc, types_i32)
+    A = atoms_h.shape[0]
+    atoms_d = atoms_h.to(dev)
+    cptr, cen, coff, ea = _lib.fc_centres(atoms_d, csr, n)
+    fptr, col = _lib.fc_columns(cptr, cen, csr, n)
+    blocks = torch.empty(col.shape[0], 3, 3, dtype=torch.float64, device=dev)
+    # units u = 3 a + alpha, each ONE job of m_a centres and E_a edges
+    Cp = _lib._prefix((cptr[1:] - cptr[:-1]).repeat_interleave(3))
+    Ep = _lib._prefix(ea.repeat_interleave(3))
+    Cp_h, Ep_h = Cp.cpu(), Ep.cpu()
+    from .nn._hessian import edge_energy_grad_tangent, hvp_edge_bytes
+
+    if max_edges is not None:
+        cap = int(max_edges)
+    else:
+        free, _ = torch.cuda.mem_get_info(dev)
+        cap = int(max(1, min(MAX_CHUNK_EDGES, free // 2 // hvp_edge_bytes(core))))
+    unit_edges = Ep_h[1:] - Ep_h[:-1]
+    if unit_edges.numel() and int(unit_edges.max()) > cap:
+        raise ValueError(f"max_edges = {cap} is below the {int(unit_edges.max())} edges of one displaced atom's cluster")
+    gscale, pair = _energy_terms(inner, core, atom_types, dev)
+    U = 3 * A
+    u0 = 0
+    while u0 < U:
+        # the largest run of units whose jobs fit in cap edges
+        u1 = int(torch.searchsorted(Ep_h, Ep_h[u0] + cap, right=True)) - 1
+        u1 = max(u0 + 1, min(u1, U))
+        while u1 > u0 + 1 and int(Cp_h[u1] - Cp_h[u0]) + n > MAX_CHUNK_EDGES:  # batched centres and atoms index int32 too
+            u1 = u0 + (u1 - u0) // 2
+        Cb, Eb = int(Cp_h[u1] - Cp_h[u0]), int(Ep_h[u1] - Ep_h[u0])
+        if Eb == 0:
+            # every cluster of the chunk is an isolated atom: zero blocks
+            gvec_dot = torch.zeros(0, 3, dtype=core.acc, device=dev)
+        else:
+            row_ptr_b, cen_b, ctr_b, nbr_b, vec_b, vdot_b = _lib.fc_gather_tangent(pos, shift, core.acc, atoms_d, cptr, cen, coff, ea, csr, Cp, Ep,
+                                                                                   u0, u1, Cb, Eb)
+            csr_b = D.EdgeCSR(Cb, ctr_b, nbr_b, row_ptr_b, None, csr.max_degree)
+            types_b = torch.cat([types_i32[cen_b.long()], types_i32])
+            _, gvec_dot = edge_energy_grad_tangent(core, inner._upstream, csr_b, vec_b, vdot_b, types_b, gscale[cen_b.long()], pair)
+        _lib.fc_fold_tangent(gvec_dot, cptr, cen, coff, ea, csr, n, fptr, col, Ep, u0, u1, blocks)
+        u0 = u1
+    return ForceConstants(atoms_d, fptr, col.long(), blocks, n)

@@ -607,6 +607,50 @@ int ab2_zbl(int acc_dtype, int64_t E, int num_types, double p_cut, double qq, co
             const int32_t* nbr, const int32_t* types, const void* Z, const void* rmax_table, void* Ez, void* gvec,
             void* stream);
 
+/* ---- tangents of the per-edge force path (nn._hessian: Hessian-vector products, analytic force constants) ------------
+ * The edge vectors vec [E][3] move along vdot [E][3] (both in the accumulate dtype).  Each kernel gives the tangent of
+ * one nonlinear step of the primal; the multilinear steps take their tangents from the primal kernels (DESIGN.md section
+ * 4.11).  Every entry returns 0 at once for E = 0 (n = 0).
+ *   ab2_sh_jvp:       Yd [E][(lmax+1)^2] = dY(vec/|vec|)/dvec . vdot  (the polynomials of ab2_sh_fwd, lmax 0..4)
+ *   ab2_sh_hvp:       gvec_dot[z] += (d2 sum_k gY[z][k] Y_k / dvec2) . vdot[z]
+ *   ab2_act_bwd_jvp:  out = ga_dot * phi'(pre) + ga * phi''(pre) * pre_dot, n elements of the activation dtype, phi the
+ *                     nonlinearity `nonlin` (AB2_NL_*); ga_dot nullable (= 0)
+ *   ab2_radial_pq_jvp / ab2_radial_jvp:  out = d out / dvec . vdot of ab2_radial_pq_fwd / ab2_radial_fwd (same arguments)
+ *   ab2_radial_pq_hvp / ab2_radial_hvp:  gvec_dot[z] += (d2 sum_c g[z][c] out[z][c] / dvec2) . vdot[z], with g = g_out *
+ *                     phi'(aux) of `nonlin` (aux nullable = plain g_out) for the PQ route and g = g_e0 for the other
+ *   ab2_zbl_hvp:      gvec_dot[z] += (d2 Ez[z] / dvec2) . vdot[z] of ab2_zbl (same arguments)
+ * Beyond r_max the radial and ZBL terms are exactly zero, as in the primal kernels. */
+int ab2_sh_jvp(int acc_dtype, int lmax, int64_t E, const void* vec, const void* vdot, void* Yd, void* stream);
+int ab2_sh_hvp(int acc_dtype, int lmax, int64_t E, const void* vec, const void* vdot, const void* gY, void* gvec_dot, void* stream);
+int ab2_act_bwd_jvp(int dtype, int64_t n, const void* ga_dot, const void* ga, const void* pre, const void* pre_dot, void* out, int nonlin,
+                    void* stream);
+int ab2_radial_pq_jvp(int dtype, int64_t E, int S, int num_bessels, double p_cut, const void* vec, const void* vdot, const int32_t* ctr,
+                      const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types, const void* bessel_w, const void* PQ,
+                      void* out, void* stream);
+int ab2_radial_jvp(int dtype, int64_t E, int S_rc, int num_bessels, double p_cut, const void* vec, const void* vdot, const int32_t* ctr,
+                   const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types, const void* bessel_w, const void* Wb,
+                   const void* center_embed, const void* neighbor_embed, void* e0_dot, void* stream);
+int ab2_radial_pq_hvp(int dtype, int64_t E, int S, int num_bessels, double p_cut, const void* vec, const void* vdot, const int32_t* ctr,
+                      const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types, const void* bessel_w, const void* PQ,
+                      const void* g_out, const void* aux, void* gvec_dot, int nonlin, void* stream);
+int ab2_radial_hvp(int dtype, int64_t E, int S_rc, int num_bessels, double p_cut, const void* vec, const void* vdot, const int32_t* ctr,
+                   const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types, const void* bessel_w, const void* Wb,
+                   const void* center_embed, const void* neighbor_embed, const void* g_e0, void* gvec_dot, void* stream);
+int ab2_zbl_hvp(int acc_dtype, int64_t E, int num_types, double p_cut, double qq, const void* vec, const void* vdot, const int32_t* ctr,
+                const int32_t* nbr, const int32_t* types, const void* Z, const void* rmax_table, void* gvec_dot, void* stream);
+/* Tangent mode of ab2_fc_gather / ab2_fc_fold (phonons.analytic_force_constants): each unit u = (a, alpha) is ONE job of
+ * m_a centres and E_a edges, from centre Cp[u] - Cp[u0] and edge Ep[u] - Ep[u0] (Cb = Cp[u0+U] - Cp[u0]).  The gather
+ * writes the undisplaced vec_b (the operations of ab2_edge_vec) and vdot_b[zb] = e_alpha ([nbr[z] = j] - [k = j]); the
+ * fold writes blocks[p][alpha][beta] = -F_dot_{i,beta} from the jobs' gradient tangents gvec_dot, F_dot as F in
+ * ab2_fc_fold (same fixed order, no atomics). */
+int ab2_fc_gather_tangent(int pos_dtype, int acc_dtype, int64_t u0, int64_t U, int64_t Cb, const void* pos, const void* shift,
+                          const int64_t* atoms, const int64_t* cptr, const int32_t* cen, const int32_t* coff, const int64_t* ea,
+                          const int32_t* row_ptr, const int32_t* nbr, const int64_t* Cp, const int64_t* Ep, int32_t* row_ptr_b,
+                          int32_t* cen_b, int32_t* ctr_b, int32_t* nbr_b, void* vec_b, void* vdot_b, void* stream);
+int ab2_fc_fold_tangent(int acc_dtype, int64_t u0, int64_t U, const int64_t* cptr, const int32_t* cen, const int32_t* coff,
+                        const int64_t* ea, const int32_t* row_ptr, const int32_t* ctr, const int32_t* col_ptr, const int32_t* col_perm,
+                        const int64_t* fptr, const int32_t* col, const int64_t* Ep, const void* gvec_dot, double* blocks, void* stream);
+
 /* ---- ghost-atom halo exchange over NVLink peer memory (SURVEY section 8e) ------------------- */
 
 /* One mailbox per rank (cudaMalloc'ed here so that it can be exported through CUDA IPC), mapped by its peers.
