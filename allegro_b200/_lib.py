@@ -64,6 +64,8 @@ _SIGNATURES = {
     "ab2_radial_pq_fwd": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_radial_pq_bwd": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_radial_pq_bwd_nl": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32], C.c_int),
+    "ab2_radial_pq_bwd_gemm": ([_i32, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp,
+                                _i32], C.c_int),
     "ab2_zbl": ([_i32, _i64, _i32, _dbl, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_p2p_mailbox_bytes": ([_i32, _i32], C.c_int64),
     "ab2_p2p_alloc": ([_i64, C.POINTER(C.c_void_p)], C.c_int),
@@ -885,14 +887,47 @@ def radial_pq_fwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table,
     return out
 
 
-def radial_pq_bwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table, bessel_w, PQ, g_out, aux, gvec, nonlin: int = NL_SILU):
-    """gvec += (d out / d vec)^T (g_out * phi'(aux)) (aux None: plain g_out); phi the nonlinearity ``nonlin`` (NL_*)."""
+def radial_pq_bwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table, bessel_w, PQ, g_out, aux, gvec, nonlin: int = NL_SILU,
+                  gemm: Optional[Tuple[Sequence[torch.Tensor], Optional[torch.Tensor]]] = None) -> bool:
+    """gvec += (d out / d vec)^T (g_out * phi'(aux)) (aux None: plain g_out); phi the nonlinearity ``nonlin`` (NL_*).
+
+    ``gemm = (gout_segs, W2T_packed)`` with ``g_out = None``: g_out is the product cat(gout_segs, -1) @ W2^T (W2T_packed from
+    ``linear_pack``), and aux the ab2_radial_pq_fwd output h of these edges.  Then one kernel (ab2_radial_pq_bwd_gemm) forms
+    the product and applies the adjoint to it, h recomputed: neither is stored.  Returns False, with nothing computed,
+    when that kernel does not take the case; the caller then forms g_out and calls again without ``gemm``."""
     E = ctr.shape[0]
+    if gemm is not None:
+        gout_segs, W2T_packed = gemm
+        assert g_out is None and aux is not None and tuple(aux.shape) == (E, S)
+        if W2T_packed is None:
+            return False
+        na = len(gout_segs)
+        a_ptr = (C.c_void_p * na)()
+        a_ld = (C.c_int64 * na)()
+        a_w = (C.c_int32 * na)()
+        for s, t in enumerate(gout_segs):
+            t, ld = _row_strided(t, f"A segment {s}")
+            assert t.dtype == dtype and t.shape[0] == E
+            a_ptr[s], a_ld[s], a_w[s] = t.data_ptr(), ld, t.shape[1]
+            _ptr(t)
+        K = sum(int(w) for w in a_w)
+        timer = _timed("radial_pq_bwd_gemm")
+        args = (DTYPE_ENUM[dtype], E, K, S, na, a_ptr, a_ld, a_w, _ptr(W2T_packed), bessel_w.numel(), float(p_cut), _ptr(_contig(vec, "vec")),
+                _ptr(ctr), _ptr(nbr), _ptr(types), _ptr(rmax_table), rmax_table.shape[0], _ptr(bessel_w), _ptr(_contig(PQ, "PQ")),
+                _ptr(_contig(gvec, "gvec")), _stream(), int(nonlin))
+        with timer:
+            rc = load().ab2_radial_pq_bwd_gemm(*args)
+        if rc == NOT_ELIGIBLE:
+            timer.cancel()
+            return False
+        _check(rc)
+        return True
     args = (DTYPE_ENUM[dtype], E, S, bessel_w.numel(), float(p_cut), _ptr(vec), _ptr(ctr), _ptr(nbr), _ptr(types), _ptr(rmax_table),
             rmax_table.shape[0], _ptr(bessel_w), _ptr(_contig(PQ, "PQ")), _ptr(_contig(g_out, "g_out")),
             _ptr(_contig(aux, "aux")) if aux is not None else None, _ptr(gvec), _stream())
     with _timed("radial_bwd"):
         _check(load().ab2_radial_pq_bwd(*args) if nonlin == NL_SILU else load().ab2_radial_pq_bwd_nl(*args, nonlin))
+    return True
 
 
 # --------------------------------------------------------------------------- #

@@ -27,6 +27,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "radial_basis.cuh"
 
 extern int g_ab2_opt_linear_tc;
 extern int g_ab2_opt_linear_tma;
@@ -1005,6 +1006,167 @@ __global__ void __launch_bounds__(NTHREADS, 1) linear_tma_kernel(const TcParams 
 }
 
 // =========================================================================================
+// Hidden-layer gradient GEMM of the scalar-embed MLP and the radial adjoint in one kernel (ab2_radial_pq_bwd_gemm).  With
+// the radial embedding folded into that MLP's first layer (radial.cu, PQ form) its pre-activation is
+// h[z][c] = sum_n B_n(x_z) PQ[pair_z][n][c], and its backward ends in
+//   g_h = Gout @ W2^T                                                                     (ab2_linear, N = H)
+//   gvec[z] += sum_c g_h[z][c] phi'(h[z][c]) sum_n dB_n(x_z) PQ[pair_z][n][c] * r_vec / (r_max |r|)   (radial_pq_bwd_kernel)
+// Here the GEMM is that of linear_tma_kernel (converter warps, ring and main loop as they are) and the accumulator goes
+// into the adjoint instead of to HBM.  Each consumer thread holds rows r8 and r8 + 8 of its warp's 16, 16 columns of each
+// (fragment layout at wgmma_bf16), and per tile
+//   - reads vec and the type pair of both rows (ctr / nbr one tile ahead, so the types gather does not wait on them);
+//   - evaluates the radial basis, two of the eight functions per lane of the quad, shared by shuffles;
+//   - recomputes its h columns with the fmaf chain of radial_pq_fwd_kernel (n order), so phi'(h) is that of the stored h;
+//   - sums g_h phi'(h) sum_n dB_n PQ over its columns in the arithmetic of radial_pq_bwd_kernel, and the quad's four
+//     partial sums with two xor shuffles;
+//   - lane 0 of the quad, the only writer of the row, adds the row's gvec: no atomics, the result does not depend on
+//     the launch.
+// Neither g_h nor h reaches HBM.  PQ of every type pair (T^2 x 8 x H floats) is staged in the epilogue staging area,
+// which this kernel does not otherwise use.
+// =========================================================================================
+constexpr int RADJ_NB = 8;  // Bessel functions of the PQ form
+
+struct RadialAdjParams {
+    const float* vec;         // [M][3]
+    const int32_t* ctr;       // [M]
+    const int32_t* nbr;       // [M]
+    const int32_t* types;     // per atom
+    const float* rmax_table;  // [T][T]
+    const float* bw;          // [RADJ_NB] Bessel weights
+    const float* PQ;          // [T * T][RADJ_NB][H]
+    float* gvec;              // [M][3], accumulated into
+    int num_types;
+    float p;                  // polynomial cutoff order
+};
+
+template <int NCH, int NL>
+__device__ __forceinline__ void radial_adjoint_consumer_role(const TcParams& p, const TcCtx& c, const RadialAdjParams& ra, const float* sPQ, int cw,
+                                                             int lane) {
+    constexpr int H = 32 * NCH;
+    const int wg = cw >> 2, w4 = cw & 3;
+    const int r8 = lane >> 2, cq = 2 * (lane & 3);
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[16 * NCH];
+    // row i (0, 1) of this thread in a tile, clamped to the last edge: rows beyond M read valid data and write nothing
+    auto row = [&](int64_t tile, int i) {
+        const int64_t m = tile * BM + wg * 64 + w4 * 16 + r8 + 8 * i;
+        return m < p.M ? m : p.M - 1;
+    };
+    int nc[2], nn[2];  // centre and neighbour of the rows of the next tile
+    auto fetch_idx = [&](int64_t tile) {
+        if (tile < p.num_tiles) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                nc[i] = __ldg(ra.ctr + row(tile, i));
+                nn[i] = __ldg(ra.nbr + row(tile, i));
+            }
+        }
+    };
+    fetch_idx(blockIdx.x);
+    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        int pair[2];
+        float v[2][3];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            pair[i] = __ldg(ra.types + nc[i]) * ra.num_types + __ldg(ra.types + nn[i]);
+            const float* vr = ra.vec + row(tile, i) * 3;
+            v[i][0] = __ldg(vr); v[i][1] = __ldg(vr + 1); v[i][2] = __ldg(vr + 2);
+        }
+        fetch_idx(tile + gridDim.x);
+        tc_mma_ring<true, NCH>(acc, p, c, wg, lane, stage, phase);  // acc = g_h of this thread's fragment
+        float f[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const float r = sqrtf(v[i][0] * v[i][0] + v[i][1] * v[i][1] + v[i][2] * v[i][2]);
+            const float rmax = __ldg(ra.rmax_table + pair[i]);
+            float Bq[2], dBq[2];
+            bessel_basis<float, true>(r / rmax, ra.p, 2, ra.bw + cq, Bq, dBq);  // functions cq, cq + 1
+            float B[RADJ_NB], dB[RADJ_NB];
+#pragma unroll
+            for (int n = 0; n < RADJ_NB; ++n) {
+                B[n] = __shfl_sync(0xffffffffu, Bq[n & 1], (lane & ~3) | (n >> 1));
+                dB[n] = __shfl_sync(0xffffffffu, dBq[n & 1], (lane & ~3) | (n >> 1));
+            }
+            const float* m = sPQ + pair[i] * RADJ_NB * H + cq;
+            float gx = 0.f;
+#pragma unroll
+            for (int j = 0; j < 4 * NCH; ++j) {  // columns 8 j + cq, 8 j + cq + 1
+                float2 pq[RADJ_NB];
+#pragma unroll
+                for (int n = 0; n < RADJ_NB; ++n) pq[n] = *reinterpret_cast<const float2*>(m + n * H + 8 * j);
+                float h0 = 0.f, h1 = 0.f, s0 = 0.f, s1 = 0.f;
+#pragma unroll
+                for (int n = 0; n < RADJ_NB; ++n) {
+                    h0 = fmaf(B[n], pq[n].x, h0);
+                    h1 = fmaf(B[n], pq[n].y, h1);
+                    s0 = fmaf(dB[n], pq[n].x, s0);
+                    s1 = fmaf(dB[n], pq[n].y, s1);
+                }
+                gx = fmaf(acc[4 * j + 2 * i] * dact_f<NL>(h0), s0, gx);
+                gx = fmaf(acc[4 * j + 2 * i + 1] * dact_f<NL>(h1), s1, gx);
+            }
+            gx += __shfl_xor_sync(0xffffffffu, gx, 1);
+            gx += __shfl_xor_sync(0xffffffffu, gx, 2);
+            f[i] = gx / (rmax * r);  // dx/dr_vec = r_vec / (|r| r_max)
+        }
+        if ((lane & 3) == 0) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int64_t m = tile * BM + wg * 64 + w4 * 16 + r8 + 8 * i;
+                if (m < p.M) {
+                    float* g = ra.gvec + m * 3;
+                    g[0] += f[i] * v[i][0];
+                    g[1] += f[i] * v[i][1];
+                    g[2] += f[i] * v[i][2];
+                }
+            }
+        }
+    }
+}
+
+template <int G, int NCH, int NL>
+__global__ void __launch_bounds__(NTHREADS, 1) radial_adjoint_tma_kernel(const TcParams p, const __grid_constant__ TmaMaps maps, int NR,
+                                                                         const RadialAdjParams ra) {
+    constexpr int WPG = NPROD / G;  // warps per converter group
+    extern __shared__ __align__(1024) uint8_t smem[];
+    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;  // warp-uniform role index
+    const int w_half = p.Npad * p.K * 2;
+    const int w_bytes = 2 * w_half;
+    const int stage_bytes = 2 * STAGE_HALF;
+    // the plan of linear_tma_kernel without silu' multiplier (one box per raw slot); PQ in the epilogue staging area
+    uint8_t* sRaw = smem + ((1024u - (smem_u32(smem) & 1023u)) & 1023u);
+    uint8_t* sW = sRaw + (size_t)NR * TMA_BOX_BYTES;
+    uint8_t* sA = sW + ((w_bytes + 127) & ~127);
+    float* sPQ = reinterpret_cast<float*>(sA + p.nstage * stage_bytes);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sPQ) + EPI_BYTES);
+    int4* sKseg = reinterpret_cast<int4*>(reinterpret_cast<uint8_t*>(bars) + TAIL_BARS + TAIL_CHUNK);
+    uint64_t* rbars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sKseg) + (MAX_K / 32) * 16);  // raw_full[8]
+    const uint32_t bar0 = smem_u32(bars), rbar0 = smem_u32(rbars);
+    const int nkb = p.K / KC;
+
+    // ---- one-time setup ----
+    if (threadIdx.x == 0) tma_init_bars(bar0, rbar0, WPG);
+    if (threadIdx.x < MAX_K / 32) sKseg[threadIdx.x] = tma_kseg_entry(p, threadIdx.x);
+    const int n_pq = ra.num_types * ra.num_types * RADJ_NB * 32 * NCH;
+    for (int e = threadIdx.x; e < n_pq; e += NTHREADS) sPQ[e] = __ldg(ra.PQ + e);
+    stage_w(sW, p.Wpacked, p.Wlo, w_half);
+    fence_proxy_async();
+    __syncthreads();
+    TcCtx ctx;
+    ctx.sW = sW; ctx.sA = sA; ctx.sEpi = sPQ; ctx.sChunk = nullptr; ctx.bar0 = bar0;
+    ctx.nkb = nkb; ctx.stage_bytes = stage_bytes; ctx.w_half = w_half;
+    const int64_t my_tiles = (p.num_tiles > blockIdx.x) ? (p.num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+
+    if (warp >= NPROD) {
+        radial_adjoint_consumer_role<NCH, NL>(p, ctx, ra, sPQ, warp - NPROD, lane);
+    } else {
+        // the ring carries Gout as it is (p.act == AB2_ACT_NONE): the converters take no nonlinearity
+        tma_converter_role<G, AB2_NL_SILU>(p, maps, NR, ctx, sRaw, sKseg, rbar0, my_tiles * nkb, warp, lane);
+    }
+}
+
+// =========================================================================================
 // Two-layer SiLU MLP in one kernel (ab2_mlp2).  Stage 1 is the TMA-fed GEMM of linear_tma_kernel (A @ W1, converter
 // warps unchanged); stage 2 multiplies the hidden layer, kept on chip, by W2.  Per 128-row tile each consumer warpgroup,
 // for its own 64 rows:
@@ -1895,6 +2057,81 @@ extern "C" int ab2_mlp2(int dtype, int backward, int64_t M, int K, int H, int N,
                         void* const* o_ptr, const int64_t* o_ld, const int32_t* o_width, const int32_t* o_accum, void* stream) {
     return ab2_mlp2_nl(dtype, backward, M, K, H, N, n_a, a_ptr, a_ld, a_width, W1_packed, W2_packed, w1_row, pre, pre_ld, n_o, o_ptr, o_ld, o_width,
                        o_accum, stream, AB2_NL_SILU);
+}
+
+// Gradient GEMM of the scalar-embed MLP + radial adjoint (radial_adjoint_tma_kernel); contract in include/allegro_b200.h.
+// Returns AB2_NOT_ELIGIBLE, with nothing enqueued and no error set, for a case the kernel does not take: the caller then
+// runs ab2_linear and ab2_radial_pq_bwd_nl.
+extern "C" int ab2_radial_pq_bwd_gemm(int dtype, int64_t M, int K, int H, int n_a, const void* const* a_ptr, const int64_t* a_ld,
+                                      const int32_t* a_width, const void* W_packed, int num_bessels, double p_cut, const void* vec,
+                                      const int32_t* ctr, const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types,
+                                      const void* bessel_w, const void* PQ, void* gvec, void* stream, int nonlin) {
+    AB2_CHECK_ARG(nonlin == AB2_NL_SILU || nonlin == AB2_NL_MISH || nonlin == AB2_NL_GELU, "nonlinearity");
+    AB2_CHECK_ARG(M >= 0, "shape");
+    if (M == 0) return 0;  // (empty operands may come with null pointers)
+    AB2_CHECK_ARG(n_a >= 1 && n_a <= AB2_MAX_SEG, "segment count");
+    AB2_CHECK_ARG(K > 0 && H > 0 && num_types > 0, "shape");
+    int ks = 0;
+    for (int s = 0; s < n_a; ++s) {
+        AB2_CHECK_ARG(a_ptr[s] && a_width[s] > 0 && a_ld[s] >= a_width[s], "A segment");
+        ks += a_width[s];
+    }
+    AB2_CHECK_ARG(ks == K, "A segment widths must sum to K");
+    AB2_CHECK_ARG(vec && ctr && nbr && types && rmax_table && bessel_w && PQ && gvec, "null pointer");
+    // ---- eligibility ----
+    auto al16 = [](const void* ptr, int64_t ld) { return (reinterpret_cast<uintptr_t>(ptr) % 16) == 0 && (ld * 4) % 16 == 0; };
+    if (dtype != AB2_F32 || !g_ab2_opt_linear_tc || !g_ab2_opt_linear_tma || !tc_encode_fn()) return AB2_NOT_ELIGIBLE;
+    if (num_bessels != RADJ_NB || (H != 32 && H != 64) || !W_packed || K % KC != 0 || K > MAX_K || M >= ((int64_t)1 << 31))
+        return AB2_NOT_ELIGIBLE;
+    if ((size_t)num_types * num_types * RADJ_NB * H * 4 > (size_t)EPI_BYTES) return AB2_NOT_ELIGIBLE;  // PQ in the staging area
+    for (int s = 0; s < n_a; ++s)
+        if (a_width[s] % KC != 0 || !al16(a_ptr[s], a_ld[s])) return AB2_NOT_ELIGIBLE;
+    // shared-memory plan of linear_tma_kernel with four converter groups: deepest {NR raw slots, cn canonical stages}
+    int num_sms = 0, max_smem = 0;
+    tc_device_limits(num_sms, max_smem);
+    const int w_bytes = 2 * H * K * 2;
+    const int plans[2][2] = {{8, 4}, {4, 4}};  // {NR, cn}
+    int NR = 0, nstage = 0;
+    size_t smem = 0;
+    for (int q = 0; q < 2 && !NR; ++q) {
+        const size_t need = 1024 + ((w_bytes + 127) & ~127) + (size_t)plans[q][1] * 2 * STAGE_HALF + EPI_BYTES + TAIL_BYTES +
+                            (size_t)plans[q][0] * TMA_BOX_BYTES;
+        if (need <= (size_t)max_smem) { NR = plans[q][0]; nstage = plans[q][1]; smem = need; }
+    }
+    if (!NR) return AB2_NOT_ELIGIBLE;
+
+    TcParams p;
+    memset(&p, 0, sizeof(p));
+    p.M = M; p.K = K; p.N = H; p.Npad = H; p.n_a = n_a; p.act = AB2_ACT_NONE; p.epi = AB2_EPI_NONE;
+    p.Wpacked = W_packed; p.Wlo = reinterpret_cast<const uint8_t*>(W_packed) + (size_t)H * K * 2;
+    p.num_tiles = (M + BM - 1) / BM; p.nstage = nstage; p.debug = g_ab2_opt_tc_debug;
+    TmaMaps maps;
+    memset(&maps, 0, sizeof(maps));
+    for (int s = 0; s < n_a; ++s) {
+        p.a[s].ptr = a_ptr[s]; p.a[s].ld = a_ld[s]; p.a[s].width = a_width[s];
+        if (!tc_make_map(&maps.a[s], a_ptr[s], a_ld[s], a_width[s], M)) return AB2_NOT_ELIGIBLE;
+    }
+    RadialAdjParams ra;
+    ra.vec = reinterpret_cast<const float*>(vec); ra.ctr = ctr; ra.nbr = nbr; ra.types = types;
+    ra.rmax_table = reinterpret_cast<const float*>(rmax_table); ra.bw = reinterpret_cast<const float*>(bessel_w);
+    ra.PQ = reinterpret_cast<const float*>(PQ); ra.gvec = reinterpret_cast<float*>(gvec);
+    ra.num_types = num_types; ra.p = (float)p_cut;
+
+    const unsigned grid = (unsigned)((p.num_tiles < num_sms) ? p.num_tiles : num_sms);
+    cudaStream_t st = (cudaStream_t)stream;
+    auto go = [&](auto kern) -> int {
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+            cudaGetLastError();
+            return AB2_NOT_ELIGIBLE;
+        }
+        kern<<<grid, NTHREADS, smem, st>>>(p, maps, NR, ra);
+        AB2_CUDA_LAUNCH_CHECK();
+        return 0;
+    };
+    return tc_with_nl(nonlin, [&](auto nl) -> int {
+        constexpr int NL = decltype(nl)::value;
+        return H == 32 ? go(radial_adjoint_tma_kernel<4, 1, NL>) : go(radial_adjoint_tma_kernel<4, 2, NL>);
+    });
 }
 
 // Last latent MLP + readout MLP (mlp2_readout_fwd_kernel / mlp2_readout_bwd_kernel); contract in include/allegro_b200.h.

@@ -374,6 +374,8 @@ class UpstreamPack:
         self.fold = fold_embed_of is not None
         self.mlp = PackedMLP(scalar_embed_mlp, dtype, device, post=fold_embed_of.embed.W64[0] if self.fold else None)
         self.dtype = dtype
+        # route of the last pq_fold backward: "fused" (ab2_radial_pq_bwd_gemm) or "two_launch" (hidden_grad + radial_pq_bwd)
+        self.bwd_path: Optional[str] = None
         self.S_rc = radial.out_dim
         self.kind = "spline" if hasattr(radial, "spline") else "bessel"
         if self.kind == "spline":
@@ -445,6 +447,15 @@ class UpstreamPack:
         dt = self.dtype
         E = vec.shape[0]
         if kind == "pq_fold":
+            # One kernel where it takes the case: the hidden-gradient GEMM with the radial adjoint as its epilogue, so g_h
+            # and h never reach memory.  fp32 storage, hidden width 32 or 64, a packed W2^T image; the entry itself declines
+            # the rest (segment layout, PQ beyond the shared-memory budget), and then the two launches below run.
+            if dt == torch.float32 and self.S_pq in (32, 64) and self.mlp.WTp[1] is not None and _lib.radial_pq_bwd(
+                    dt, self.S_pq, self.p, vec, csr.ctr, csr.nbr, types_i32, self.rmax_table, self.bessel_w, self.PQ, None, pre[0], gvec,
+                    gemm=(gouts, self.mlp.WTp[1]), **self.mlp.nl_kw):
+                self.bwd_path = "fused"
+                return
+            self.bwd_path = "two_launch"
             g_h = self.mlp.hidden_grad(gouts)  # gradient w.r.t. phi(h); phi'(h) is applied by the radial adjoint (aux = h)
             _lib.radial_pq_bwd(dt, self.S_pq, self.p, vec, csr.ctr, csr.nbr, types_i32, self.rmax_table, self.bessel_w, self.PQ, g_h, pre[0], gvec,
                                **self.mlp.nl_kw)

@@ -595,6 +595,23 @@ int ab2_radial_pq_bwd_nl(int dtype, int64_t E, int S, int num_bessels, double p_
                          const int32_t* ctr, const int32_t* nbr, const int32_t* types, const void* rmax_table,
                          int num_types, const void* bessel_w, const void* PQ, const void* g_out, const void* aux,
                          void* gvec, void* stream, int nonlin);
+/* The end of the scalar-embed MLP's backward when its first layer is folded into PQ (H = PQ's width, the hidden width),
+ * in one tensor-core kernel: with Gout = [A_0 | A_1 | ...] [M][K] (A segments as in ab2_linear) and W2T_packed the packed
+ * image (ab2_linear_pack) of the MLP's transposed last layer W2^T [K][H],
+ *   g_h = Gout @ W2^T,   h[z][c] = sum_n B_n(x_z) PQ[pair_z][n][c]   (the ab2_radial_pq_fwd output),
+ *   gvec[z] += (d h / d vec)^T (g_h * phi'(h))
+ * which is ab2_linear followed by ab2_radial_pq_bwd_nl(g_out = g_h, aux = h), without g_h or h in memory.  h is
+ * recomputed with the forward's arithmetic; the sum over columns runs in another order, so gvec differs from the two
+ * calls' in the last bits.  Each row of gvec is written by one thread, no atomics: the result is reproducible.
+ * Returns AB2_NOT_ELIGIBLE (nothing enqueued, no error set) for dtype other than AB2_F32, num_bessels other than 8, H
+ * other than 32 or 64, A segments not multiples of 32 columns or not 16-byte aligned, PQ above 20 KB (T^2 8 H floats),
+ * or a shared-memory plan that does not fit one SM.  The caller then makes the two calls.  Returns 1 (and sets
+ * ab2_last_error) for an unknown nonlin. */
+int ab2_radial_pq_bwd_gemm(int dtype, int64_t M, int K, int H, int n_a, const void* const* a_ptr_host,
+                           const int64_t* a_ld_host, const int32_t* a_width_host, const void* W2T_packed, int num_bessels,
+                           double p_cut, const void* vec, const int32_t* ctr, const int32_t* nbr, const int32_t* types,
+                           const void* rmax_table, int num_types, const void* bessel_w, const void* PQ, void* gvec,
+                           void* stream, int nonlin);
 
 /* ZBL pair term (reference call site allegro/model/allegro_models.py:270-288; the module is nequip's
  * nequip.nn.pair_potential.ZBL = LAMMPS pair_style zbl, constants of pair_zbl_const.h):
