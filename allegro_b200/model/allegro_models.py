@@ -151,11 +151,8 @@ class FusedAllegroEnergy(torch.nn.Module):
         if self._core is None or self._core_key != key:
             self._core = AllegroCore(self.tensor_embed, self.allegro, self.edge_readout, self.avg_num_neighbors,
                                      self.model_dtype, dev)
-            import os
-
-            fold = self._core if os.environ.get("ALLEGRO_B200_FOLD_EMBED", "1") == "1" else None  # default on: one GEMM less per direction
             self._upstream = UpstreamPack(self.edge_norm, self.radial_chemical_embed, self.scalar_embed_mlp, self.model_dtype, dev,
-                                          fold_embed_of=fold)
+                                          self._core)
             self._core_key = key
         return self._core
 

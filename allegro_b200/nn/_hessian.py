@@ -144,16 +144,10 @@ def edge_energy_grad_tangent(core, up, csr: EdgeCSR, vec: torch.Tensor, vdot: to
 
     # ---- (a) primal forward (stored-V path) ---------------------------------------------------------------------
     _lib.set_tag("hvp.fwd")
-    if up.fold:
-        box = []
-        _, _, _, sv = core.forward(csr, vec, None, fill_embed=lambda w0, x0, om0: box.append(up.forward(vec, csr, types_i32, [w0, x0, om0])),
-                                   stored_v=True)
-        up_saved = box[0]
-    else:
-        x_emb = empty(E, core.S_in)
-        up_saved = up.forward(vec, csr, types_i32, [x_emb])
-        _, _, _, sv = core.forward(csr, vec, x_emb, stored_v=True)
-    kind, sp_saved, up_pre = up_saved
+    box = []
+    _, _, _, sv = core.forward(csr, vec, None, fill_embed=lambda w0, x0, om0: box.append(up.forward(vec, csr, types_i32, [w0, x0, om0])),
+                               stored_v=True)
+    kind, sp_saved, up_pre = box[0]
     k0_up = 1 if kind == "pq_fold" else 0
 
     # ---- (a) primal backward, keeping the adjoints ----------------------------------------------------------------
@@ -185,16 +179,9 @@ def edge_energy_grad_tangent(core, up, csr: EdgeCSR, vec: torch.Tensor, vdot: to
         gom[l] = empty(E, nw)
         _lib.env_bwd(dt, lmax, U, ctr, sv.Y, sv.omega[l], ggam[l], sf, gom[l], gY, row_ptr=row_ptr)
     g_emb = [gw0, gX[:, :S], gom[0]]
-    ga_emb: Dict[int, torch.Tensor] = {}
-    if up.fold:
-        g_up_out = g_emb
-    else:
-        g_xemb = empty(E, core.S_in)
-        _mlp_bwd(core.embed, [], 0, g_emb, [g_xemb], [False])
-        g_up_out = [g_xemb]
     gvec = _lib.sh_bwd(vec, gY, lmax)
     g_r = empty(E, up.mlp.dims[k0_up])  # gradient w.r.t. the radial output (pq_fold: w.r.t. phi(h))
-    ga_up = _mlp_bwd(up.mlp, up_pre, k0_up, g_up_out, [g_r], [False])
+    ga_up = _mlp_bwd(up.mlp, up_pre, k0_up, g_emb, [g_r], [False])
     _radial_bwd(up, kind, sp_saved, up_pre, vec, csr, types_i32, g_r, gvec)
     if pair is not None:
         pair[0].edge_energy_and_grad(vec, csr, types_i32, pair[1], gvec)
@@ -206,12 +193,7 @@ def edge_energy_grad_tangent(core, up, csr: EdgeCSR, vec: torch.Tensor, vdot: to
     w0d, omd = empty(E, nw), [empty(E, nw)]
     emb_outs = [w0d, Xd[:, :S], omd[0]]
     rd = _radial_jvp(up, kind, vec, vdot, csr, types_i32)
-    if up.fold:
-        pd_up = _mlp_tangent(up.mlp, up_pre, k0_up, [rd], emb_outs)
-    else:
-        xd_emb = empty(E, core.S_in)
-        pd_up = _mlp_tangent(up.mlp, up_pre, k0_up, [rd], [xd_emb])
-        _mlp_tangent(core.embed, [], 0, [xd_emb], emb_outs)
+    pd_up = _mlp_tangent(up.mlp, up_pre, k0_up, [rd], emb_outs)
     Vd: List[Optional[torch.Tensor]] = [None] * (L + 1)
     gamd: List[torch.Tensor] = []
     pd_lat = []
@@ -278,16 +260,10 @@ def edge_energy_grad_tangent(core, up, csr: EdgeCSR, vec: torch.Tensor, vdot: to
         _lib.env_bwd(dt, lmax, U, ctr, sv.Y, sv.omega[l], ggd_l, sf, go[1], gYd, row_ptr=row_ptr)
         gomd[l] = go[0] + go[1]
     g_emb_d = [gw0d, gXd[:, :S], gomd[0]]
-    if up.fold:
-        g_up_out_d = g_emb_d
-    else:
-        gxd = zeros(E, core.S_in)
-        _mlp_bwd_tangent(core.embed, [], {}, ga_emb, 0, g_emb_d, [gxd])
-        g_up_out_d = [gxd]
     gvec_dot = _lib.sh_bwd(vec, gYd, lmax)
     _lib.sh_hvp(vec, vdot, gY, lmax, gvec_dot)
     g_rd = zeros(E, up.mlp.dims[k0_up])
-    _mlp_bwd_tangent(up.mlp, up_pre, pd_up, ga_up, k0_up, g_up_out_d, [g_rd])
+    _mlp_bwd_tangent(up.mlp, up_pre, pd_up, ga_up, k0_up, g_emb_d, [g_rd])
     _radial_bwd_tangent(up, kind, sp_saved, up_pre, pd_up, vec, vdot, csr, types_i32, g_r, g_rd, gvec_dot)
     if pair is not None:
         zbl = pair[0]

@@ -118,37 +118,13 @@ class AllegroCore:
             W1r = self.readout.W[0]
             self.ro_fwd_p = [last.Wp[0], last.Wp[1], _lib.linear_pack(W1r[:P].contiguous()), _lib.linear_pack(W1r[P:].contiguous())]
             self.ro_bwd_p = [self.readout.WTp[0], last.WTp[1], last.WTp[0]]
-        # "plain GEMM" backward plan (all latent/readout MLPs are 2-layer with one nonlinearity): the gradient of the
-        # densenet block x_b is ONE GEMM over all its consumers (readout, latents m >= b), concatenated
-        # along K, each consumer's g_h scaled by phi'(pre) in the GEMM prologue -- no accumulation.  That GEMM applies one
-        # phi' to all its segments, so every latent MLP must share the readout's nonlinearity.
-        import os as _os
-
-        # the epilogue/accumulate plan is the default, this one is opt-in (ALLEGRO_B200_PLAIN_BWD=1); both are covered
-        # by the GPU tests.
-        self.plain_ok = (_os.environ.get("ALLEGRO_B200_PLAIN_BWD", "0") == "1" and self.readout.is_two_layer_nonlinear
-                         and all(ly["mlp"].is_two_layer_nonlinear and ly["mlp"].nonlinearity == self.readout.nonlinearity
-                                 for ly in self.layers))
-        if self.plain_ok:
-            L = self.L
-            self.gxW, self.gxWp, self.gsW, self.gsWp = [], [], [], []
-            for b in range(L + 1):
-                blocks = [self.readout.WT[0][:, S * b : S * (b + 1)]]
-                blocks += [self.layers[mm]["mlp"].WT[0][:, S * b : S * (b + 1)] for mm in range(L - 1, b - 1, -1) if mm >= b]
-                Wg = torch.cat(blocks, dim=0).contiguous()
-                self.gxW.append(Wg)
-                self.gxWp.append(_lib.linear_pack(Wg))
-            for l in range(L):
-                Ws = self.layers[l]["mlp"].WT[0][:, S * (l + 1) : S * (l + 1) + U].contiguous()
-                self.gsW.append(Ws)
-                self.gsWp.append(_lib.linear_pack(Ws))
         # the two tensor products composed per centre (ab2_tp_chain_*, DESIGN.md section 4.1): a two-layer l_max = 2
-        # model whose tables have the baked structure, default backward, and (tp_chain_plan) fp32 with U = 32 or 64.
+        # model whose tables have the baked structure, and (tp_chain_plan) fp32 with U = 32 or 64.
         # Then the forward keeps the compact scalars s_1, s_2 instead of V_1, and the backward passes the compact
         # gradients g1, g2 instead of gV_1.
         self.chain = None
         l0, l1 = (self.layers + [None, None])[:2]
-        if (self.L == 2 and not self.plain_ok and self.D == 9
+        if (self.L == 2 and self.D == 9
                 and (l0["d_in"], l0["d_out"], l1["d_in"], l1["d_out"]) == (9, 9, 9, 1)
                 and torch.equal(l0["tab"].cpu(), _baked_table(9)) and torch.equal(l1["tab"].cpu(), _baked_table(1))):
             self.chain = _lib.tp_chain_plan(dtype, U, l0["cgw"], l1["cgw"])
@@ -223,74 +199,9 @@ class AllegroCore:
 
     # ------------------------------------------------------------------------------------
     def backward(self, sv: _Saved, gEi: torch.Tensor):
-        """gEi [N] (acc dtype) -> (gvec [E,3] acc dtype, gx_emb [E,S_in] act dtype)."""
-        if self.plain_ok:
-            return self._backward_plain(sv, gEi)
-        return self._backward_legacy(sv, gEi)
-
-    def _backward_plain(self, sv: _Saved, gEi: torch.Tensor):
-        csr = sv.csr
-        E, N, U, S, L, D = csr.num_edges, csr.num_atoms, self.U, self.S, self.L, self.D
-        dt, dev = self.dtype, self.device
-        _lib.set_tag("bwd.readout")
-        gEz = _lib.edge_sum_bwd(gEi.contiguous(), csr.ctr, self.factor).to(dt).view(E, 1)
-        g_h = {"r": self.readout.hidden_grad([gEz])}
-        pre = {"r": sv.pre_read[0]}
-        for l in range(L):
-            pre[l] = sv.pre_lat[l][0]
-        gY = torch.zeros(E, D, dtype=self.acc, device=dev)
-        gV_next: Optional[torch.Tensor] = None
-        gomega_next: Optional[torch.Tensor] = None
-        gw0 = None
-
-        def block_grad(b: int) -> torch.Tensor:
-            cons = ["r"] + [mm for mm in range(L - 1, b - 1, -1) if mm >= b]
-            out = torch.empty(E, S, dtype=dt, device=dev)
-            _lib.linear([g_h[c] for c in cons], self.gxW[b], [out], act=_lib.ACT_MUL_DSILU, a_aux=[pre[c] for c in cons],
-                        W_packed=self.gxWp[b], **self.readout.nl_kw)
-            return out
-
-        for l in range(L - 1, -1, -1):
-            ly = self.layers[l]
-            _lib.set_tag(f"bwd.L{l}")
-            gouts = [block_grad(l + 1)]
-            if not ly["last"]:
-                gouts.append(gomega_next)
-            g_h[l] = ly["mlp"].hidden_grad(gouts)
-            if ly["last"]:
-                gV_next = torch.empty(E, ly["d_out"], U, dtype=dt, device=dev)
-                if ly["d_out"] > 1:
-                    gV_next.zero_()
-                gs_acc = False
-            else:
-                gs_acc = True
-            gs = gV_next.view(E, ly["d_out"] * U)[:, :U]
-            _lib.linear([g_h[l]], self.gsW[l], [gs], o_accum=[gs_acc], act=_lib.ACT_MUL_DSILU, a_aux=[pre[l]], W_packed=self.gsWp[l],
-                        **self.readout.nl_kw)
-            ggamma = torch.empty(N, D, U, dtype=self.acc, device=dev)
-            if l == 0:
-                gw0 = torch.empty(E, self.nw, dtype=dt, device=dev)
-                _lib.tp_bwd(dt, self.lmax, N, E, U, ly["d_in"], ly["d_out"], ly["tab"], ly["cgw"], csr.row_ptr, csr.ctr,
-                            sv.gamma[l], None, sv.Y, sv.w0, gV_next, None, gw0, gY, ggamma)
-                gV_in = None
-            else:
-                gV_in = torch.empty(E, ly["d_in"], U, dtype=dt, device=dev)
-                _lib.tp_bwd(dt, self.lmax, N, E, U, ly["d_in"], ly["d_out"], ly["tab"], ly["cgw"], csr.row_ptr, csr.ctr,
-                            sv.gamma[l], sv.V[l], None, None, gV_next, gV_in, None, None, ggamma)
-            gomega = torch.empty(E, self.nw, dtype=dt, device=dev)
-            _lib.env_bwd(dt, self.lmax, U, csr.ctr, sv.Y, sv.omega[l], ggamma, self.sf, gomega, gY, row_ptr=csr.row_ptr)
-            gV_next, gomega_next = gV_in, gomega
-        _lib.set_tag("bwd.embed")
-        g_x0 = block_grad(0)
-        gvec = _lib.sh_bwd(sv.vec, gY, self.lmax)
-        if sv.fold:  # the caller back-propagates the three embed-output gradients through its folded MLP
-            return gvec, [gw0, g_x0, gomega_next]
-        gx_emb = torch.empty(E, self.S_in, dtype=dt, device=dev)
-        self.embed.backward([gw0, g_x0, gomega_next], [], [gx_emb], [False])
-        return gvec, gx_emb
-
-    def _backward_legacy(self, sv: _Saved, gEi: torch.Tensor):
-        """General MLP depth / nonlinearity: phi' in the GEMM epilogue, gradient accumulation."""
+        """gEi [N] (acc dtype) -> (gvec [E,3] acc dtype, gx_emb [E,S_in] act dtype), or, when the forward ran with
+        ``fill_embed``, (gvec, [gw0, gx_0, gomega_0]): the gradients of the three embed outputs.  phi' is applied in the
+        GEMM epilogues, and the gradients of shared inputs are accumulated."""
         csr = sv.csr
         E, N, U, S, L, D = csr.num_edges, csr.num_atoms, self.U, self.S, self.L, self.D
         dt, dev = self.dtype, self.device
@@ -365,14 +276,13 @@ class UpstreamPack:
     """Device constants of the two-body scalar embedding (edge_norm, radial_chemical_embed,
     scalar_embed_mlp) for ab2_radial_fwd/bwd + the packed scalar-embed MLP."""
 
-    def __init__(self, edge_norm, radial, scalar_embed_mlp, dtype, device, fold_embed_of: Optional["AllegroCore"] = None):
+    def __init__(self, edge_norm, radial, scalar_embed_mlp, dtype, device, core: "AllegroCore"):
         acc = _lib.ACC_DTYPE[dtype]
-        # fold_embed_of: x_emb only feeds two LINEAR maps (tensorembed.py:88-89 env_embed_linear, _allegro.py:251
+        # x_emb only feeds two LINEAR maps of the core (tensorembed.py:88-89 env_embed_linear, _allegro.py:251
         # first_layer_env_embed_projection), and the scalar-embed MLP ends in a linear layer, so their product is
         # one matrix: [w0 | x_0 | omega_0] = silu(h) @ (W_last @ W_embed).  One GEMM and the x_emb round trip less
-        # in each direction.  Default on; ALLEGRO_B200_FOLD_EMBED=0 switches it off.
-        self.fold = fold_embed_of is not None
-        self.mlp = PackedMLP(scalar_embed_mlp, dtype, device, post=fold_embed_of.embed.W64[0] if self.fold else None)
+        # in each direction.
+        self.mlp = PackedMLP(scalar_embed_mlp, dtype, device, post=core.embed.W64[0])
         self.dtype = dtype
         # route of the last pq_fold backward: "fused" (ab2_radial_pq_bwd_gemm) or "two_launch" (hidden_grad + radial_pq_bwd)
         self.bwd_path: Optional[str] = None
@@ -402,15 +312,13 @@ class UpstreamPack:
         # emits the pre-activation h directly (no [E][S_rc] embedding tensor, one GEMM less per direction).
         self.PQ, self.S_pq, self.fold_radial = None, 0, False
         nb = int(self.bessel_w.numel())
-        import os as _os
-
-        if nb == 8 and _os.environ.get("ALLEGRO_B200_RADIAL_PQ", "1") == "1":
+        if nb == 8:
             Wb64 = te.basis_linear.folded_weights()[0].detach().double().cpu()             # [nb, S_rc]
             ce, ne = te.center_embed.weight.detach().double().cpu(), te.neighbor_embed.weight.detach().double().cpu()
             T = ce.shape[0]
             temb = torch.cat([ce.unsqueeze(1).expand(T, T, -1), ne.unsqueeze(0).expand(T, T, -1)], dim=-1)  # [tc, tn, S_rc]
             PQ0 = temb.reshape(T * T, 1, -1) * Wb64.unsqueeze(0)                          # [T*T, nb, S_rc]
-            if self.mlp.is_two_layer_nonlinear and self.mlp.dims[1] <= 128 and _os.environ.get("ALLEGRO_B200_FOLD_RADIAL", "1") == "1":
+            if self.mlp.is_two_layer_nonlinear and self.mlp.dims[1] <= 128:
                 self.fold_radial = True
                 PQ0 = PQ0 @ self.mlp.W64[0]                                                # [T*T, nb, width]
             if PQ0.shape[-1] <= 128:
@@ -421,8 +329,8 @@ class UpstreamPack:
 
     # ---- forward / adjoint of the whole upstream scalar track -----------------------------------------------
     def forward(self, vec, csr: EdgeCSR, types_i32, outs):
-        """vec [E,3] -> the scalar-embed MLP's outputs written into ``outs`` ([x_emb], or with the embed fold
-        [w0, x_0, omega_0]).  Returns what ``backward`` needs."""
+        """vec [E,3] -> the scalar-embed MLP's outputs, with the embed linears folded in, written into ``outs``
+        ([w0, x_0, omega_0]).  Returns what ``backward`` needs."""
         dt = self.dtype
         if self.kind == "spline":
             from ._spline import spline_forward
@@ -481,20 +389,12 @@ def edge_energy_grad(core: "AllegroCore", up: UpstreamPack, csr: EdgeCSR, vec: t
     X, Ez, gvec [E,3] = d E_total / d vec (acc dtype), Ei_pair or None).  ``types_i32`` is indexed by both ``csr.ctr`` and
     ``csr.nbr``; ``gEi_scale`` and ``pair`` as in ``energy_forces``.  Positions never enter: the caller may hand in edge
     vectors of any geometry (phonons.force_constants passes displaced copies of the rows of a cluster)."""
-    dt = core.dtype
-    E = csr.num_edges
-    if up.fold:
-        box = []
-        Ei, X, Ez, sv = core.forward(csr, vec, None, fill_embed=lambda w0, x0, om0: box.append(up.forward(vec, csr, types_i32, [w0, x0, om0])))
-        up_saved = box[0]
-    else:
-        x_emb = torch.empty(E, core.S_in, dtype=dt, device=vec.device)
-        up_saved = up.forward(vec, csr, types_i32, [x_emb])
-        Ei, X, Ez, sv = core.forward(csr, vec, x_emb)
+    box = []
+    Ei, X, Ez, sv = core.forward(csr, vec, None, fill_embed=lambda w0, x0, om0: box.append(up.forward(vec, csr, types_i32, [w0, x0, om0])))
     gEi = gEi_scale if gEi_scale is not None else torch.ones_like(Ei)
-    gvec, gx_emb = core.backward(sv, gEi)
+    gvec, g_emb = core.backward(sv, gEi)
     _lib.set_tag("bwd.radial")
-    up.backward(up_saved, gx_emb if up.fold else [gx_emb], vec, csr, types_i32, gvec)
+    up.backward(box[0], g_emb, vec, csr, types_i32, gvec)
     Ei_pair = None
     if pair is not None:
         Ez_pair = pair[0].edge_energy_and_grad(vec, csr, types_i32, pair[1], gvec)

@@ -32,8 +32,7 @@ TOL = 1e-4
 # 1.3e-5: the CUDA error is 5-9x that at every l_max (lmax0, lmax1 and lmax3 alike), so it is not the l_max 4 tables.
 TOL_F = {"lmax3": 2e-4, "lmax4": 4e-5, "lmax4_L3": 1.2e-4}
 
-# c2 widths (S = H = readout hidden width = 64, U = 32, l_max = 2, L = 2), then per case the overrides, and whether the
-# opt-in plain-GEMM backward is switched on
+# c2 widths (S = H = readout hidden width = 64, U = 32, l_max = 2, L = 2), then per case the overrides
 C3_AT_C2_WIDTHS = dict(num_scalar_features=64, num_tensor_features=32, radial_chemical_embed_dim=64, scalar_embed_mlp_hidden_layers_width=64,
                        allegro_mlp_hidden_layers_width=64, readout_mlp_hidden_layers_width=64)
 CASES = {
@@ -55,12 +54,10 @@ CASES = {
     "linear_latents": dict(allegro_mlp_nonlinearity=None),
     "three_species": dict(C3_AT_C2_WIDTHS, per_type_energy_scales=[2.5, 0.5, 1.25], per_type_energy_shifts=[-1.25, 0.5, 2.0],
                           per_edge_type_cutoff={"Li": 4.0, "P": {"Li": 5.0, "P": 4.5, "S": 6.0}, "S": 5.5}),
-    "plain_bwd_L3": dict(num_layers=3),
     "lmax0": dict(l_max=0),
     "lmax4": dict(l_max=4),
     "lmax4_L3": dict(l_max=4, num_layers=3),
 }
-PLAIN_BWD = {"plain_bwd_L3"}
 
 # Which entry each stage asks, in call order, and its verdict: "+" taken, "-" declined (the caller then runs the separate
 # MLPs or the plain linear layers).  mlp2 = ab2_mlp2, ro = ab2_mlp2_readout, chain / chain_bwd = ab2_tp_chain_fwd / _bwd.
@@ -70,7 +67,7 @@ PLAIN_BWD = {"plain_bwd_L3"}
 #   (2, 96) 243 840 / 242 816, (3, 32) 260 224 / 259 200, (3, 64) 268 416 / 267 392; H = 32 is not built (RO_H = 64).
 #   ab2_mlp2 takes every stage except: N > 256 (more than four 64-column chunks), and 192 x 64 -> 256 / 256 x 64 -> 192
 #   (235 520 bytes), 352 x 64 -> 160 (251 904 bytes).
-#   ab2_tp_chain_*: two-layer l_max = 2 models with the baked tables, U = 32 or 64, the default backward, E > 0.
+#   ab2_tp_chain_*: two-layer l_max = 2 models with the baked tables, U = 32 or 64, E > 0.
 C2 = {  # L = 2, U = 32 (c2): composed tensor products, fused readout
     "fwd.L0": "chain+ mlp2+",          # 96 x 64 -> 160: 219 136 bytes
     "fwd.L1": "chain+ ro+",            # 227 456 bytes
@@ -133,8 +130,6 @@ DISPATCH = {
     "linear_latents": {"fwd.L0": "chain+", "fwd.L1": "chain+", "fwd.readout": "mlp2+", "bwd.readout": "mlp2+",
                        "bwd.L1": "chain_bwd+", "bwd.L0": "chain_bwd+"},
     "three_species": C2,
-    # the plain-GEMM backward runs no fused MLP kernel; its forward is that of L3_U32
-    "plain_bwd_L3": {"fwd.L0": "mlp2+", "fwd.L1": "mlp2+", "fwd.L2": "ro- mlp2+", "fwd.readout": "mlp2+"},
     # l_max 0 and 4: no composed tensor products either; the env weights are (l_max + 1) U wide, so the first latent MLP is
     # 96 x 64 -> 96 and 96 x 64 -> 224 (S + 5U, under the four-chunk limit) and its backward 96 / 224 x 64 -> 96; the fused
     # readout depends on (L, U) only: taken at (2, 32), declined at (3, 32) as in L3_U32
@@ -221,8 +216,6 @@ def _spy_tp(monkeypatch):
 @pytest.mark.parametrize("case,frame", _cases())
 def test_fp32_grid(case, frame, monkeypatch):
     over = CASES[case]
-    if case in PLAIN_BWD:
-        monkeypatch.setenv("ALLEGRO_B200_PLAIN_BWD", "1")
     if frame.startswith(("c2_", "c3_")):
         name, scale = frame.split("_")
         oracle, model, d = _pair(name, int(scale), "float32", **over)
@@ -234,7 +227,6 @@ def test_fp32_grid(case, frame, monkeypatch):
     got = _dispatch(rec)
     print(f"\n{case} {frame} (E = {E}): E {ee:.2e} F {ef:.2e}  dispatch {got}")
     core = model.model.core()
-    assert core.plain_ok == (case in PLAIN_BWD)
     assert got == (DISPATCH[case] if E else {})
     if E == 0:
         assert tp_rec == []

@@ -100,16 +100,6 @@ def test_autograd_path_matches_direct_path():
     assert (direct[D.PER_ATOM_ENERGY_KEY] - auto[D.PER_ATOM_ENERGY_KEY]).abs().max() < 1e-10
 
 
-def test_plain_gemm_backward_plan(monkeypatch):
-    """Alternative backward orchestration (producer-side SiLU', concat-K block gradients)."""
-    monkeypatch.setenv("ALLEGRO_B200_PLAIN_BWD", "1")
-    oracle, model, d = _pair("c2", 3, "float32")
-    assert model.model.core().plain_ok
-    _check(oracle, model, d, 1e-4, 1e-4)
-    oracle, model, d = _pair("c2", 3, "float64")
-    _check(oracle, model, d, 1e-9, 1e-9)
-
-
 def test_c2_bf16():
     oracle, model, d = _pair("c2", 3, "bfloat16")
     ee, ef = _check(oracle, model, d, 2e-2, 5e-2)

@@ -552,17 +552,18 @@ def test_edge_sum_force_scatter_ragged(dtype):
 # GPU: whole models on the stored-feature kernels at c3 widths
 # --------------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_c3_widths_plain_backward_fp32(monkeypatch):
-    """c3 widths (S = 128, U = 64: the two-chunk UT = 64 builds) on the 6^3 reduced cell with the opt-in plain backward,
-    which keeps the model on the stored-feature tensor-product kernels (no composed two-layer path)."""
+def test_c3_widths_stored_v_fp32(monkeypatch):
+    """c3 widths (S = 128, U = 64: the two-chunk UT = 64 builds) on the 6^3 reduced cell, with the composed two-layer
+    path declined so that the model runs on the stored-feature tensor-product kernels."""
+    from allegro_b200 import _lib
     from test_gpu_model import _check, _pair
 
-    monkeypatch.setenv("ALLEGRO_B200_PLAIN_BWD", "1")
+    monkeypatch.setattr(_lib, "tp_chain_plan", lambda *a: None)
     oracle, model, d = _pair("c3", 6, "float32")
     core = model.model.core()
-    assert core.U == 64 and core.plain_ok and core.chain is None
+    assert core.U == 64 and core.chain is None
     ee, ef = _check(oracle, model, d, 1e-4, 1e-4)
-    print(f"c3 widths fp32 plain backward: E {ee:.2e} F {ef:.2e}")
+    print(f"c3 widths fp32 stored V: E {ee:.2e} F {ef:.2e}")
 
 
 @pytest.mark.gpu

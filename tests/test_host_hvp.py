@@ -182,7 +182,7 @@ def spec_kernels(monkeypatch):
 
 
 @pytest.mark.parametrize("variant", ["default", "nofold", "product_embed", "zbl", "lmax3_L3"])
-def test_composed_tangent_equals_the_oracle_hessian(variant, spec_kernels, monkeypatch):
+def test_composed_tangent_equals_the_oracle_hessian(variant, spec_kernels):
     from allegro_b200 import data as D
     from allegro_b200 import systems
     from allegro_b200.model import AllegroModel
@@ -190,9 +190,6 @@ def test_composed_tangent_equals_the_oracle_hessian(variant, spec_kernels, monke
     from allegro_b200.phonons import _energy_terms
     from oracle.model_ref import AllegroOracle
 
-    env = {"nofold": {"ALLEGRO_B200_FOLD_EMBED": "0", "ALLEGRO_B200_FOLD_RADIAL": "0"}, "product_embed": {"ALLEGRO_B200_RADIAL_PQ": "0"}}
-    for k, v in env.get(variant, {}).items():
-        monkeypatch.setenv(k, v)
     small = dict(num_scalar_features=16, num_tensor_features=8, radial_chemical_embed_dim=16, scalar_embed_mlp_hidden_layers_width=16,
                  allegro_mlp_hidden_layers_width=16, readout_mlp_hidden_layers_width=8)
     sysname = "c3" if variant == "zbl" else "c2"
@@ -203,6 +200,10 @@ def test_composed_tangent_equals_the_oracle_hessian(variant, spec_kernels, monke
                   per_type_energy_scales=[1.5, 0.5, 2.0])
     if variant == "lmax3_L3":
         kw.update(l_max=3, num_layers=3)
+    if variant == "nofold":  # two hidden layers: the per-type-pair radial kernel without the first layer folded in
+        kw.update(scalar_embed_mlp_hidden_layers_depth=2)
+    if variant == "product_embed":  # not 8 Bessels: the product-embedding radial kernel
+        kw.update(radial_chemical_embed=dict(kw["radial_chemical_embed"], num_bessels=5))
     oracle = AllegroOracle(**kw)
     model = AllegroModel(**dict(kw, model_dtype="float64"))
     model.load_state_dict(oracle.state_dict())
@@ -214,6 +215,11 @@ def test_composed_tangent_equals_the_oracle_hessian(variant, spec_kernels, monke
     row_ptr, ctr, nbr, sv = frame_list(pos, None, (False,) * 3, kw["r_max"])
     csr = D.EdgeCSR(n, ctr.to(torch.int32), nbr.to(torch.int32), row_ptr.to(torch.int32), None, int((row_ptr[1:] - row_ptr[:-1]).max()))
     core = inner.core()
+    up = inner._upstream
+    if variant == "nofold":
+        assert up.PQ is not None and not up.fold_radial
+    if variant == "product_embed":
+        assert up.PQ is None
     types_i32 = types.to(torch.int32)
     gscale, pair = _energy_terms(inner, core, types, torch.device("cpu"))
     vec = pos[nbr] - pos[ctr] + sv

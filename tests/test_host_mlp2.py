@@ -67,13 +67,10 @@ def _rel(a, b):
     return float((a - b).abs().max()) / (den if den > 0 else 1.0)
 
 
-@pytest.mark.parametrize("plain", [False, True], ids=["legacy_bwd", "plain_bwd"])
 @pytest.mark.parametrize("name", model_case_ids())
-def test_host_pipeline_with_fused_mlp(name, plain, spec_kernels_mlp2, monkeypatch):
+def test_host_pipeline_with_fused_mlp(name, spec_kernels_mlp2):
     from allegro_b200.model import AllegroModel
 
-    if plain:
-        monkeypatch.setenv("ALLEGRO_B200_PLAIN_BWD", "1")
     rec = MODELS[name]
     model = AllegroModel(**rec["kwargs"])
     model.load_state_dict(unpack_state_dict(rec["state_dict"]), strict=True)
@@ -86,7 +83,6 @@ def test_host_pipeline_with_fused_mlp(name, plain, spec_kernels_mlp2, monkeypatc
     calls = spec_kernels_mlp2
     if fp32:
         assert any(not bwd for bwd, _ in calls), "the forward MLPs did not take the fused path"
-        if not plain:  # the default backward: latent MLPs and the rank-1 readout
-            assert any(bwd and k == 1 for bwd, k in calls), "the readout backward did not take the rank-1 fused path"
+        assert any(bwd and k == 1 for bwd, k in calls), "the readout backward did not take the rank-1 fused path"
     else:
         assert not calls

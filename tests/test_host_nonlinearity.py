@@ -264,11 +264,8 @@ def _models(case):
     return ref, model, dict(rec["data"]), kw
 
 
-@pytest.mark.parametrize("plain", [False, True], ids=["default_bwd", "plain_bwd"])
 @pytest.mark.parametrize("case", list(CASES))
-def test_host_pipeline_against_oracle(case, plain, spec, monkeypatch):
-    if plain:
-        monkeypatch.setenv("ALLEGRO_B200_PLAIN_BWD", "1")
+def test_host_pipeline_against_oracle(case, spec):
     ref, model, d, kw = _models(case)
     expect = ref(dict(d))
     out = model.model._energy_and_forces(dict(d), True)
@@ -291,22 +288,20 @@ def test_host_pipeline_against_oracle(case, plain, spec, monkeypatch):
     uniform = kw["allegro_mlp_nonlinearity"] == kw["readout_mlp_nonlinearity"]
     same_width = kw["allegro_mlp_hidden_layers_width"] == kw["readout_mlp_hidden_layers_width"]
     assert core.ro_fused == (two and uniform and same_width)
-    assert core.plain_ok == (plain and two and uniform)
     assert any(e == "ro" for e, _, _ in spec) == core.ro_fused
     assert any(e == "ro" and ok for e, _, ok in spec) == (fp32 and core.ro_fused)
     assert any(e == "mlp2" and ok for e, _, ok in spec) == (fp32 and any(e == "mlp2" for e, _, _ in spec))
 
 
-def test_mixed_models_decline_the_shared_nonlinearity_paths(spec, monkeypatch):
-    """A model whose last latent MLP and readout differ in nonlinearity does not ask ab2_mlp2_readout, and with the
-    plain-GEMM backward requested does not take it; the uniform model of the same shape takes both."""
-    monkeypatch.setenv("ALLEGRO_B200_PLAIN_BWD", "1")
+def test_mixed_models_decline_the_shared_nonlinearity_paths(spec):
+    """A model whose last latent MLP and readout differ in nonlinearity does not ask ab2_mlp2_readout; the uniform model
+    of the same shape does."""
     for case, uniform in (("mixed_f32", False), ("mish_c2arch_f32", True)):
         spec.clear()
         _, model, d, _ = _models(case)
         model.model._energy_and_forces(dict(d), True)
         core = model.model.core()
-        assert core.ro_fused == uniform and core.plain_ok == uniform
+        assert core.ro_fused == uniform
         assert any(e == "ro" for e, _, _ in spec) == uniform
 
 

@@ -49,10 +49,10 @@ def _run(name, stress=True):
     return rec, model.model._energy_and_forces(dict(rec["data"]), stress)
 
 
-@pytest.mark.parametrize("fold", ["1", "0"], ids=["fold", "nofold"])
 @pytest.mark.parametrize("name", model_case_ids())
-def test_host_pipeline_reproduces_reference(name, fold, spec_kernels, monkeypatch):
-    monkeypatch.setenv("ALLEGRO_B200_FOLD_EMBED", fold)
+def test_host_pipeline_reproduces_reference(name, spec_kernels):
+    """The two linear maps that consume the two-body embedding are folded into the last layer of the scalar-embed MLP
+    (one GEMM less per direction): energies, forces and per-edge outputs are the reference's."""
     rec, out = _run(name)
     tol = 1e-10 if rec["kwargs"]["model_dtype"] == "float64" else 5e-5
     for key in ("atomic_energy", "forces", "edge_energy", "edge_features", "total_energy"):
@@ -60,24 +60,32 @@ def test_host_pipeline_reproduces_reference(name, fold, spec_kernels, monkeypatc
             assert _rel(out[key], rec[key]) < tol, (key, _rel(out[key], rec[key]))
 
 
-@pytest.mark.parametrize("env", [{"ALLEGRO_B200_FOLD_RADIAL": "0"}, {"ALLEGRO_B200_RADIAL_PQ": "0"}, {"ALLEGRO_B200_FOLD_RADIAL": "0", "ALLEGRO_B200_FOLD_EMBED": "0"}],
-                         ids=["pq_nofold", "product_embed_kernel", "pq_nofold_noembedfold"])
+@pytest.mark.parametrize("variant", ["pq_nofold", "product_embed_kernel", "pq_linear_mlp"])
 @pytest.mark.parametrize("name", ["c2_lmax2_L2", "c5_lmax3_L3_5species", "per_edge_type_cutoff"])
-def test_host_pipeline_radial_variants(name, env, spec_kernels, monkeypatch):
-    """The upstream scalar track with the first MLP layer folded into the radial kernel (default), with the per-type-pair
-    kernel but no fold, and with the round-1 product-embedding kernel: same energies and forces."""
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-    rec, out = _run(name)
-    assert _rel(out["forces"], rec["forces"]) < 1e-10 and _rel(out["atomic_energy"], rec["atomic_energy"]) < 1e-10
+def test_host_pipeline_radial_variants(name, variant, spec_kernels):
+    """The radial routes the model shape selects besides the default (first MLP layer folded into the per-type-pair
+    kernel): a scalar-embed MLP with two hidden layers or none keeps the per-type-pair kernel without the fold, and a
+    basis other than 8 Bessels takes the product-embedding kernel.  Same energies and forces as the oracle."""
+    from allegro_b200.model import AllegroModel
+    from oracle.model_ref import AllegroOracle
 
-
-@pytest.mark.parametrize("name", ["c2_lmax2_L2", "c5_lmax3_L3_5species", "shared_irrep_weights", "spline_embed_reftest_cfg"])
-def test_host_pipeline_plain_backward_plan(name, spec_kernels, monkeypatch):
-    """The alternative backward orchestration (producer-side SiLU', concat-K block gradients) gives the same forces."""
-    monkeypatch.setenv("ALLEGRO_B200_PLAIN_BWD", "1")
-    rec, out = _run(name)
-    assert _rel(out["forces"], rec["forces"]) < 1e-10
+    rec = MODELS[name]
+    kw = dict(rec["kwargs"])
+    if variant == "product_embed_kernel":
+        kw["radial_chemical_embed"] = dict(kw["radial_chemical_embed"], num_bessels=5)
+    else:
+        kw["scalar_embed_mlp_hidden_layers_depth"] = 2 if variant == "pq_nofold" else 0
+    oracle = AllegroOracle(**kw)
+    model = AllegroModel(**kw)
+    model.load_state_dict(oracle.state_dict(), strict=True)
+    out = model.model._energy_and_forces(dict(rec["data"]), True)
+    up = model.model._upstream
+    if variant == "product_embed_kernel":
+        assert up.PQ is None
+    else:
+        assert up.PQ is not None and not up.fold_radial
+    ref = oracle(dict(rec["data"]))
+    assert _rel(out["forces"], ref["forces"]) < 1e-10 and _rel(out["atomic_energy"], ref["atomic_energy"]) < 1e-10
 
 
 def test_host_pipeline_stress_matches_oracle(spec_kernels):
@@ -122,21 +130,6 @@ def test_host_pipeline_under_the_md_driver(spec_kernels, monkeypatch):
         assert _rel(out["stress"], ref["stress"]) < 1e-10
         p = p + 0.1 * torch.randn(p.shape, generator=g, dtype=p.dtype)
     assert calc.n_rebuilds >= 1 and calc.n_evaluations == 3
-
-
-@pytest.mark.parametrize("plain", [False, True], ids=["legacy_bwd", "plain_bwd"])
-@pytest.mark.parametrize("name", model_case_ids())
-def test_host_pipeline_with_folded_embed_linears(name, plain, spec_kernels, monkeypatch):
-    """ALLEGRO_B200_FOLD_EMBED=1: the two linear maps that consume the two-body embedding are folded into the last layer
-    of the scalar-embed MLP (one GEMM less per direction).  Same energies, forces and per-edge outputs."""
-    monkeypatch.setenv("ALLEGRO_B200_FOLD_EMBED", "1")
-    if plain:
-        monkeypatch.setenv("ALLEGRO_B200_PLAIN_BWD", "1")
-    rec, out = _run(name)
-    tol = 1e-10 if rec["kwargs"]["model_dtype"] == "float64" else 5e-5
-    for key in ("atomic_energy", "forces", "edge_energy", "edge_features"):
-        if key in rec:
-            assert _rel(out[key], rec[key]) < tol, (key, _rel(out[key], rec[key]))
 
 
 def test_prepared_csr_with_owned_centres_only(spec_kernels):

@@ -143,15 +143,12 @@ def test_host_pipeline_with_tp_chain(name, monkeypatch):
         assert calls == [("fwd", False), ("fwd", True), ("bwd", False), ("bwd", True)], calls
 
 
-@pytest.mark.parametrize("dtype,plain,taken", [("float32", False, True), ("float64", False, False), ("bfloat16", False, False),
-                                               ("float32", True, False)], ids=["fp32", "fp64", "bf16", "fp32_plain_bwd"])
-def test_which_models_take_tp_chain(dtype, plain, taken, monkeypatch):
+@pytest.mark.parametrize("dtype,taken", [("float32", True), ("float64", False), ("bfloat16", False)], ids=["fp32", "fp64", "bf16"])
+def test_which_models_take_tp_chain(dtype, taken, monkeypatch):
     """The GPU rule of tp_chain_plan (fp32, U = 32 or 64) with the device check left out, on the U = 32 case."""
     from allegro_b200 import _lib
 
     _patch_spec(monkeypatch)
-    if plain:
-        monkeypatch.setenv("ALLEGRO_B200_PLAIN_BWD", "1")
     takes = _lib.tp_chain_takes
     monkeypatch.setattr(_lib, "tp_chain_plan",
                         lambda dt, U, cgw0, cgw1: {"cgw0": cgw0, "cgw1": cgw1, "U": U} if takes(dt, U) else None)

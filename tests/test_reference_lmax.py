@@ -48,14 +48,11 @@ def test_oracle_reproduces_reference(name):
         assert _rel(out[key], rec[key]) < 1e-10, (key, _rel(out[key], rec[key]))
 
 
-@pytest.mark.parametrize("plain", [False, True], ids=["legacy_bwd", "plain_bwd"])
 @pytest.mark.parametrize("name", list(CASES))
-def test_host_pipeline_reproduces_reference(name, plain, spec_kernels, monkeypatch):  # noqa: F811
+def test_host_pipeline_reproduces_reference(name, spec_kernels):  # noqa: F811
     from allegro_b200.model import AllegroModel
     from oracle.model_ref import AllegroOracle
 
-    if plain:
-        monkeypatch.setenv("ALLEGRO_B200_PLAIN_BWD", "1")
     rec = CASES[name]
     sd = unpack_state_dict(rec["state_dict"])
     model = AllegroModel(**rec["kwargs"])
