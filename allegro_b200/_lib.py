@@ -66,6 +66,8 @@ _SIGNATURES = {
     "ab2_radial_pq_bwd_nl": ([_i32, _i64, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32], C.c_int),
     "ab2_radial_pq_bwd_gemm": ([_i32, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp,
                                 _i32], C.c_int),
+    "ab2_radial_embed_fwd": ([_i32, _i64, _i32, _i32, _vp, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32],
+                             C.c_int),
     "ab2_zbl": ([_i32, _i64, _i32, _dbl, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp], C.c_int),
     "ab2_p2p_mailbox_bytes": ([_i32, _i32], C.c_int64),
     "ab2_p2p_alloc": ([_i64, C.POINTER(C.c_void_p)], C.c_int),
@@ -887,14 +889,47 @@ def radial_pq_fwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table,
     return out
 
 
+def radial_embed_fwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table, bessel_w, PQ, W_packed, o_segs: Sequence[torch.Tensor],
+                     nonlin: int = NL_SILU) -> bool:
+    """cat(o_segs, -1) = phi(h) @ W with h = radial_pq_fwd(...) [E,S] and ``W_packed`` the ``linear_pack`` image of W [S,N],
+    in one kernel (ab2_radial_embed_fwd): h is never stored, and the result is bitwise that of ``radial_pq_fwd`` followed
+    by ``linear(act=ACT_SILU)``.  Returns False, with nothing computed, when the kernel does not take the case; the
+    caller then makes those two calls."""
+    if W_packed is None:
+        return False
+    E = ctr.shape[0]
+    no = len(o_segs)
+    o_ptr = (C.c_void_p * no)()
+    o_ld = (C.c_int64 * no)()
+    o_w = (C.c_int32 * no)()
+    for s, t in enumerate(o_segs):
+        t, ld = _row_strided(t, f"output segment {s}")
+        assert t.dtype == dtype and t.shape[0] == E
+        o_ptr[s], o_ld[s], o_w[s] = t.data_ptr(), ld, t.shape[1]
+        _ptr(t)
+    N = sum(int(w) for w in o_w)
+    assert W_packed.numel() == 2 * 2 * S * (-(-N // 32) * 32), "W_packed is not the image of an [S, N] matrix"
+    timer = _timed("radial_embed_fwd")
+    args = (DTYPE_ENUM[dtype], E, S, N, _ptr(W_packed), bessel_w.numel(), float(p_cut), _ptr(_contig(vec, "vec")), _ptr(ctr), _ptr(nbr),
+            _ptr(types), _ptr(rmax_table), rmax_table.shape[0], _ptr(bessel_w), _ptr(_contig(PQ, "PQ")), no, o_ptr, o_ld, o_w, _stream(), int(nonlin))
+    with timer:
+        rc = load().ab2_radial_embed_fwd(*args)
+    if rc == NOT_ELIGIBLE:
+        timer.cancel()
+        return False
+    _check(rc)
+    return True
+
+
 def radial_pq_bwd(dtype, S: int, p_cut: float, vec, ctr, nbr, types, rmax_table, bessel_w, PQ, g_out, aux, gvec, nonlin: int = NL_SILU,
                   gemm: Optional[Tuple[Sequence[torch.Tensor], Optional[torch.Tensor]]] = None) -> bool:
     """gvec += (d out / d vec)^T (g_out * phi'(aux)) (aux None: plain g_out); phi the nonlinearity ``nonlin`` (NL_*).
 
     ``gemm = (gout_segs, W2T_packed)`` with ``g_out = None``: g_out is the product cat(gout_segs, -1) @ W2^T (W2T_packed from
     ``linear_pack``), and aux the ab2_radial_pq_fwd output h of these edges.  Then one kernel (ab2_radial_pq_bwd_gemm) forms
-    the product and applies the adjoint to it, h recomputed: neither is stored.  Returns False, with nothing computed,
-    when that kernel does not take the case; the caller then forms g_out and calls again without ``gemm``."""
+    the product and applies the adjoint to it, h recomputed: neither is stored, and aux, which that kernel never reads, may
+    be a meta tensor of h's shape.  Returns False, with nothing computed, when that kernel does not take the case; the
+    caller then forms g_out and calls again without ``gemm``."""
     E = ctr.shape[0]
     if gemm is not None:
         gout_segs, W2T_packed = gemm

@@ -1167,6 +1167,170 @@ __global__ void __launch_bounds__(NTHREADS, 1) radial_adjoint_tma_kernel(const T
 }
 
 // =========================================================================================
+// Radial embedding and the scalar-embed MLP's folded last layer in one kernel (ab2_radial_embed_fwd): the forward of
+//   h = radial_pq_fwd(vec)  [M][H]                                                         (radial_pq_fwd_kernel)
+//   [w0 | x_0 | omega_0] = phi(h) @ W_fold   [M][N]                                         (ab2_linear, N / 128 slices)
+// without h in memory, and with the whole output formed from one on-chip A tile instead of one pass over h per slice.
+//   warps 0-7    : generators.  Thread t of the 256 owns row 16 (t / 32) + (t % 16) of each 128-row tile and half
+//                  (t % 32) / 16 of its H / 8 core-matrix columns: it evaluates the row's basis (vec, ctr, nbr one tile
+//                  ahead), forms h with the fmaf chain of radial_pq_fwd_kernel (n order from 0, so h is bitwise the
+//                  stored one), applies phi as the converters do and writes the bf16 hi + lo split, one 16-byte store per
+//                  image and core-matrix row, into a double-buffered canonical K-major [128][H] tile.  Each aligned
+//                  group of 8 lanes writes one whole core matrix: conflict-free.
+//   warps 8-15   : two consumer warpgroups.  Per tile and column chunk (the slicing of ab2_linear, so the same wgmma
+//                  shapes) acc = phi(h) @ W_fold[:, chunk] from the resident tile in the k16 / split-product order of
+//                  tc_mma_ring, then tc_epilogue into the chunk's output segments: bitwise the sliced launches' result.
+//                  The A buffer is released once the last chunk's wgmma group has retired.
+// W_fold (hi + lo) and PQ of every type pair stay resident.  PQ rows of consecutive pairs are 16 bytes further apart than
+// 8 H floats, so that generator lanes of different pairs read different bank groups.
+// =========================================================================================
+constexpr int REMB_MAX_CHUNKS = 2;  // N <= 256 in column chunks of <= MAX_N
+
+struct RadialEmbedParams {
+    TcParams s[REMB_MAX_CHUNKS];  // per column chunk: M, N, Npad, output segments
+    int n0[REMB_MAX_CHUNKS];      // first column of each chunk
+    int n_chunks;
+    int w_half;                   // bytes of the whole W_fold hi image (= lo image)
+    const void* W;                // packed W_fold: hi image, then lo image
+    const float* vec;             // [M][3]
+    const int32_t* ctr;
+    const int32_t* nbr;
+    const int32_t* types;
+    const float* rmax_table;      // [T][T]
+    const float* bw;              // [RADJ_NB]
+    const float* PQ;              // [T * T][RADJ_NB][H]
+    int num_types;
+    float p;                      // polynomial cutoff order
+    int64_t M, num_tiles;
+};
+
+template <int NCH>
+__device__ __forceinline__ void radial_embed_chunk(const TcParams& pc, const ChunkInfo* chunks, float* stg, uint32_t a_u, uint32_t a_half, int H,
+                                                   uint32_t w_u, uint32_t w_half, bool release, uint32_t empty, int64_t tile, int wg, int w4,
+                                                   int lane) {
+    float acc[16 * NCH];
+    tc_mma_resident<NCH>(acc, a_u, a_half, H, w_u, w_half);
+    if (release && lane == 0) mbar_arrive(empty);  // this warp's wgmma reads of the A buffer have retired
+    tc_epilogue<float, NCH, false, false>(pc, chunks, stg, acc, tile, wg, w4, lane);
+}
+
+template <int NCH1, int NL>
+__global__ void __launch_bounds__(NTHREADS, 1) radial_embed_fwd_kernel(const __grid_constant__ RadialEmbedParams q) {
+    constexpr int H = 32 * NCH1;
+    constexpr int A_HALF = BM * H * 2;          // one bf16 image of a [128][H] tile
+    constexpr int PQ_LD = RADJ_NB * H + 4;      // floats between the PQ blocks of consecutive type pairs
+    extern __shared__ __align__(1024) uint8_t smem[];
+    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;  // warp-uniform role index
+    // plan: W_fold (hi, lo) | A tiles [2] (hi, lo) | epilogue staging | PQ | barriers | chunk tables
+    uint8_t* sW = smem;
+    uint8_t* sA = sW + 2 * q.w_half;
+    float* sEpi = reinterpret_cast<float*>(sA + 2 * 2 * A_HALF);
+    float* sPQ = sEpi + EPI_BYTES / 4;
+    const int npair = q.num_types * q.num_types;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sPQ + ((npair * PQ_LD + 3) & ~3));  // full[2], empty[2]
+    ChunkInfo* sChunk = reinterpret_cast<ChunkInfo*>(bars + 4);                     // REMB_MAX_CHUNKS x MAX_CHUNK
+    const uint32_t bar0 = smem_u32(bars);
+    auto full_bar = [&](int b) { return bar0 + 8u * b; };
+    auto empty_bar = [&](int b) { return bar0 + 8u * (2 + b); };
+
+    // ---- one-time setup ----
+    if (threadIdx.x == 0) {
+        for (int b = 0; b < 2; ++b) {
+            mbar_init(full_bar(b), NPROD * 32);
+            mbar_init(empty_bar(b), NCONS);
+        }
+        fence_barrier_init();
+    }
+    if (threadIdx.x >= 32 && threadIdx.x < 32 + REMB_MAX_CHUNKS * MAX_CHUNK) {
+        const int i = threadIdx.x - 32, c = i / MAX_CHUNK;
+        sChunk[i] = c < q.n_chunks ? tc_chunk_info<float>(q.s[c], (i % MAX_CHUNK) * 32) : ChunkInfo{nullptr, nullptr, 0, 0, 0};
+    }
+    for (int e = threadIdx.x; e < npair * RADJ_NB * H; e += NTHREADS) sPQ[(e / (RADJ_NB * H)) * PQ_LD + e % (RADJ_NB * H)] = __ldg(q.PQ + e);
+    stage_w(sW, q.W, reinterpret_cast<const uint8_t*>(q.W) + q.w_half, q.w_half);
+    fence_proxy_async();
+    __syncthreads();
+
+    if (warp < NPROD) {
+        // =============================== generators ===============================
+        const int rloc = warp * 16 + (lane & 15), half = lane >> 4;
+        constexpr int ITEMS = H / 16;  // core-matrix columns of this thread's half row
+        auto row = [&](int64_t tile) {
+            const int64_t m = tile * BM + rloc;
+            return m < q.M ? m : q.M - 1;  // rows beyond M compute on row M - 1; their results are never stored
+        };
+        int nc = 0, nn = 0;
+        float v[3] = {0.f, 0.f, 0.f};
+        auto fetch = [&](int64_t tile) {
+            if (tile < q.num_tiles) {
+                const int64_t m = row(tile);
+                nc = __ldg(q.ctr + m);
+                nn = __ldg(q.nbr + m);
+                v[0] = __ldg(q.vec + m * 3); v[1] = __ldg(q.vec + m * 3 + 1); v[2] = __ldg(q.vec + m * 3 + 2);
+            }
+        };
+        fetch(blockIdx.x);
+        int it = 0;
+        for (int64_t tile = blockIdx.x; tile < q.num_tiles; tile += gridDim.x, ++it) {
+            const int pair = __ldg(q.types + nc) * q.num_types + __ldg(q.types + nn);
+            const float vx = v[0], vy = v[1], vz = v[2];
+            fetch(tile + gridDim.x);
+            const float r = sqrtf(vx * vx + vy * vy + vz * vz);
+            float B[RADJ_NB];
+            bessel_basis<float, false>(r / __ldg(q.rmax_table + pair), q.p, RADJ_NB, q.bw, B, nullptr);
+            const float* m = sPQ + pair * PQ_LD;
+            const int buf = it & 1;
+            mbar_wait(empty_bar(buf), ((it >> 1) & 1) ^ 1);
+            uint8_t* st = sA + buf * 2 * A_HALF + (rloc >> 3) * (H / 8) * 128 + (rloc & 7) * 16;
+#pragma unroll
+            for (int i = 0; i < ITEMS; ++i) {
+                const int c8 = half * ITEMS + i;
+                float h[8];
+#pragma unroll
+                for (int j = 0; j < 8; ++j) h[j] = 0.f;
+#pragma unroll
+                for (int n = 0; n < RADJ_NB; ++n) {
+                    const float4 a = *reinterpret_cast<const float4*>(m + n * H + c8 * 8);
+                    const float4 b = *reinterpret_cast<const float4*>(m + n * H + c8 * 8 + 4);
+                    h[0] = fmaf(B[n], a.x, h[0]); h[1] = fmaf(B[n], a.y, h[1]); h[2] = fmaf(B[n], a.z, h[2]); h[3] = fmaf(B[n], a.w, h[3]);
+                    h[4] = fmaf(B[n], b.x, h[4]); h[5] = fmaf(B[n], b.y, h[5]); h[6] = fmaf(B[n], b.z, h[6]); h[7] = fmaf(B[n], b.w, h[7]);
+                }
+                uint32_t hi[4], lo[4];
+#pragma unroll
+                for (int t = 0; t < 4; ++t) split_bf16x2(act_fast<NL>(h[2 * t]), act_fast<NL>(h[2 * t + 1]), hi[t], lo[t]);
+                *reinterpret_cast<uint4*>(st + c8 * 128) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+                *reinterpret_cast<uint4*>(st + A_HALF + c8 * 128) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+            }
+            fence_proxy_async();  // generic-proxy writes, read by wgmma through the async proxy
+            mbar_arrive(full_bar(buf));
+        }
+        return;
+    }
+    // =============================== consumers ===============================
+    const int cw = warp - NPROD, wg = cw >> 2, w4 = cw & 3;
+    float* stg = sEpi + cw * 16 * EPI_LD;
+    const uint32_t sA_u = smem_u32(sA), sW_u = smem_u32(sW);
+    int it = 0;
+    for (int64_t tile = blockIdx.x; tile < q.num_tiles; tile += gridDim.x, ++it) {
+        const int buf = it & 1;
+        mbar_wait(full_bar(buf), (it >> 1) & 1);
+        const uint32_t a_u = sA_u + buf * 2 * A_HALF + wg * 64 * H * 2;  // this warpgroup's 64 rows
+#pragma unroll 1
+        for (int c = 0; c < q.n_chunks; ++c) {
+            const TcParams& pc = q.s[c];
+            const ChunkInfo* ch = sChunk + c * MAX_CHUNK;
+            const uint32_t w_u = sW_u + (uint32_t)q.n0[c] * H * 2;
+            const bool last = c == q.n_chunks - 1;
+            switch (pc.Npad / 32) {
+                case 1: radial_embed_chunk<1>(pc, ch, stg, a_u, A_HALF, H, w_u, q.w_half, last, empty_bar(buf), tile, wg, w4, lane); break;
+                case 2: radial_embed_chunk<2>(pc, ch, stg, a_u, A_HALF, H, w_u, q.w_half, last, empty_bar(buf), tile, wg, w4, lane); break;
+                case 3: radial_embed_chunk<3>(pc, ch, stg, a_u, A_HALF, H, w_u, q.w_half, last, empty_bar(buf), tile, wg, w4, lane); break;
+                default: radial_embed_chunk<4>(pc, ch, stg, a_u, A_HALF, H, w_u, q.w_half, last, empty_bar(buf), tile, wg, w4, lane); break;
+            }
+        }
+    }
+}
+
+// =========================================================================================
 // Two-layer SiLU MLP in one kernel (ab2_mlp2).  Stage 1 is the TMA-fed GEMM of linear_tma_kernel (A @ W1, converter
 // warps unchanged); stage 2 multiplies the hidden layer, kept on chip, by W2.  Per 128-row tile each consumer warpgroup,
 // for its own 64 rows:
@@ -2131,6 +2295,87 @@ extern "C" int ab2_radial_pq_bwd_gemm(int dtype, int64_t M, int K, int H, int n_
     return tc_with_nl(nonlin, [&](auto nl) -> int {
         constexpr int NL = decltype(nl)::value;
         return H == 32 ? go(radial_adjoint_tma_kernel<4, 1, NL>) : go(radial_adjoint_tma_kernel<4, 2, NL>);
+    });
+}
+
+// Radial embedding + the scalar-embed MLP's folded last layer (radial_embed_fwd_kernel); contract in include/allegro_b200.h.
+// Returns AB2_NOT_ELIGIBLE, with nothing enqueued and no error set, for a case the kernel does not take: the caller then
+// runs ab2_radial_pq_fwd and ab2_linear_nl.
+extern "C" int ab2_radial_embed_fwd(int dtype, int64_t M, int H, int N, const void* W_packed, int num_bessels, double p_cut, const void* vec,
+                                    const int32_t* ctr, const int32_t* nbr, const int32_t* types, const void* rmax_table, int num_types,
+                                    const void* bessel_w, const void* PQ, int n_o, void* const* o_ptr, const int64_t* o_ld, const int32_t* o_width,
+                                    void* stream, int nonlin) {
+    AB2_CHECK_ARG(nonlin == AB2_NL_SILU || nonlin == AB2_NL_MISH || nonlin == AB2_NL_GELU, "nonlinearity");
+    AB2_CHECK_ARG(M >= 0, "shape");
+    if (M == 0) return 0;  // (empty operands may come with null pointers)
+    AB2_CHECK_ARG(n_o >= 1 && n_o <= AB2_MAX_SEG, "segment count");
+    AB2_CHECK_ARG(H > 0 && N > 0 && num_types > 0, "shape");
+    int ns = 0;
+    for (int s = 0; s < n_o; ++s) {
+        AB2_CHECK_ARG(o_ptr[s] && o_width[s] > 0 && o_ld[s] >= o_width[s], "output segment");
+        ns += o_width[s];
+    }
+    AB2_CHECK_ARG(ns == N, "output segment widths must sum to N");
+    AB2_CHECK_ARG(W_packed && vec && ctr && nbr && types && rmax_table && bessel_w && PQ, "null pointer");
+    // ---- eligibility ----
+    if (dtype != AB2_F32 || !g_ab2_opt_linear_tc || !g_ab2_opt_linear_tma) return AB2_NOT_ELIGIBLE;
+    if (num_bessels != RADJ_NB || (H != 32 && H != 64) || N > REMB_MAX_CHUNKS * MAX_N || M >= ((int64_t)1 << 31)) return AB2_NOT_ELIGIBLE;
+    for (int s = 0; s < n_o; ++s)  // every 32-column chunk inside one segment, on the coalesced epilogue path
+        if (o_width[s] % 32 != 0 || (reinterpret_cast<uintptr_t>(o_ptr[s]) % 16) != 0 || (o_ld[s] * 4) % 16 != 0) return AB2_NOT_ELIGIBLE;
+    const int Npad = tc_npad(N);
+    const int w_half = Npad * H * 2;
+    const size_t pq_bytes = (size_t)num_types * num_types * (RADJ_NB * H + 4) * 4;
+    const size_t smem = (size_t)2 * w_half + (size_t)4 * BM * H * 2 + EPI_BYTES + ((pq_bytes + 15) & ~(size_t)15) + 4 * 8 +
+                        REMB_MAX_CHUNKS * MAX_CHUNK * sizeof(ChunkInfo);
+    int num_sms = 0, max_smem = 0;
+    tc_device_limits(num_sms, max_smem);
+    if (smem > (size_t)max_smem) return AB2_NOT_ELIGIBLE;  // PQ beyond what is left next to W_fold and the A tiles
+
+    RadialEmbedParams q;
+    memset(&q, 0, sizeof(q));
+    q.M = M; q.num_tiles = (M + BM - 1) / BM;
+    // column chunks: the slices of ab2_linear_tc_try (equal, multiples of 32, <= MAX_N), so each chunk runs the wgmma shape
+    // of the launch it replaces
+    const int nchunks = (N + MAX_N - 1) / MAX_N;
+    const int cwidth = ((N + nchunks - 1) / nchunks + 31) / 32 * 32;
+    for (int n0 = 0; n0 < N; n0 += cwidth, ++q.n_chunks) {
+        const int nc = (N - n0 < cwidth) ? (N - n0) : cwidth;
+        TcParams& pc = q.s[q.n_chunks];
+        pc.M = M; pc.K = H; pc.N = nc; pc.Npad = tc_npad(nc); pc.epi = AB2_EPI_NONE; pc.num_tiles = q.num_tiles;
+        q.n0[q.n_chunks] = n0;
+        int seg_lo = 0;
+        for (int s = 0; s < n_o; ++s) {  // output segments covered by [n0, n0 + nc)
+            const int seg_hi = seg_lo + o_width[s];
+            const int a = n0 > seg_lo ? n0 : seg_lo, b = (n0 + nc) < seg_hi ? (n0 + nc) : seg_hi;
+            if (a < b) {
+                TcSeg& o = pc.o[pc.n_o++];
+                o.ptr = reinterpret_cast<float*>(o_ptr[s]) + (a - seg_lo);
+                o.ld = o_ld[s];
+                o.width = b - a;
+            }
+            seg_lo = seg_hi;
+        }
+    }
+    q.w_half = w_half;
+    q.W = W_packed;
+    q.vec = reinterpret_cast<const float*>(vec); q.ctr = ctr; q.nbr = nbr; q.types = types;
+    q.rmax_table = reinterpret_cast<const float*>(rmax_table); q.bw = reinterpret_cast<const float*>(bessel_w);
+    q.PQ = reinterpret_cast<const float*>(PQ); q.num_types = num_types; q.p = (float)p_cut;
+
+    const unsigned grid = (unsigned)((q.num_tiles < num_sms) ? q.num_tiles : num_sms);
+    cudaStream_t st = (cudaStream_t)stream;
+    auto go = [&](auto kern) -> int {
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+            cudaGetLastError();
+            return AB2_NOT_ELIGIBLE;
+        }
+        kern<<<grid, NTHREADS, smem, st>>>(q);
+        AB2_CUDA_LAUNCH_CHECK();
+        return 0;
+    };
+    return tc_with_nl(nonlin, [&](auto nl) -> int {
+        constexpr int NL = decltype(nl)::value;
+        return H == 32 ? go(radial_embed_fwd_kernel<1, NL>) : go(radial_embed_fwd_kernel<2, NL>);
     });
 }
 

@@ -145,7 +145,7 @@ def edge_energy_grad_tangent(core, up, csr: EdgeCSR, vec: torch.Tensor, vdot: to
     # ---- (a) primal forward (stored-V path) ---------------------------------------------------------------------
     _lib.set_tag("hvp.fwd")
     box = []
-    _, _, _, sv = core.forward(csr, vec, None, fill_embed=lambda w0, x0, om0: box.append(up.forward(vec, csr, types_i32, [w0, x0, om0])),
+    _, _, _, sv = core.forward(csr, vec, None, fill_embed=lambda w0, x0, om0: box.append(up.forward(vec, csr, types_i32, [w0, x0, om0], keep_h=True)),
                                stored_v=True)
     kind, sp_saved, up_pre = box[0]
     k0_up = 1 if kind == "pq_fold" else 0

@@ -286,6 +286,8 @@ class UpstreamPack:
         self.dtype = dtype
         # route of the last pq_fold backward: "fused" (ab2_radial_pq_bwd_gemm) or "two_launch" (hidden_grad + radial_pq_bwd)
         self.bwd_path: Optional[str] = None
+        # route of the last pq_fold forward: "fused" (ab2_radial_embed_fwd) or "two_launch" (radial_pq_fwd + linear)
+        self.fwd_path: Optional[str] = None
         self.S_rc = radial.out_dim
         self.kind = "spline" if hasattr(radial, "spline") else "bessel"
         if self.kind == "spline":
@@ -328,9 +330,11 @@ class UpstreamPack:
                 self.fold_radial = False
 
     # ---- forward / adjoint of the whole upstream scalar track -----------------------------------------------
-    def forward(self, vec, csr: EdgeCSR, types_i32, outs):
+    def forward(self, vec, csr: EdgeCSR, types_i32, outs, keep_h: bool = False):
         """vec [E,3] -> the scalar-embed MLP's outputs, with the embed linears folded in, written into ``outs``
-        ([w0, x_0, omega_0]).  Returns what ``backward`` needs."""
+        ([w0, x_0, omega_0]).  Returns what ``backward`` needs.  With the first layer folded into PQ, the hidden
+        pre-activation h is stored only if ``keep_h``: the fused forward does not form it, and saves a meta tensor of its
+        shape in its place (``backward`` recomputes h where it needs it)."""
         dt = self.dtype
         if self.kind == "spline":
             from ._spline import spline_forward
@@ -340,6 +344,14 @@ class UpstreamPack:
                                           self.sp_w, self.num_types, dt)
             return ("spline", sp_saved, self.mlp.forward([e0], outs))
         if self.fold_radial:
+            # One kernel where it takes the case: the radial basis and h formed in the GEMM's producers, all output columns
+            # from one on-chip tile; bitwise the two launches below, which run where the entry declines.
+            if not keep_h and self.mlp.Wp[1] is not None and _lib.radial_embed_fwd(
+                    dt, self.S_pq, self.p, vec, csr.ctr, csr.nbr, types_i32, self.rmax_table, self.bessel_w, self.PQ, self.mlp.Wp[1], outs,
+                    **self.mlp.nl_kw):
+                self.fwd_path = "fused"
+                return ("pq_fold", None, [torch.empty(vec.shape[0], self.S_pq, dtype=dt, device="meta")])
+            self.fwd_path = "two_launch"
             h = _lib.radial_pq_fwd(dt, self.S_pq, self.p, vec, csr.ctr, csr.nbr, types_i32, self.rmax_table, self.bessel_w, self.PQ)
             _lib.linear([h], self.mlp.W[1], outs, act=_lib.ACT_SILU, W_packed=self.mlp.Wp[1], **self.mlp.nl_kw)
             return ("pq_fold", None, [h])
@@ -364,8 +376,11 @@ class UpstreamPack:
                 self.bwd_path = "fused"
                 return
             self.bwd_path = "two_launch"
+            h = pre[0]
+            if h.is_meta:  # the fused forward did not store h
+                h = _lib.radial_pq_fwd(dt, self.S_pq, self.p, vec, csr.ctr, csr.nbr, types_i32, self.rmax_table, self.bessel_w, self.PQ)
             g_h = self.mlp.hidden_grad(gouts)  # gradient w.r.t. phi(h); phi'(h) is applied by the radial adjoint (aux = h)
-            _lib.radial_pq_bwd(dt, self.S_pq, self.p, vec, csr.ctr, csr.nbr, types_i32, self.rmax_table, self.bessel_w, self.PQ, g_h, pre[0], gvec,
+            _lib.radial_pq_bwd(dt, self.S_pq, self.p, vec, csr.ctr, csr.nbr, types_i32, self.rmax_table, self.bessel_w, self.PQ, g_h, h, gvec,
                                **self.mlp.nl_kw)
             return
         g_e0 = torch.empty(E, self.S_rc, dtype=dt, device=vec.device)

@@ -612,6 +612,21 @@ int ab2_radial_pq_bwd_gemm(int dtype, int64_t M, int K, int H, int n_a, const vo
                            double p_cut, const void* vec, const int32_t* ctr, const int32_t* nbr, const int32_t* types,
                            const void* rmax_table, int num_types, const void* bessel_w, const void* PQ, void* gvec,
                            void* stream, int nonlin);
+/* The forward of the same folded embedding in one tensor-core kernel: with h = the ab2_radial_pq_fwd output [M][H] and
+ * W_packed the packed image (ab2_linear_pack) of the folded last layer W [H][N],
+ *   Out = phi(h) @ W,   Out = [O_0 | O_1 | ...] [M][N] (output segments as in ab2_linear, written, not accumulated)
+ * which is ab2_radial_pq_fwd followed by ab2_linear_nl(act = AB2_ACT_SILU), without h in memory and with one pass over
+ * the rows for all N columns.  h, its bf16 split and every output column are formed in the arithmetic of those two calls:
+ * the result is bitwise theirs.
+ * Returns AB2_NOT_ELIGIBLE (nothing enqueued, no error set) for dtype other than AB2_F32, num_bessels other than 8, H
+ * other than 32 or 64, N above 256, output segments not multiples of 32 columns or not 16-byte aligned, PQ (T^2 8 H
+ * floats) beyond the shared memory left next to W and the A tiles, M >= 2^31, or the linear_tc / linear_tma options
+ * off.  The caller then makes the two calls.  Returns 1 (and sets ab2_last_error) for an unknown nonlin. */
+int ab2_radial_embed_fwd(int dtype, int64_t M, int H, int N, const void* W_packed, int num_bessels, double p_cut,
+                         const void* vec, const int32_t* ctr, const int32_t* nbr, const int32_t* types,
+                         const void* rmax_table, int num_types, const void* bessel_w, const void* PQ, int n_o,
+                         void* const* o_ptr_host, const int64_t* o_ld_host, const int32_t* o_width_host, void* stream,
+                         int nonlin);
 
 /* ZBL pair term (reference call site allegro/model/allegro_models.py:270-288; the module is nequip's
  * nequip.nn.pair_potential.ZBL = LAMMPS pair_style zbl, constants of pair_zbl_const.h):
